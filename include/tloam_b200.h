@@ -325,11 +325,11 @@ int tloam_b200_pca_info(tloam_b200_handle* h, const tloam_feature_config* cfg, c
 /* ------------------------------------------------------------------------------------------------
  * "Next" row (f)-4, first part: multi-region ground extraction of the segmentation nodelet on the device.  Replaces
  * Segmentation::groundRemove (ref: src/models/segmentation/segmentation.cpp:738-770) with everything it calls:
- * initSections / getSection (:174-238), estimateRingsAndTimes2 HDL_64E (:341-384), filterByHeight (:454-470),
+ * initSections / getSection (:174-238), estimateRingsAndTimes2 HDL_64E / VLP_16 (:341-443), filterByHeight (:454-470),
  * fillSectionIndex (:507-541), segmentGroundThread (:626-730), findBestPlane (:551-616).  Bit-exact against
  * oracle/segmentation_oracle.cpp.  The handle is only used for its device, stream and scratch memory. */
 typedef struct tloam_ground_config {   /* ref: config/mapping/segmentation.yaml (velodyne: / groundSeg:) */
-  int sensor_model;                    /* 64: HDL-64E, the only branch built */
+  int sensor_model;                    /* 64: HDL-64E or 16: VLP-16 (verticalRes 2.0, initAngle -15.0); others: INVALID_ARG */
   double sensor_height;                /* 1.73 */
   double vertical_res, init_angle;     /* 0.4, -24.9 */
   double sensor_min_range, sensor_max_range;   /* 1.0, 120.0 */
@@ -342,11 +342,18 @@ void tloam_b200_ground_default_config(tloam_ground_config* c);
  * ground_index / object_index receive the indices (into xyz) of the points the reference's ground_scan / object_scan
  * receive, in that order with regions taken in (quadrant, section) order (the reference appends regions from four
  * racing threads); points of a region with <= 3 seeds reach neither list, as in the reference.  Optional outputs:
- * beam (n): the beam estimate stored in the intensity channel; region (n): quadrant * num_sec + section, 12 = above the
- * height threshold, 13 = dropped; height_threshold: mean z + 0.5; planes: 12 x 8 x 4 plane models [region][iteration]. */
+ * beam (n): (int) of the value stored in the intensity channel (HDL-64E: the beam estimate; VLP-16: beamId + correctTime,
+ * see tloam_b200_ground_remove); region (n): quadrant * num_sec + section, 12 = above the height threshold, 13 = dropped;
+ * height_threshold: mean z + 0.5; planes: 12 x 8 x 4 plane models [region][iteration]. */
 int tloam_b200_ground_extract(tloam_b200_handle* h, const tloam_ground_config* cfg, const double* xyz, size_t n,
                               size_t* ground_index, size_t* n_ground, size_t* object_index, size_t* n_object, int* beam,
                               int* region, double* height_threshold, double* planes);
+/* tloam_b200_ground_extract with the intensity channel as the reference computes it, in FP64 (optional, n values):
+ * HDL-64E the beam estimate (an integer), VLP-16 beamId + correctTime (a real number; within a few ulp of libm's, the sign
+ * tests of the half pass are exact).  Index lists, regions, threshold and planes are bit-exact for both sensors. */
+int tloam_b200_ground_remove(tloam_b200_handle* h, const tloam_ground_config* cfg, const double* xyz, size_t n,
+                             size_t* ground_index, size_t* n_ground, size_t* object_index, size_t* n_object, double* intensity,
+                             int* region, double* height_threshold, double* planes);
 
 /* ---- "next" row (f)-4, second part: LOAM-style edge extraction of the segmentation nodelet,
  * Segmentation::extractEdgePoint + extractFromSection (ref: src/models/segmentation/segmentation.cpp:1144-1304, called at
@@ -396,6 +403,16 @@ int tloam_b200_object_segmentation(tloam_b200_handle* h, const tloam_dcvc_config
 int tloam_b200_segment_scan(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg, int ring_min_num,
                             const double* xyz, size_t n, size_t* ground_index, size_t* n_ground, size_t* edge_index, size_t* n_edge,
                             size_t* general_index, size_t* n_general, int* n_clusters, int* sizes, double* boxes, int* beam);
+/* Segmentation::spinOnce's compute steps :48-66 in one call: RemoveClosedNonFinitePoints(near_dis) on the device (a point
+ * is kept iff it has no NaN / Inf coordinate and its norm is >= near_dis * near_dis -- a norm against a SQUARED
+ * threshold, as in the reference: near_dis 3.0 removes every point closer than 9 m), then the chain of
+ * tloam_b200_segment_scan on the surviving points.  xyz: the raw scan as the driver delivers it (HOST, n x 3 FP64, may
+ * hold NaN / Inf rows).  All lists index the RAW scan.  intensity (optional, n values): the FP64 channel of every
+ * surviving point (see tloam_b200_ground_remove), NaN for removed points.  One upload, one download. */
+int tloam_b200_segment_raw_scan(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg, int ring_min_num,
+                                double near_dis, const double* xyz, size_t n, size_t* ground_index, size_t* n_ground, size_t* edge_index,
+                                size_t* n_edge, size_t* general_index, size_t* n_general, int* n_clusters, int* sizes, double* boxes,
+                                double* intensity);
 
 /* Pinned host memory helpers (optional; pinned inputs make set_* a direct DMA, no staging threads). */
 int tloam_b200_host_alloc(void** p, size_t bytes);

@@ -58,34 +58,35 @@ class GroundExtractB200 {
 
   // ref: segmentation.cpp:738-770.  current_scan: the scan after RemoveClosedNonFinitePoints (:472-505).  On return
   // ground_scan / object_scan have received (+=, like the reference) the ground / non-ground points; the ground
-  // intensities are the fractional part of the beam estimate (0 for the HDL-64E branch, :692-695), the object
-  // intensities the beam estimate (:707-709); current_scan keeps the points at or below the height threshold with the
-  // beam estimate as intensity (filterByHeight, :454-470).
+  // intensities are the fractional part of the channel (0 for the HDL-64E branch, :692-695), the object intensities the
+  // channel (:707-709); current_scan keeps the points at or below the height threshold with the channel as intensity
+  // (filterByHeight, :454-470).  The channel: HDL-64E the beam estimate, VLP-16 beamId + correctTime (:386-429).
   bool groundRemove(CloudData& current_scan, CloudData& ground_scan, CloudData& object_scan) {
     const auto pts = current_scan.cloud_ptr->points_;          // copy: current_scan is rewritten below
     const size_t n = pts.size();
-    gi_.resize(n); oi_.resize(n); beam_.resize(n); region_.resize(n);
+    gi_.resize(n); oi_.resize(n); intensity_.resize(n); region_.resize(n);
     size_t ng = 0, no = 0;
-    last_status_ = tloam_b200_ground_extract(h_, &cfg_, n ? reinterpret_cast<const double*>(pts.data()) : nullptr, n, gi_.data(), &ng,
-                                             oi_.data(), &no, beam_.data(), region_.data(), &height_threshold_, nullptr);
+    last_status_ = tloam_b200_ground_remove(h_, &cfg_, n ? reinterpret_cast<const double*>(pts.data()) : nullptr, n, gi_.data(), &ng,
+                                            oi_.data(), &no, intensity_.data(), region_.data(), &height_threshold_, nullptr);
     if (last_status_ != TLOAM_B200_OK) {
       std::fprintf(stderr, "[tloam_b200] groundRemove: %s %s\n", tloam_b200_status_string(last_status_), tloam_b200_last_error(h_));
       return false;
     }
     for (size_t k = 0; k < ng; ++k) {
+      const double c = intensity_[gi_[k]];
       ground_scan.cloud_ptr->points_.push_back(pts[gi_[k]]);
-      ground_scan.cloud_ptr->intensity_.push_back(0.0);
+      ground_scan.cloud_ptr->intensity_.push_back(c - static_cast<int>(c));
     }
     for (size_t k = 0; k < no; ++k) {
       object_scan.cloud_ptr->points_.push_back(pts[oi_[k]]);
-      object_scan.cloud_ptr->intensity_.push_back(static_cast<double>(beam_[oi_[k]]));
+      object_scan.cloud_ptr->intensity_.push_back(intensity_[oi_[k]]);
     }
     current_scan.cloud_ptr->points_.clear();
     current_scan.cloud_ptr->intensity_.clear();
     for (size_t i = 0; i < n; ++i)
       if (region_[i] != 12) {                                   // 12 = above the height threshold (moved to non_ground_scan)
         current_scan.cloud_ptr->points_.push_back(pts[i]);
-        current_scan.cloud_ptr->intensity_.push_back(static_cast<double>(beam_[i]));
+        current_scan.cloud_ptr->intensity_.push_back(intensity_[i]);
       }
     return true;
   }
@@ -110,7 +111,8 @@ class GroundExtractB200 {
   int last_status_ = TLOAM_B200_OK;
   double height_threshold_ = 0.0;
   std::vector<size_t> gi_, oi_;
-  std::vector<int> beam_, region_;
+  std::vector<double> intensity_;
+  std::vector<int> region_;
 };
 
 }  // namespace tloam

@@ -46,6 +46,7 @@ class SegmentationB200 {
     dcvc_.sensor_max_range = config_node["velodyne"]["sensorMaxRange"].as<double>();
     dcvc_.min_polar_init = dcvc_.max_polar_init = 5.0;        // the members' initial values (segmentation.hpp:332-333), first frame only
     sensor_model_ = config_node["velodyne"]["sensorModel"].as<int>();
+    near_dis_ = config_node["velodyne"]["near_dis"].as<double>();
     ring_min_num_ = config_node["groundSeg"]["ringMinNum"].as<int>();
     h_ = ground_.handle();
   }
@@ -112,32 +113,53 @@ class SegmentationB200 {
     return true;
   }
 
-  // The three steps above as ONE device pass (tloam_b200_segment_scan): the scan crosses PCIe once.  ground_scan / edge_scan /
-  // general_scan receive the points the three separate calls would have produced (same order, same intensities: 0 for
-  // ground points, the beam estimate for the others); `scan` is left untouched.
+  // The three steps above as ONE device pass: the scan crosses PCIe once.  ground_scan / edge_scan / general_scan receive
+  // the points the three separate calls would have produced (same order, same intensities: the fractional part of the
+  // channel for ground points, the channel for the others); `scan` (finite points) is left untouched.
   bool segmentScan(const CloudData& scan, CloudData& ground_scan, CloudData& edge_scan, CloudData& general_scan,
                    std::vector<BoxB200>* boxes = nullptr) {
+    return chain(scan, 0.0, ground_scan, edge_scan, general_scan, boxes);   // near_dis 0 keeps every finite point
+  }
+
+  // Segmentation::spinOnce's compute steps (:48-66) in one device pass: RemoveClosedNonFinitePoints(near_dis) -- every
+  // point without NaN / Inf and with a norm >= near_dis * near_dis survives, as in the reference -- then segmentScan.
+  // raw_scan: the scan as the driver delivers it; it is left untouched (the reference compacts current_scan in place).
+  bool segmentRawScan(const CloudData& raw_scan, CloudData& ground_scan, CloudData& edge_scan, CloudData& general_scan,
+                      std::vector<BoxB200>* boxes = nullptr) {
+    return chain(raw_scan, near_dis_, ground_scan, edge_scan, general_scan, boxes);
+  }
+
+  double nearDis() const { return near_dis_; }
+  void setNearDis(double d) { near_dis_ = d; }
+  int lastStatus() const { return last_status_; }
+  tloam_b200_handle* handle() const { return h_; }
+
+ private:
+  bool chain(const CloudData& scan, double near_dis, CloudData& ground_scan, CloudData& edge_scan, CloudData& general_scan,
+             std::vector<BoxB200>* boxes) {
     const auto& pts = scan.cloud_ptr->points_;
     const size_t n = pts.size();
     if (n == 0) return false;
-    seg_.resize(n); edge_.resize(n); non_.resize(n); sizes_.resize(n); boxes_.resize(6 * n); beam_.resize(n);
+    seg_.resize(n); edge_.resize(n); non_.resize(n); sizes_.resize(n); boxes_.resize(6 * n); intensity_.resize(n);
     size_t ng = 0, ne = 0, nn = 0;
     int nc = 0;
-    last_status_ = tloam_b200_segment_scan(h_, &ground_.config(), &dcvc_, ring_min_num_, reinterpret_cast<const double*>(pts.data()), n, seg_.data(),
-                                           &ng, edge_.data(), &ne, non_.data(), &nn, &nc, sizes_.data(), boxes_.data(), beam_.data());
+    last_status_ = tloam_b200_segment_raw_scan(h_, &ground_.config(), &dcvc_, ring_min_num_, near_dis, reinterpret_cast<const double*>(pts.data()),
+                                               n, seg_.data(), &ng, edge_.data(), &ne, non_.data(), &nn, &nc, sizes_.data(), boxes_.data(),
+                                               intensity_.data());
     if (last_status_ != TLOAM_B200_OK) {
       std::fprintf(stderr, "[tloam_b200] segmentScan: %s %s\n", tloam_b200_status_string(last_status_), tloam_b200_last_error(h_));
       return false;
     }
-    auto append = [&](CloudData& out, const std::vector<size_t>& idx, size_t cnt, bool with_beam) {
+    auto append = [&](CloudData& out, const std::vector<size_t>& idx, size_t cnt, bool ground) {
       for (size_t k = 0; k < cnt; ++k) {
+        const double c = intensity_[idx[k]];
         out.cloud_ptr->points_.push_back(pts[idx[k]]);
-        out.cloud_ptr->intensity_.push_back(with_beam ? static_cast<double>(beam_[idx[k]]) : 0.0);
+        out.cloud_ptr->intensity_.push_back(ground ? c - static_cast<int>(c) : c);   // ground: :692-693
       }
     };
-    append(ground_scan, seg_, ng, false);
-    append(edge_scan, edge_, ne, true);
-    append(general_scan, non_, nn, true);
+    append(ground_scan, seg_, ng, true);
+    append(edge_scan, edge_, ne, false);
+    append(general_scan, non_, nn, false);
     if (boxes)
       for (int c = 0; c < nc; ++c) {
         BoxB200 b;
@@ -150,18 +172,15 @@ class SegmentationB200 {
     return true;
   }
 
-  int lastStatus() const { return last_status_; }
-  tloam_b200_handle* handle() const { return h_; }
-
- private:
   GroundExtractB200 ground_;
   tloam_dcvc_config dcvc_;
   int sensor_model_ = 64, ring_min_num_ = 131;
+  double near_dis_ = 3.0;                                      // velodyne.near_dis (config/mapping/segmentation.yaml)
   tloam_b200_handle* h_ = nullptr;
   int last_status_ = TLOAM_B200_OK;
   std::vector<size_t> seg_, edge_, non_;
-  std::vector<int> sizes_, beam_;
-  std::vector<double> boxes_;
+  std::vector<int> sizes_;
+  std::vector<double> boxes_, intensity_;
 };
 
 }  // namespace tloam

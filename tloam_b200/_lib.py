@@ -117,7 +117,7 @@ EXPORTS = [
     "tloam_b200_batch_set_profiling", "tloam_b200_batch_get_profile",
     "tloam_b200_submap_update_chained", "tloam_b200_set_frame_fitness", "tloam_b200_get_frame_fitness",
     "tloam_b200_set_async_inputs", "tloam_b200_wait_stream", "tloam_b200_dense_check_counters",
-    "tloam_b200_ground_default_config", "tloam_b200_ground_extract", "tloam_b200_extract_edge", "tloam_b200_dcvc_default_config", "tloam_b200_object_segmentation", "tloam_b200_segment_scan", "tloam_b200_map_layout_bytes",
+    "tloam_b200_ground_default_config", "tloam_b200_ground_extract", "tloam_b200_extract_edge", "tloam_b200_dcvc_default_config", "tloam_b200_object_segmentation", "tloam_b200_segment_scan", "tloam_b200_ground_remove", "tloam_b200_segment_raw_scan", "tloam_b200_map_layout_bytes",
     "tloam_b200_map_send_buffer", "tloam_b200_map_recv_buffer", "tloam_b200_map_adopt", "tloam_b200_signal_stream",
 ]
 
@@ -224,12 +224,15 @@ def load():
     L.tloam_b200_ground_default_config.argtypes = [C.POINTER(GroundConfig)]
     L.tloam_b200_ground_default_config.restype = None
     L.tloam_b200_ground_extract.argtypes = [vp, C.POINTER(GroundConfig), dp, C.c_size_t, szp, szp, szp, szp, ip, ip, dp, dp]
+    L.tloam_b200_ground_remove.argtypes = [vp, C.POINTER(GroundConfig), dp, C.c_size_t, szp, szp, szp, szp, dp, ip, dp, dp]
     L.tloam_b200_extract_edge.argtypes = [vp, C.c_int, C.c_int, dp, dp, C.c_size_t, szp, szp, szp, szp]
     L.tloam_b200_dcvc_default_config.argtypes = [C.POINTER(DcvcConfig)]
     L.tloam_b200_dcvc_default_config.restype = None
     L.tloam_b200_object_segmentation.argtypes = [vp, C.POINTER(DcvcConfig), dp, C.c_size_t, szp, szp, ip, ip, dp, ip, ip, ip, dp]
     L.tloam_b200_segment_scan.argtypes = [vp, C.POINTER(GroundConfig), C.POINTER(DcvcConfig), C.c_int, dp, C.c_size_t, szp, szp, szp, szp, szp, szp,
                                           ip, ip, dp, ip]
+    L.tloam_b200_segment_raw_scan.argtypes = [vp, C.POINTER(GroundConfig), C.POINTER(DcvcConfig), C.c_int, C.c_double, dp, C.c_size_t, szp, szp,
+                                              szp, szp, szp, szp, ip, ip, dp, dp]
     L.tloam_b200_batch_get_profile.argtypes = [vp, C.POINTER(Profile)]
     _lib = L
     return L

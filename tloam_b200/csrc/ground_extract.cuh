@@ -1,13 +1,16 @@
 // ground_extract.cuh -- "next" row (f)-4, first part: multi-region ground extraction of the segmentation nodelet on the
 // device.  Replaces Segmentation::groundRemove (ref: src/models/segmentation/segmentation.cpp:738-770) and what it calls:
-// estimateRingsAndTimes2 / HDL_64E (:341-384), filterByHeight (:454-470), fillSectionIndex with cv::fastAtan2
-// (:507-541), getSection (:230-238), segmentGroundThread (:626-730), findBestPlane (:551-616).
+// estimateRingsAndTimes2 / HDL_64E (:341-384) and VLP_16 (:386-429), filterByHeight (:454-470), fillSectionIndex with
+// cv::fastAtan2 (:507-541), getSection (:230-238), segmentGroundThread (:626-730), findBestPlane (:551-616); and, for the
+// raw-scan chain, RemoveClosedNonFinitePoints (:472-499, k_rm_* at the end of this file).
 //
 // Pipeline (7 launches, no host round trip until the index lists are fetched):
-//   k_ge_pre      per 256-point chunk: quadrant 4 -> 1 transition flags (beam estimate), chunk sum of z
-//   k_ge_scan1    prefix of the transition counts over the chunks; mean height -> height threshold
-//   k_ge_region   per point: beam = min(prefix, 63), key = region (quadrant x section) | above-threshold | dropped;
-//                 per-chunk key histogram
+//   k_ge_pre      per 256-point chunk: quadrant 4 -> 1 transition count (HDL-64E) / first half-pass index (VLP-16),
+//                 chunk sum of z
+//   k_ge_scan1    prefix of the transition counts (HDL-64E) / first half pass, startOri, scanOri, halfOri (VLP-16);
+//                 mean height -> height threshold
+//   k_ge_region   per point: the intensity channel (HDL-64E: beam = min(prefix, 63); VLP-16: beamId + correctTime),
+//                 key = region (quadrant x section) | above-threshold | dropped; per-chunk key histogram
 //   k_ge_scan2    prefix of the histograms per key over the chunks (stable 14-way partition)
 //   k_ge_scatter  order[] = point ids grouped by key, index order inside a key (= the reference's regionIndex lists)
 //   k_ge_fit      one block per region: 20 lowest seeds of every 10th point, seed set, 3 x (findBestPlane + classify),
@@ -33,14 +36,18 @@ constexpr int kGeSeedCache = 4096;     // seed candidates whose height is cached
 struct GeArgs {
   const double* pts;                   // AoS xyz
   unsigned n, nchunk;
-  int sensor_model, num_sec, max_iter, seed_num;
+  int sensor_model, num_sec, max_iter, seed_num;   // sensor_model 64: HDL-64E branch, 16: VLP-16 branch
   double sensor_height, min_range, max_range, plane_dis;
+  double ang_bot, vertical_res;        // VLP-16 branch: |initAngle| + 0.1, verticalRes
   float bounds[4];
   int nbounds;
-  unsigned* chunk_trans;               // [nchunk] transitions in the chunk -> exclusive prefix
+  unsigned* chunk_trans;               // [nchunk] HDL-64E: transitions in the chunk -> exclusive prefix;
+                                       //          VLP-16: first half-pass index in the chunk (0xFFFFFFFF: none)
   double* chunk_sum;                   // [nchunk]
-  double* scal;                        // [0] height threshold
-  int* beam;                           // [n]
+  double* scal;                        // [0] height threshold; VLP-16: [1] startOri, [2] scanOri, [3] halfOri
+  unsigned* first_trans;               // VLP-16: first half-pass index of the scan (0xFFFFFFFF: none)
+  int* beam;                           // [n] (int) of the channel
+  double* intensity;                   // [n] the reference's intensity channel (FP64)
   unsigned char* key;                  // [n]
   unsigned* chunk_cnt;                 // [nchunk][kGeKeys] -> exclusive prefix per key
   unsigned* key_base;                  // [kGeKeys + 1]
@@ -95,13 +102,36 @@ __device__ __forceinline__ bool ge_transition(const GeArgs& a, unsigned i) {
   return q == 1 && pq == 4;
 }
 
+// Sign of atan2(y, x) without rounding: atan2(+-0, x < 0 or x = -0) = +-pi, atan2(+-0, +0 or x > 0) = +-0.
+__device__ __forceinline__ bool ge_ori_negative(double x, double y) {
+  return !isnan(x) && (y < 0.0 || (y == 0.0 && signbit(y) && signbit(x)));
+}
+__device__ __forceinline__ bool ge_ori_positive(double x, double y) {
+  return !isnan(x) && (y > 0.0 || (y == 0.0 && !signbit(y) && signbit(x)));
+}
+
+// VLP-16 branch (ref: :386-429): the half pass starts at the first i >= 1 with ori[i-1] < 0 < ori[i] (prevOri = 0.0 before
+// point 0; after the half pass prevOri = pi - ori >= 0, so the transition fires at most once)
+__device__ __forceinline__ bool ge_vlp_transition(const GeArgs& a, unsigned i) {
+  if (i == 0u || i >= a.n) return false;
+  return ge_ori_positive(a.pts[3ull * i], a.pts[3ull * i + 1]) && ge_ori_negative(a.pts[3ull * (i - 1)], a.pts[3ull * (i - 1) + 1]);
+}
+
 __global__ void __launch_bounds__(kGeChunk) k_ge_pre(const __grid_constant__ GeArgs a) {
   const unsigned i = blockIdx.x * kGeChunk + threadIdx.x;
+  const bool vlp = a.sensor_model == 16;
   __shared__ double s_z[kGeChunk];
+  __shared__ unsigned s_first;
+  if (threadIdx.x == 0) s_first = 0xFFFFFFFFu;
   s_z[threadIdx.x] = i < a.n ? a.pts[3ull * i + 2] : 0.0;
-  const int cnt = __syncthreads_count(ge_transition(a, i));
+  const bool tr = vlp ? ge_vlp_transition(a, i) : ge_transition(a, i);
+  const int cnt = __syncthreads_count(tr);                                 // also orders s_first's initialisation
+  if (vlp) {
+    if (tr) atomicMin(&s_first, i);
+    __syncthreads();
+  }
   if (threadIdx.x == 0) {
-    a.chunk_trans[blockIdx.x] = (unsigned)cnt;
+    a.chunk_trans[blockIdx.x] = vlp ? s_first : (unsigned)cnt;
     const unsigned m = min((unsigned)kGeChunk, a.n - blockIdx.x * kGeChunk);
     double s = 0.0;
     for (unsigned k = 0; k < m; ++k) s = ge_add(s, s_z[k]);            // chunk sum in index order (see the oracle)
@@ -135,12 +165,43 @@ __device__ __forceinline__ void ge_block_exclusive_scan(unsigned* v, unsigned n,
 }
 
 __global__ void __launch_bounds__(1024) k_ge_scan1(const __grid_constant__ GeArgs a) {
-  ge_block_exclusive_scan(a.chunk_trans, a.nchunk, 1u, nullptr);
+  const bool vlp = a.sensor_model == 16;
+  if (!vlp) ge_block_exclusive_scan(a.chunk_trans, a.nchunk, 1u, nullptr);
   if (threadIdx.x == 0) {
     double total = 0.0;
-    for (unsigned c = 0; c < a.nchunk; ++c) total = ge_add(total, a.chunk_sum[c]);
+    unsigned first = 0xFFFFFFFFu;
+    for (unsigned c = 0; c < a.nchunk; ++c) {
+      total = ge_add(total, a.chunk_sum[c]);
+      if (vlp) first = min(first, a.chunk_trans[c]);
+    }
     a.scal[0] = ge_add(__ddiv_rn(total, (double)a.n), 0.5);              // mean height + 0.5, ref: :743
+    if (vlp) {                                                             // ref: :391-400, :413-416
+      const double* p = a.pts;
+      const double start = atan2(p[1], p[0]);
+      double end = atan2(p[3ull * (a.n - 1) + 1], p[3ull * (a.n - 1)]);
+      if (ge_sub(end, start) > 3 * M_PI) end = ge_sub(end, 2 * M_PI);
+      else if (ge_sub(end, start) < M_PI) end = ge_add(end, 2 * M_PI);
+      a.scal[1] = start;
+      a.scal[2] = ge_sub(end, start);
+      a.scal[3] = first != 0xFFFFFFFFu ? fabs(ge_sub(atan2(p[3ull * (first - 1) + 1], p[3ull * (first - 1)]), start)) : 0.0;
+      *a.first_trans = first;
+    }
   }
+}
+
+// the VLP-16 channel of point i (ref: :404-425): beamId + correctTime, in the reference's operation order
+__device__ __forceinline__ double ge_vlp_channel(const GeArgs& a, unsigned i, double x, double y, double z) {
+  const double pitch = __ddiv_rn(ge_mul(atan2(z, __dsqrt_rn(ge_add(ge_mul(x, x), ge_mul(y, y)))), 180.0), M_PI);
+  const double beam_id = __ddiv_rn((double)(int)ge_add(pitch, a.ang_bot), a.vertical_res);
+  const double ori = atan2(y, x);
+  double t;
+  if (i >= *a.first_trans) {
+    t = __ddiv_rn(ge_add(ge_sub(M_PI, ori), a.scal[3]), a.scal[2]);
+    if (t > 1.0) t = 0.99999;
+  } else {
+    t = __ddiv_rn(fabs(ge_sub(ori, a.scal[1])), a.scal[2]);
+  }
+  return ge_add(beam_id, t);
 }
 
 __device__ __forceinline__ int ge_section(const GeArgs& a, double radius) {   // getSection, ref: :230-238 (see the oracle)
@@ -189,8 +250,9 @@ __global__ void __launch_bounds__(kGeChunk) k_ge_region(const __grid_constant__ 
   const unsigned i = blockIdx.x * kGeChunk + threadIdx.x;
   __shared__ unsigned s_cnt[kGeChunk / 32][kGeKeys];
   __shared__ unsigned s_w[kGeChunk / 32];
-  // beam = transitions up to and including this point, saturating (ref: :367-374)
-  const bool tr = ge_transition(a, i);
+  // HDL-64E: beam = transitions up to and including this point, saturating (ref: :367-374)
+  const bool vlp = a.sensor_model == 16;
+  const bool tr = !vlp && ge_transition(a, i);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const unsigned b = __ballot_sync(0xffffffffu, tr);
   if (lane == 0) s_w[warp] = __popc(b);
@@ -199,8 +261,15 @@ __global__ void __launch_bounds__(kGeChunk) k_ge_region(const __grid_constant__ 
   for (int w = 0; w < warp; ++w) pre += s_w[w];
   int key = -1;
   if (i < a.n) {
-    const int bm = (int)pre < a.sensor_model - 1 ? (int)pre : a.sensor_model - 1;
-    a.beam[i] = bm;
+    if (vlp) {
+      const double c = ge_vlp_channel(a, i, a.pts[3ull * i], a.pts[3ull * i + 1], a.pts[3ull * i + 2]);
+      a.intensity[i] = c;
+      a.beam[i] = (int)c;
+    } else {
+      const int bm = (int)pre < a.sensor_model - 1 ? (int)pre : a.sensor_model - 1;
+      a.beam[i] = bm;
+      a.intensity[i] = (double)bm;
+    }
     key = ge_key_of(a, a.pts[3ull * i], a.pts[3ull * i + 1], a.pts[3ull * i + 2], a.scal[0]);
     a.key[i] = (unsigned char)key;
   }
@@ -482,6 +551,50 @@ __global__ void __launch_bounds__(256) k_ge_emit(const __grid_constant__ GeArgs 
     }
   }
   for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < cnt; i += gridDim.x * blockDim.x) dst[off + i] = src[i];
+}
+
+// ---- Segmentation::RemoveClosedNonFinitePoints (ref: :472-499) on the uploaded raw scan: a stable compaction that keeps
+// a point iff it has no NaN / Inf coordinate and pt.norm() >= dis_th * dis_th (a norm against a SQUARED threshold:
+// near_dis 3.0 removes every point closer than 9 m).  kept[] = the surviving points, map[k] = raw index of kept point k.
+struct RmArgs {
+  const double* raw;                   // AoS xyz
+  unsigned n, nchunk;
+  double norm_min;                     // dis_th * dis_th
+  unsigned* chunk_cnt;                 // [nchunk] kept points in the chunk -> exclusive prefix
+  unsigned* total;                     // [1]
+  double* kept;                        // [n] AoS xyz
+  unsigned* map;                       // [n]
+};
+
+__device__ __forceinline__ bool rm_keep(const RmArgs& a, unsigned i) {
+  if (i >= a.n) return false;
+  const double x = a.raw[3ull * i], y = a.raw[3ull * i + 1], z = a.raw[3ull * i + 2];
+  if (!isfinite(x) || !isfinite(y) || !isfinite(z)) return false;
+  return __dsqrt_rn(ge_add(ge_add(ge_mul(x, x), ge_mul(y, y)), ge_mul(z, z))) >= a.norm_min;   // Eigen norm(): (x^2 + y^2) + z^2
+}
+
+__global__ void __launch_bounds__(kGeChunk) k_rm_count(const __grid_constant__ RmArgs a) {
+  const int cnt = __syncthreads_count(rm_keep(a, blockIdx.x * kGeChunk + threadIdx.x));
+  if (threadIdx.x == 0) a.chunk_cnt[blockIdx.x] = (unsigned)cnt;
+}
+
+__global__ void __launch_bounds__(1024) k_rm_scan(const __grid_constant__ RmArgs a) {
+  ge_block_exclusive_scan(a.chunk_cnt, a.nchunk, 1u, a.total);
+}
+
+__global__ void __launch_bounds__(kGeChunk) k_rm_scatter(const __grid_constant__ RmArgs a) {
+  const unsigned i = blockIdx.x * kGeChunk + threadIdx.x;
+  __shared__ unsigned s_w[kGeChunk / 32];
+  const bool keep = rm_keep(a, i);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned b = __ballot_sync(0xffffffffu, keep);
+  if (lane == 0) s_w[warp] = __popc(b);
+  __syncthreads();
+  if (!keep) return;
+  unsigned k = a.chunk_cnt[blockIdx.x] + __popc(b & ((1u << lane) - 1u));
+  for (int w = 0; w < warp; ++w) k += s_w[w];
+  a.kept[3ull * k] = a.raw[3ull * i]; a.kept[3ull * k + 1] = a.raw[3ull * i + 1]; a.kept[3ull * k + 2] = a.raw[3ull * i + 2];
+  a.map[k] = i;
 }
 
 }  // namespace tloam

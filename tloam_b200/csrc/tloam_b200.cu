@@ -60,7 +60,8 @@ struct tloam_b200_handle {
   struct SegChain {
     bool active = false;
     const double* dev_xyz = nullptr; const double* dev_intensity = nullptr;
-    const unsigned* ground = nullptr; const unsigned* object = nullptr; const int* beam = nullptr; unsigned n_ground = 0, n_object = 0;
+    const unsigned* ground = nullptr; const unsigned* object = nullptr; const int* beam = nullptr; const double* intensity = nullptr;
+    unsigned n_ground = 0, n_object = 0;
     const unsigned long long* seg = nullptr; unsigned n_seg = 0;
     const unsigned long long* edge = nullptr; const unsigned long long* non_edge = nullptr; unsigned n_edge = 0, n_non = 0;
   } seg;
@@ -2297,14 +2298,15 @@ static int ground_section_bounds(const tloam_ground_config& c, float out[4]) {
   return nb;
 }
 
-int tloam_b200_ground_extract(tloam_b200_handle* h, const tloam_ground_config* cfg, const double* xyz, size_t n,
-                              size_t* ground_index, size_t* n_ground, size_t* object_index, size_t* n_object, int* beam,
-                              int* region, double* height_threshold, double* planes) {
+// groundRemove with both forms of the per-point channel: beam = (int)intensity, intensity = the reference's FP64 value
+static int ground_run(tloam_b200_handle* h, const tloam_ground_config* cfg, const double* xyz, size_t n, size_t* ground_index,
+                      size_t* n_ground, size_t* object_index, size_t* n_object, int* beam, double* intensity, int* region,
+                      double* height_threshold, double* planes) {
   if (!h || !cfg || !ground_index || !n_ground || !object_index || !n_object) return TLOAM_B200_ERR_INVALID_ARG;
   *n_ground = *n_object = 0;
-  if (cfg->sensor_model != 64 || cfg->quadrant != 4 || cfg->num_sec < 1 || cfg->num_sec > 3 || cfg->max_iter < 1 ||
-      cfg->max_iter > kGeMaxIter || cfg->ground_seed_num < 1)
-    return TLOAM_B200_ERR_INVALID_ARG;                            // only the HDL-64E branch is built (:439-441)
+  if ((cfg->sensor_model != 64 && cfg->sensor_model != 16) || cfg->quadrant != 4 || cfg->num_sec < 1 || cfg->num_sec > 3 ||
+      cfg->max_iter < 1 || cfg->max_iter > kGeMaxIter || cfg->ground_seed_num < 1)
+    return TLOAM_B200_ERR_INVALID_ARG;                            // the HDL-64E and VLP-16 branches (:433-442); others: `default:`
   if (planes) for (int i = 0; i < 12 * kGeMaxIter * 4; ++i) planes[i] = std::nan("");
   if (n == 0) { if (height_threshold) *height_threshold = 1.0; return TLOAM_B200_OK; }   // :335-338
   if (!xyz || n > ((size_t)1 << 30)) return TLOAM_B200_ERR_INVALID_ARG;
@@ -2315,13 +2317,14 @@ int tloam_b200_ground_extract(tloam_b200_handle* h, const tloam_ground_config* c
   a.sensor_model = cfg->sensor_model; a.num_sec = cfg->num_sec; a.max_iter = cfg->max_iter; a.seed_num = cfg->ground_seed_num;
   a.sensor_height = cfg->sensor_height; a.min_range = cfg->sensor_min_range; a.max_range = cfg->sensor_max_range;
   a.plane_dis = cfg->plane_dis;
-  a.nbounds = ground_section_bounds(*cfg, a.bounds);
+  a.ang_bot = std::fabs(cfg->init_angle) + 0.1; a.vertical_res = cfg->vertical_res;
+  a.nbounds = ground_section_bounds(*cfg, a.bounds);              // VLP-16 with the shipped values: ONE bound (see DESIGN.md §4d)
   size_t off = 0;
   auto take = [&](size_t bytes) { const size_t o = off; off += round_up(bytes, 256); return o; };
   const size_t o_pts = take(n * 24), o_ct = take(a.nchunk * 4), o_cs = take(a.nchunk * 8), o_sc = take(64), o_beam = take(n * 4),
                o_key = take(n), o_cc = take((size_t)a.nchunk * kGeKeys * 4), o_kb = take((kGeKeys + 1) * 4), o_ord = take(n * 4),
                o_flag = take(n), o_lists = take(2 * n * 4), o_rc = take(12 * 2 * 4), o_pl = take(12 * kGeMaxIter * 4 * 8),
-               o_og = take(n * 4), o_oo = take(n * 4), o_oc = take(64);
+               o_og = take(n * 4), o_oo = take(n * 4), o_oc = take(64), o_int = take(n * 8);
   if (off > h->cap_ge) {
     CU_TRY(cudaStreamSynchronize(h->stream));
     cudaFree(h->d_ge); h->d_ge = nullptr; h->cap_ge = 0;
@@ -2334,6 +2337,7 @@ int tloam_b200_ground_extract(tloam_b200_handle* h, const tloam_ground_config* c
   a.key_base = (unsigned*)(b + o_kb); a.order = (unsigned*)(b + o_ord); a.flag = b + o_flag; a.lists = (unsigned*)(b + o_lists);
   a.reg_cnt = (unsigned*)(b + o_rc); a.planes = (double*)(b + o_pl); a.out_ground = (unsigned*)(b + o_og);
   a.out_object = (unsigned*)(b + o_oo); a.out_counts = (unsigned*)(b + o_oc);
+  a.intensity = (double*)(b + o_int); a.first_trans = (unsigned*)(a.scal + 4);
   if (h->seg.active) a.pts = h->seg.dev_xyz;
   else CU_TRY(cudaMemcpyAsync(b + o_pts, xyz, n * 24, cudaMemcpyHostToDevice, h->stream));
   TL_LAUNCH(TLOAM_B200_K_GROUND, (k_ge_pre<<<a.nchunk, kGeChunk, 0, h->stream>>>(a)));
@@ -2357,7 +2361,7 @@ int tloam_b200_ground_extract(tloam_b200_handle* h, const tloam_ground_config* c
   memcpy(counts, h->h_result + 28, sizeof(counts));
   if (height_threshold) *height_threshold = h->h_result[29];
   if (h->seg.active) {                                                     // chained: the lists stay on the device
-    h->seg.ground = a.out_ground; h->seg.object = a.out_object; h->seg.beam = a.beam;
+    h->seg.ground = a.out_ground; h->seg.object = a.out_object; h->seg.beam = a.beam; h->seg.intensity = a.intensity;
     h->seg.n_ground = counts[0]; h->seg.n_object = counts[1];
     *n_ground = counts[0]; *n_object = counts[1];
     return TLOAM_B200_OK;
@@ -2366,6 +2370,7 @@ int tloam_b200_ground_extract(tloam_b200_handle* h, const tloam_ground_config* c
   if (counts[0]) CU_TRY(cudaMemcpyAsync(gi.data(), a.out_ground, counts[0] * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
   if (counts[1]) CU_TRY(cudaMemcpyAsync(oi.data(), a.out_object, counts[1] * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
   if (beam) CU_TRY(cudaMemcpyAsync(beam, a.beam, n * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  if (intensity) CU_TRY(cudaMemcpyAsync(intensity, a.intensity, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   std::vector<unsigned char> keys;
   if (region) { keys.resize(n); CU_TRY(cudaMemcpyAsync(keys.data(), a.key, n, cudaMemcpyDeviceToHost, h->stream)); }
   if (planes) CU_TRY(cudaMemcpyAsync(planes, a.planes, 12 * kGeMaxIter * 4 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
@@ -2375,6 +2380,18 @@ int tloam_b200_ground_extract(tloam_b200_handle* h, const tloam_ground_config* c
   if (region) for (size_t i = 0; i < n; ++i) region[i] = keys[i];
   *n_ground = counts[0]; *n_object = counts[1];
   return TLOAM_B200_OK;
+}
+
+int tloam_b200_ground_remove(tloam_b200_handle* h, const tloam_ground_config* cfg, const double* xyz, size_t n, size_t* ground_index,
+                             size_t* n_ground, size_t* object_index, size_t* n_object, double* intensity, int* region,
+                             double* height_threshold, double* planes) {
+  return ground_run(h, cfg, xyz, n, ground_index, n_ground, object_index, n_object, nullptr, intensity, region, height_threshold, planes);
+}
+
+int tloam_b200_ground_extract(tloam_b200_handle* h, const tloam_ground_config* cfg, const double* xyz, size_t n,
+                              size_t* ground_index, size_t* n_ground, size_t* object_index, size_t* n_object, int* beam,
+                              int* region, double* height_threshold, double* planes) {
+  return ground_run(h, cfg, xyz, n, ground_index, n_ground, object_index, n_object, beam, nullptr, region, height_threshold, planes);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -2586,13 +2603,13 @@ int tloam_b200_object_segmentation(tloam_b200_handle* h, const tloam_dcvc_config
 // final lists come home -- as indices into the ORIGINAL scan.
 // ---------------------------------------------------------------------------------------------
 namespace {
-__global__ void __launch_bounds__(256) k_chain_gather_object(const double* pts, const int* beam, const unsigned* idx, unsigned n, double* out_pts,
-                                                             double* out_beam) {
+__global__ void __launch_bounds__(256) k_chain_gather_object(const double* pts, const double* intensity, const unsigned* idx, unsigned n,
+                                                             double* out_pts, double* out_beam) {
   const unsigned j = blockIdx.x * 256 + threadIdx.x;
   if (j >= n) return;
   const unsigned i = idx[j];
   out_pts[3ull * j] = pts[3ull * i]; out_pts[3ull * j + 1] = pts[3ull * i + 1]; out_pts[3ull * j + 2] = pts[3ull * i + 2];
-  out_beam[j] = (double)beam[i];                                           // the intensity channel carries the beam id (:707-709)
+  out_beam[j] = intensity[i];                                              // the object points carry the channel (:707-709)
 }
 __global__ void __launch_bounds__(256) k_chain_gather_segmented(const double* obj_pts, const double* obj_beam, const unsigned* obj_idx,
                                                                 const unsigned long long* seg, unsigned n, double* out_pts, double* out_beam,
@@ -2604,32 +2621,44 @@ __global__ void __launch_bounds__(256) k_chain_gather_segmented(const double* ob
   out_beam[j] = obj_beam[i];
   out_orig[j] = obj_idx[i];
 }
-// blockIdx.y: 0 ground, 1 edge, 2 general -- index lists into the original scan, as 64-bit values
+// blockIdx.y: 0 ground, 1 edge, 2 general -- index lists into the original scan, as 64-bit values (raw_of: kept -> raw
+// index after the removal step, null = no removal step); 3: the channel of kept point j into slot raw_of[j] of out_intensity
 __global__ void __launch_bounds__(256) k_chain_final(const unsigned* ground, unsigned n_ground, const unsigned long long* edge, unsigned n_edge,
                                                      const unsigned long long* non_edge, unsigned n_non, const unsigned* seg_orig,
-                                                     unsigned long long* out_ground, unsigned long long* out_edge, unsigned long long* out_general) {
+                                                     const unsigned* raw_of, const double* intensity, unsigned n_kept,
+                                                     unsigned long long* out_ground, unsigned long long* out_edge, unsigned long long* out_general,
+                                                     double* out_intensity) {
   const unsigned j = blockIdx.x * 256 + threadIdx.x;
-  if (blockIdx.y == 0) { if (j < n_ground) out_ground[j] = ground[j]; }
-  else if (blockIdx.y == 1) { if (j < n_edge) out_edge[j] = seg_orig[(unsigned)edge[j]]; }
-  else { if (j < n_non) out_general[j] = seg_orig[(unsigned)non_edge[j]]; }
+  auto raw = [&](unsigned k) { return raw_of ? raw_of[k] : k; };
+  if (blockIdx.y == 0) { if (j < n_ground) out_ground[j] = raw(ground[j]); }
+  else if (blockIdx.y == 1) { if (j < n_edge) out_edge[j] = raw(seg_orig[(unsigned)edge[j]]); }
+  else if (blockIdx.y == 2) { if (j < n_non) out_general[j] = raw(seg_orig[(unsigned)non_edge[j]]); }
+  else { if (j < n_kept) out_intensity[raw(j)] = intensity[j]; }
 }
 }  // namespace
 
-int tloam_b200_segment_scan(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg, int ring_min_num,
-                            const double* xyz, size_t n, size_t* ground_index, size_t* n_ground, size_t* edge_index, size_t* n_edge,
-                            size_t* general_index, size_t* n_general, int* n_clusters, int* sizes, double* boxes, int* beam) {
+// The one implementation of the chained segmentation.  remove: run RemoveClosedNonFinitePoints(near_dis) on the device
+// first (tloam_b200_segment_raw_scan); tloam_b200_segment_scan runs without that step.  beam / intensity (optional, n
+// values): the channel of every point of the scan as int / FP64 (NaN for removed points).
+static int segment_chain(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg, int ring_min_num, bool remove,
+                         double near_dis, const double* xyz, size_t n, size_t* ground_index, size_t* n_ground, size_t* edge_index,
+                         size_t* n_edge, size_t* general_index, size_t* n_general, int* n_clusters, int* sizes, double* boxes, int* beam,
+                         double* intensity) {
   if (!h || !gcfg || !dcfg || !ground_index || !n_ground || !edge_index || !n_edge || !general_index || !n_general || !n_clusters)
     return TLOAM_B200_ERR_INVALID_ARG;
   *n_ground = *n_edge = *n_general = 0; *n_clusters = 0;
+  if (remove && gcfg->sensor_model != 64 && gcfg->sensor_model != 16) return TLOAM_B200_ERR_INVALID_ARG;
   if (n == 0) return TLOAM_B200_OK;
   if (!xyz || n > ((size_t)1 << 26)) return TLOAM_B200_ERR_INVALID_ARG;
   CU_TRY(cudaSetDevice(h->device));
   // chain buffer: what must outlive a stage's arena
+  const unsigned nchunk = (unsigned)((n + kGeChunk - 1) / kGeChunk);
   size_t off = 0;
   auto take = [&](size_t bytes) { const size_t o = off; off += round_up(bytes, 256); return o; };
   const size_t o_scan = take(n * 24), o_gnd = take(n * 4), o_oidx = take(n * 4), o_opts = take(n * 24), o_obeam = take(n * 8),
                o_spts = take(n * 24), o_sbeam = take(n * 8), o_sorig = take(n * 4), o_fg = take(n * 8), o_fe = take(n * 8), o_fn = take(n * 8),
-               o_beam = take(n * 4);
+               o_beam = take(n * 4), o_kept = remove ? take(n * 24) : 0, o_map = remove ? take(n * 4) : 0,
+               o_rmc = remove ? take(nchunk * 4 + 64) : 0, o_int = intensity ? take(n * 8) : 0, o_fi = intensity ? take(n * 8) : 0;
   if (off > h->cap_chain) {
     CU_TRY(cudaStreamSynchronize(h->stream));
     cudaFree(h->d_chain); h->d_chain = nullptr; h->cap_chain = 0;
@@ -2646,42 +2675,65 @@ int tloam_b200_segment_scan(tloam_b200_handle* h, const tloam_ground_config* gcf
   if (HostStage::pageable(xyz) && getenv("TLOAM_B200_NO_HOST_STAGE") == nullptr) CU_TRY(h->hstage.upload(d_scan, xyz, n * 24, h->stream));
   else CU_TRY(cudaMemcpyAsync(d_scan, xyz, n * 24, cudaMemcpyHostToDevice, h->stream));
   struct Reset { tloam_b200_handle* h; ~Reset() { h->seg = tloam_b200_handle::SegChain(); } } reset{h};
-  h->seg.active = true;
-  // ---- 1. groundRemove ----
-  h->seg.dev_xyz = d_scan;
-  size_t ng = 0, no = 0;
-  int rc = tloam_b200_ground_extract(h, gcfg, xyz, n, ground_index, &ng, general_index /*scratch: not written when chained*/, &no, nullptr, nullptr,
-                                     nullptr, nullptr);
-  if (rc != TLOAM_B200_OK) return rc;
-  if (ng) CU_TRY(cudaMemcpyAsync(d_gnd, h->seg.ground, ng * 4, cudaMemcpyDeviceToDevice, h->stream));
-  if (beam) CU_TRY(cudaMemcpyAsync(c + o_beam, h->seg.beam, n * 4, cudaMemcpyDeviceToDevice, h->stream));
-  if (no) {
-    CU_TRY(cudaMemcpyAsync(d_oidx, h->seg.object, no * 4, cudaMemcpyDeviceToDevice, h->stream));
-    k_chain_gather_object<<<(unsigned)((no + 255) / 256), 256, 0, h->stream>>>(d_scan, h->seg.beam, h->seg.object, (unsigned)no, d_opts, d_obeam);
+  // ---- 0. RemoveClosedNonFinitePoints (:48, :472-499): kept points + kept -> raw map ----
+  const double* pts = d_scan;
+  const unsigned* raw_of = nullptr;
+  size_t nk = n;
+  if (remove) {
+    RmArgs r;
+    r.raw = d_scan; r.n = (unsigned)n; r.nchunk = nchunk; r.norm_min = near_dis * near_dis;
+    r.chunk_cnt = (unsigned*)(c + o_rmc); r.total = r.chunk_cnt + round_up(nchunk, 16);
+    r.kept = (double*)(c + o_kept); r.map = (unsigned*)(c + o_map);
+    TL_LAUNCH(TLOAM_B200_K_GROUND, (k_rm_count<<<nchunk, kGeChunk, 0, h->stream>>>(r)));
+    TL_LAUNCH(TLOAM_B200_K_GROUND, (k_rm_scan<<<1, 1024, 0, h->stream>>>(r)));
+    TL_LAUNCH(TLOAM_B200_K_GROUND, (k_rm_scatter<<<nchunk, kGeChunk, 0, h->stream>>>(r)));
     CU_TRY(cudaGetLastError());
+    CU_TRY(cudaMemcpyAsync(h->h_result + 28, r.total, sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    unsigned kept;
+    memcpy(&kept, h->h_result + 28, sizeof(kept));
+    pts = r.kept; raw_of = r.map; nk = kept;
   }
-  size_t ne = 0, nn = 0;
-  if (no) {
-    // ---- 2. objectSegmentation ----
-    h->seg.dev_xyz = d_opts;
-    size_t ns = 0;
-    rc = tloam_b200_object_segmentation(h, dcfg, d_opts /*placeholder: read on the device*/, no, general_index, &ns, n_clusters, sizes, boxes, nullptr,
-                                        nullptr, nullptr, nullptr);
+  if (intensity) CU_TRY(cudaMemsetAsync(c + o_fi, 0xFF, n * 8, h->stream));   // all-ones: NaN for the removed points
+  size_t ng = 0, no = 0, ne = 0, nn = 0;
+  if (nk) {
+    h->seg.active = true;
+    // ---- 1. groundRemove ----
+    h->seg.dev_xyz = pts;
+    int rc = ground_run(h, gcfg, xyz, nk, ground_index, &ng, general_index /*scratch: not written when chained*/, &no, nullptr, nullptr,
+                        nullptr, nullptr, nullptr);
     if (rc != TLOAM_B200_OK) return rc;
-    if (ns) {
-      k_chain_gather_segmented<<<(unsigned)((ns + 255) / 256), 256, 0, h->stream>>>(d_opts, d_obeam, d_oidx, h->seg.seg, (unsigned)ns, d_spts, d_sbeam,
-                                                                                     d_sorig);
+    if (ng) CU_TRY(cudaMemcpyAsync(d_gnd, h->seg.ground, ng * 4, cudaMemcpyDeviceToDevice, h->stream));
+    if (beam) CU_TRY(cudaMemcpyAsync(c + o_beam, h->seg.beam, nk * 4, cudaMemcpyDeviceToDevice, h->stream));
+    if (intensity) CU_TRY(cudaMemcpyAsync(c + o_int, h->seg.intensity, nk * 8, cudaMemcpyDeviceToDevice, h->stream));
+    if (no) {
+      CU_TRY(cudaMemcpyAsync(d_oidx, h->seg.object, no * 4, cudaMemcpyDeviceToDevice, h->stream));
+      k_chain_gather_object<<<(unsigned)((no + 255) / 256), 256, 0, h->stream>>>(pts, h->seg.intensity, h->seg.object, (unsigned)no, d_opts, d_obeam);
       CU_TRY(cudaGetLastError());
-      // ---- 3. extractEdgePoint ----
-      h->seg.dev_xyz = d_spts; h->seg.dev_intensity = d_sbeam;
-      rc = tloam_b200_extract_edge(h, gcfg->sensor_model, ring_min_num, d_spts, d_sbeam, ns, edge_index, &ne, general_index, &nn);
+      // ---- 2. objectSegmentation ----
+      h->seg.dev_xyz = d_opts;
+      size_t ns = 0;
+      rc = tloam_b200_object_segmentation(h, dcfg, d_opts /*placeholder: read on the device*/, no, general_index, &ns, n_clusters, sizes, boxes,
+                                          nullptr, nullptr, nullptr, nullptr);
       if (rc != TLOAM_B200_OK) return rc;
+      if (ns) {
+        k_chain_gather_segmented<<<(unsigned)((ns + 255) / 256), 256, 0, h->stream>>>(d_opts, d_obeam, d_oidx, h->seg.seg, (unsigned)ns, d_spts,
+                                                                                       d_sbeam, d_sorig);
+        CU_TRY(cudaGetLastError());
+        // ---- 3. extractEdgePoint ----
+        h->seg.dev_xyz = d_spts; h->seg.dev_intensity = d_sbeam;
+        rc = tloam_b200_extract_edge(h, gcfg->sensor_model, ring_min_num, d_spts, d_sbeam, ns, edge_index, &ne, general_index, &nn);
+        if (rc != TLOAM_B200_OK) return rc;
+      }
     }
   }
-  const size_t most = ng > ne ? (ng > nn ? ng : nn) : (ne > nn ? ne : nn);
+  const size_t nki = intensity ? nk : 0;
+  size_t most = ng > ne ? (ng > nn ? ng : nn) : (ne > nn ? ne : nn);
+  most = most > nki ? most : nki;
   if (most) {
-    k_chain_final<<<dim3((unsigned)((most + 255) / 256), 3), 256, 0, h->stream>>>(d_gnd, (unsigned)ng, h->seg.edge, (unsigned)ne, h->seg.non_edge,
-                                                                                   (unsigned)nn, d_sorig, d_fg, d_fe, d_fn);
+    k_chain_final<<<dim3((unsigned)((most + 255) / 256), intensity ? 4 : 3), 256, 0, h->stream>>>(
+        d_gnd, (unsigned)ng, h->seg.edge, (unsigned)ne, h->seg.non_edge, (unsigned)nn, d_sorig, raw_of, (const double*)(c + o_int), (unsigned)nki,
+        d_fg, d_fe, d_fn, (double*)(c + o_fi));
     CU_TRY(cudaGetLastError());
     static_assert(sizeof(size_t) == sizeof(unsigned long long), "index lists are copied straight into size_t arrays");
     if (ng) CU_TRY(cudaMemcpyAsync(ground_index, d_fg, ng * 8, cudaMemcpyDeviceToHost, h->stream));
@@ -2689,9 +2741,25 @@ int tloam_b200_segment_scan(tloam_b200_handle* h, const tloam_ground_config* gcf
     if (nn) CU_TRY(cudaMemcpyAsync(general_index, d_fn, nn * 8, cudaMemcpyDeviceToHost, h->stream));
   }
   if (beam) CU_TRY(cudaMemcpyAsync(beam, c + o_beam, n * 4, cudaMemcpyDeviceToHost, h->stream));
+  if (intensity) CU_TRY(cudaMemcpyAsync(intensity, c + o_fi, n * 8, cudaMemcpyDeviceToHost, h->stream));
   CU_TRY(cudaStreamSynchronize(h->stream));
   *n_ground = ng; *n_edge = ne; *n_general = nn;
   return TLOAM_B200_OK;
+}
+
+int tloam_b200_segment_scan(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg, int ring_min_num,
+                            const double* xyz, size_t n, size_t* ground_index, size_t* n_ground, size_t* edge_index, size_t* n_edge,
+                            size_t* general_index, size_t* n_general, int* n_clusters, int* sizes, double* boxes, int* beam) {
+  return segment_chain(h, gcfg, dcfg, ring_min_num, false, 0.0, xyz, n, ground_index, n_ground, edge_index, n_edge, general_index, n_general,
+                       n_clusters, sizes, boxes, beam, nullptr);
+}
+
+int tloam_b200_segment_raw_scan(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg, int ring_min_num,
+                                double near_dis, const double* xyz, size_t n, size_t* ground_index, size_t* n_ground, size_t* edge_index,
+                                size_t* n_edge, size_t* general_index, size_t* n_general, int* n_clusters, int* sizes, double* boxes,
+                                double* intensity) {
+  return segment_chain(h, gcfg, dcfg, ring_min_num, true, near_dis, xyz, n, ground_index, n_ground, edge_index, n_edge, general_index, n_general,
+                       n_clusters, sizes, boxes, nullptr, intensity);
 }
 
 int tloam_b200_host_alloc(void** p, size_t bytes) {

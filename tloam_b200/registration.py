@@ -331,6 +331,29 @@ class LocalRegistration:
         return dict(ground=g[:ng.value].copy(), object=o[:no.value].copy(), beam=beam[:n].copy(), region=region[:n].copy(),
                     height_threshold=thr.value, planes=planes)
 
+    def ground_remove(self, scan, **overrides):
+        """ground_extract with the reference's FP64 intensity channel (VLP-16: beamId + correctTime, sensor_model=16).
+        Returns dict(ground, object, intensity, region, height_threshold, planes)."""
+        a = _f64(scan).reshape(-1, 3)
+        n = a.shape[0]
+        c = _lib.GroundConfig()
+        self._L.tloam_b200_ground_default_config(C.byref(c))
+        for k, v in overrides.items():
+            setattr(c, k, v)
+        g = np.zeros(max(n, 1), dtype=np.uintp)
+        o = np.zeros(max(n, 1), dtype=np.uintp)
+        ng, no = C.c_size_t(0), C.c_size_t(0)
+        inten = np.zeros(max(n, 1))
+        region = np.zeros(max(n, 1), dtype=np.int32)
+        thr = C.c_double(0)
+        planes = np.zeros((12, 8, 4))
+        szp, ip = C.POINTER(C.c_size_t), C.POINTER(C.c_int)
+        self._check(self._L.tloam_b200_ground_remove(self._h, C.byref(c), _dp(a), n, g.ctypes.data_as(szp), C.byref(ng),
+                                                     o.ctypes.data_as(szp), C.byref(no), _dp(inten), region.ctypes.data_as(ip),
+                                                     C.byref(thr), _dp(planes)), "ground_remove")
+        return dict(ground=g[:ng.value].copy(), object=o[:no.value].copy(), intensity=inten[:n].copy(), region=region[:n].copy(),
+                    height_threshold=thr.value, planes=planes)
+
     # ---- "next" row (f)-4, second part: edge extraction (ref: segmentation.cpp:1144-1304) ----
     def extract_edge(self, points, intensity, sensor_model=64, ring_min_num=16):
         """Segmentation::extractEdgePoint on the device.  intensity holds the beam id of every point (as groundRemove leaves
@@ -410,6 +433,36 @@ class LocalRegistration:
         k = ncl.value
         return dict(ground=g[:ng.value].copy(), edge=e[:ne.value].copy(), general=o[:no.value].copy(), sizes=sizes[:k].copy(),
                     boxes=boxes[:k].copy(), beam=beam[:n].copy())
+
+    def segment_raw_scan(self, scan, near_dis=3.0, ring_min_num=131, ground=None, dcvc=None):
+        """RemoveClosedNonFinitePoints(near_dis) -> groundRemove -> objectSegmentation -> extractEdgePoint on the device, the
+        raw scan as the driver delivers it (NaN / Inf rows allowed; a point is kept iff its norm is >= near_dis**2, as in the
+        reference).  Returns dict(ground, edge, general, sizes, boxes, intensity): index lists into the RAW scan, the cluster
+        table, the FP64 channel per raw point (NaN where removed).  ground / dcvc: dicts of configuration overrides."""
+        a = _f64(scan).reshape(-1, 3)
+        n = a.shape[0]
+        gc, dc = _lib.GroundConfig(), _lib.DcvcConfig()
+        self._L.tloam_b200_ground_default_config(C.byref(gc))
+        self._L.tloam_b200_dcvc_default_config(C.byref(dc))
+        for k, v in (ground or {}).items():
+            setattr(gc, k, v)
+        for k, v in (dcvc or {}).items():
+            setattr(dc, k, v)
+        m = max(n, 1)
+        g, e, o = (np.zeros(m, dtype=np.uintp) for _ in range(3))
+        ng, ne, no = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+        ncl = C.c_int(0)
+        sizes = np.zeros(m, dtype=np.int32)
+        inten = np.zeros(m)
+        boxes = np.zeros((m, 6))
+        szp, ip = C.POINTER(C.c_size_t), C.POINTER(C.c_int)
+        self._check(self._L.tloam_b200_segment_raw_scan(self._h, C.byref(gc), C.byref(dc), ring_min_num, float(near_dis), _dp(a), n,
+                                                        g.ctypes.data_as(szp), C.byref(ng), e.ctypes.data_as(szp), C.byref(ne),
+                                                        o.ctypes.data_as(szp), C.byref(no), C.byref(ncl), sizes.ctypes.data_as(ip),
+                                                        _dp(boxes), _dp(inten)), "segment_raw_scan")
+        k = ncl.value
+        return dict(ground=g[:ng.value].copy(), edge=e[:ne.value].copy(), general=o[:no.value].copy(), sizes=sizes[:k].copy(),
+                    boxes=boxes[:k].copy(), intensity=inten[:n].copy())
 
     # ---- shared map (multi-GPU) ----
     def map_blob_size(self):
