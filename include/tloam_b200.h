@@ -414,6 +414,44 @@ int tloam_b200_segment_raw_scan(tloam_b200_handle* h, const tloam_ground_config*
                                 size_t* n_edge, size_t* general_index, size_t* n_general, int* n_clusters, int* sizes, double* boxes,
                                 double* intensity);
 
+/* ---- FrontEnd::processCloud on the device (ref: src/front_end/front_end.cpp:181-199): the scan features become the
+ * registration source without leaving the GPU.  VoxelDownSample(ground, ground_down_sample) and VoxelDownSample(edge,
+ * edge_down_sample), extractPlanarSphere(general) with fcfg, SelectByIndex of the planar and sphere features, then
+ * setInputSource: the four clouds become the handle's source exactly as if tloam_b200_set_source had been called with
+ * them (staged, so tloam_b200_submap_update[_chained] can append them).  n_source[4] receives their sizes (edge, sphere,
+ * planar, ground).
+ *   - The down-sampled ground / edge features come out in ascending voxel index (ix, iy, iz) -- the registration caps
+ *     (*_maxnum) take features in index order, so the order is part of the result -- with the averages in the fixed-point
+ *     form of tloam_b200_voxel_down_sample (within 1e-12 m of an FP64 running sum, bit-reproducible).
+ *   - The sphere feature is general[0 .. n_sphere_scan): the reference's sphere lists hold ranks, not point indices
+ *     (feature_extract.cpp:183-188; see tloam_b200_extract_planar_sphere), and SelectByIndex takes them literally.
+ *   - The frame's raw edge and ground clouds, its planar-submap selection general[planar_submap_index] and its sphere-submap
+ *     count stay on the device for tloam_b200_submap_init_frame / tloam_b200_submap_update_frame*.
+ *   - Empty clouds are allowed: an empty general cloud selects nothing, an empty ground / edge cloud gives an empty feature.
+ *     Voxel sizes must be > 0 even then.  A map cell of the PCA grid holding more than 65535 points: MAP_DENSITY.
+ *   - Synchronises once to read the counts; no point data crosses PCIe except the three input clouds (HOST, n x 3 FP64).
+ *   - All device work runs on the handle's stream, so frame k+1 may be processed as soon as frame k's submap update has
+ *     been enqueued. */
+int tloam_b200_process_cloud(tloam_b200_handle* h, const tloam_feature_config* fcfg, double ground_down_sample, double edge_down_sample,
+                             const double* ground, size_t ng, const double* edge, size_t ne, const double* general, size_t nn,
+                             size_t n_source[4]);
+/* tloam_b200_segment_raw_scan followed by tloam_b200_process_cloud without the host in between: the raw scan (HOST, may hold
+ * NaN / Inf rows) is uploaded once, segmented on the device, the ground / edge / general clouds are gathered from it on the
+ * device, then processed as above.  An all-NaN or all-near scan gives four empty sources and OK. */
+int tloam_b200_process_raw_scan(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg, int ring_min_num,
+                                double near_dis, const tloam_feature_config* fcfg, double ground_down_sample, double edge_down_sample,
+                                const double* xyz, size_t n, size_t n_source[4]);
+/* copies source cloud `cloud` (0 edge, 1 sphere, 2 planar, 3 ground; sensor frame, FP64 AoS) to the host (synchronises) */
+int tloam_b200_source_download(tloam_b200_handle* h, int cloud, double* out, size_t capacity_points);
+/* tloam_b200_submap_init from the last processed frame (front_end.cpp:285-305): edge = its raw edge cloud, ground =
+ * VoxelDownSample(cfg->ground_down_sample) of its raw ground cloud, planar = general[planar_submap_index], sphere =
+ * general[0 .. n_sphere_submap).  NOT_READY before any processed frame. */
+int tloam_b200_submap_init_frame(tloam_b200_handle* h, const tloam_submap_config* cfg);
+/* tloam_b200_submap_update / _chained with planar_sub = the last processed frame's planar-submap selection, read on the
+ * device.  NOT_READY before any processed frame. */
+int tloam_b200_submap_update_frame(tloam_b200_handle* h, const double pose[16]);
+int tloam_b200_submap_update_frame_chained(tloam_b200_handle* h);
+
 /* Pinned host memory helpers (optional; pinned inputs make set_* a direct DMA, no staging threads). */
 int tloam_b200_host_alloc(void** p, size_t bytes);
 int tloam_b200_host_free(void* p);

@@ -1,0 +1,113 @@
+// front_end_b200.hpp -- C++ shim: tloam::FrontEndB200, the device side of FrontEnd's per-frame glue
+// (ref: src/front_end/front_end.cpp:181-199 processCloud, :201-267 updateSubmap, :285-305 the first-frame branch) on the
+// C ABI of libtloam_b200.so, driving a tloam::LocalRegistrationB200 handle.  Header-only; from the host side it needs only
+// CloudData::cloud_ptr->points_ (contiguous std::vector<Eigen::Vector3d>) and Eigen::Isometry3d::matrix().data().
+//
+// The per-frame loop of FrontEnd::updateLidarOdometry becomes three calls, each on the registration handle's stream:
+//     processCloud(ground, edge, general)    replaces processCloud() + setInputSource(current_scan)
+//     registration.scanMatchingPredicted(pose)  (or scanMatching with the caller's prediction)
+//     updateSubmap(pose)                      replaces updateSubmap() + setInputTarget(submap)
+// and on the first frame processCloud + initSubmap() replace the `!odometry_inited` branch.  The scan features, the frame's
+// submap selections and the submap itself stay on the GPU; the caller reads a source cloud back only to inspect it.
+// Without the reference headers (this repository's tests) define TLOAM_B200_MOCK_HOST_TYPES and provide the host types
+// (tests/mock/mock_tloam.hpp).
+#ifndef TLOAM_B200_FRONT_END_B200_HPP
+#define TLOAM_B200_FRONT_END_B200_HPP
+
+#include <cstdio>
+#include <string>
+#include <vector>
+
+#include "../tloam_b200.h"
+#include "local_registration_b200.hpp"
+
+#ifndef TLOAM_B200_MOCK_HOST_TYPES
+#include <yaml-cpp/yaml.h>
+#include "tloam/models/utils/sensor_data.hpp"
+#include "tloam/models/utils/work_space_path.h"
+#endif
+
+namespace tloam {
+
+class FrontEndB200 {
+ public:
+  // reg: the registration handle the features are handed to (it must outlive this object)
+  FrontEndB200(LocalRegistrationB200& reg, const tloam_feature_config& fcfg, const tloam_submap_config& scfg, double ground_down_sample,
+               double edge_down_sample)
+      : h_(reg.handle()), fcfg_(fcfg), scfg_(scfg), ground_down_sample_(ground_down_sample), edge_down_sample_(edge_down_sample) {}
+
+#ifndef TLOAM_B200_MOCK_HOST_TYPES
+  // Same configuration as FrontEnd::FrontEnd (ref: front_end.cpp:47-57) and featureExtract::initConfig
+  // (ref: feature_extract.cpp:13-37): config/mapping/lidar_odometry.yaml and config/mapping/feature.yaml.
+  explicit FrontEndB200(LocalRegistrationB200& reg) : h_(reg.handle()) {
+    const YAML::Node lo = YAML::LoadFile(WORK_SPACE_PATH + "/config/mapping/lidar_odometry.yaml");
+    ground_down_sample_ = lo["ground_down_sample"].as<double>();
+    edge_down_sample_ = lo["edge_down_sample"].as<double>();
+    tloam_b200_submap_default_config(&scfg_);
+    scfg_.ground_down_sample = ground_down_sample_;
+    scfg_.ground_down_sample_submap = lo["ground_down_sample_submap"].as<double>();
+    scfg_.edge_down_sample_submap = lo["edge_down_sample_submap"].as<double>();
+    scfg_.sphere_frame_size = lo["sphere_frame_size"].as<int>();
+    scfg_.planar_frame_size = lo["planar_frame_size"].as<int>();
+    scfg_.edge_crop_box_length = lo["edge_crop_box_length"].as<double>();
+    scfg_.ground_crop_box_length = lo["ground_crop_box_length"].as<double>();
+    const YAML::Node fe = YAML::LoadFile(WORK_SPACE_PATH + "/config/mapping/feature.yaml")["feature"];
+    tloam_b200_feature_default_config(&fcfg_);
+    fcfg_.radius = fe["radius"].as<double>();
+    fcfg_.K = fe["K"].as<int>();
+    fcfg_.planar_num = fe["planar_num"].as<int>();
+    fcfg_.sphere_num = fe["sphere_num"].as<int>();
+    fcfg_.min_neigh = fe["min_neigh"].as<int>();
+    fcfg_.cvr_scan = fe["cvr_scan"].as<double>();
+    fcfg_.cvr_submap = fe["cvr_submap"].as<double>();
+    fcfg_.planar_scan_thres = fe["planar_scan_thres"].as<double>();
+    fcfg_.planar_submap_thres = fe["planar_submap_thres"].as<double>();
+    fcfg_.planar_vertic_thres = fe["planar_vertic_thres"].as<double>();
+  }
+#endif
+
+  // processCloud + setInputSource (ref: front_end.cpp:181-199, :313): the three clouds the segmentation nodelet publishes
+  bool processCloud(CloudData& ground, CloudData& edge, CloudData& general) {
+    return report(tloam_b200_process_cloud(h_, &fcfg_, ground_down_sample_, edge_down_sample_, data(ground), size(ground), data(edge),
+                                           size(edge), data(general), size(general), n_source_),
+                  "processCloud");
+  }
+  // the `!odometry_inited` branch (ref: front_end.cpp:285-305) from the frame processCloud saw last
+  bool initSubmap() { return report(tloam_b200_submap_init_frame(h_, &scfg_), "initSubmap"); }
+  // updateSubmap + setInputTarget (ref: front_end.cpp:201-267, :333): pose = the new lidar_odom_pose
+  bool updateSubmap(const Eigen::Isometry3d& pose) {
+    return report(tloam_b200_submap_update_frame(h_, pose.matrix().data()), "updateSubmap");
+  }
+  // the same with the pose of the frame just enqueued on the handle (tloam_b200_scan_match_predicted_async): no host round trip
+  bool updateSubmapChained() { return report(tloam_b200_submap_update_frame_chained(h_), "updateSubmapChained"); }
+
+  // sizes of the current source (edge, sphere, planar, ground) and a copy of one of its clouds (inspection)
+  const size_t* sourceSizes() const { return n_source_; }
+  bool sourceCloud(int cloud, std::vector<Eigen::Vector3d>& out) {
+    if (cloud < 0 || cloud > 3) return report(TLOAM_B200_ERR_INVALID_ARG, "sourceCloud");
+    out.resize(n_source_[cloud]);
+    return report(tloam_b200_source_download(h_, cloud, reinterpret_cast<double*>(out.data()), out.size()), "sourceCloud");
+  }
+  int lastStatus() const { return last_status_; }
+
+ private:
+  static const double* data(const CloudData& c) {
+    return c.cloud_ptr->points_.empty() ? nullptr : reinterpret_cast<const double*>(c.cloud_ptr->points_.data());
+  }
+  static size_t size(const CloudData& c) { return c.cloud_ptr->points_.size(); }
+  bool report(int rc, const char* where) {
+    last_status_ = rc;
+    if (rc != TLOAM_B200_OK)
+      std::fprintf(stderr, "[tloam_b200] %s: %s %s\n", where, tloam_b200_status_string(rc), tloam_b200_last_error(h_));
+    return rc == TLOAM_B200_OK;
+  }
+  tloam_b200_handle* h_ = nullptr;
+  tloam_feature_config fcfg_;
+  tloam_submap_config scfg_;
+  double ground_down_sample_ = 0.3, edge_down_sample_ = 0.1;
+  size_t n_source_[4] = {0, 0, 0, 0};
+  int last_status_ = TLOAM_B200_OK;
+};
+
+}  // namespace tloam
+#endif

@@ -119,6 +119,8 @@ EXPORTS = [
     "tloam_b200_set_async_inputs", "tloam_b200_wait_stream", "tloam_b200_dense_check_counters",
     "tloam_b200_ground_default_config", "tloam_b200_ground_extract", "tloam_b200_extract_edge", "tloam_b200_dcvc_default_config", "tloam_b200_object_segmentation", "tloam_b200_segment_scan", "tloam_b200_ground_remove", "tloam_b200_segment_raw_scan", "tloam_b200_map_layout_bytes",
     "tloam_b200_map_send_buffer", "tloam_b200_map_recv_buffer", "tloam_b200_map_adopt", "tloam_b200_signal_stream",
+    "tloam_b200_process_cloud", "tloam_b200_process_raw_scan", "tloam_b200_source_download", "tloam_b200_submap_init_frame",
+    "tloam_b200_submap_update_frame", "tloam_b200_submap_update_frame_chained",
 ]
 
 _lib = None
@@ -234,5 +236,13 @@ def load():
     L.tloam_b200_segment_raw_scan.argtypes = [vp, C.POINTER(GroundConfig), C.POINTER(DcvcConfig), C.c_int, C.c_double, dp, C.c_size_t, szp, szp,
                                               szp, szp, szp, szp, ip, ip, dp, dp]
     L.tloam_b200_batch_get_profile.argtypes = [vp, C.POINTER(Profile)]
+    L.tloam_b200_process_cloud.argtypes = [vp, C.POINTER(FeatureConfig), C.c_double, C.c_double, dp, C.c_size_t, dp, C.c_size_t, dp,
+                                           C.c_size_t, szp]
+    L.tloam_b200_process_raw_scan.argtypes = [vp, C.POINTER(GroundConfig), C.POINTER(DcvcConfig), C.c_int, C.c_double,
+                                              C.POINTER(FeatureConfig), C.c_double, C.c_double, dp, C.c_size_t, szp]
+    L.tloam_b200_source_download.argtypes = [vp, C.c_int, dp, C.c_size_t]
+    L.tloam_b200_submap_init_frame.argtypes = [vp, C.POINTER(SubmapConfig)]
+    L.tloam_b200_submap_update_frame.argtypes = [vp, dp]
+    L.tloam_b200_submap_update_frame_chained.argtypes = [vp]
     _lib = L
     return L

@@ -4,7 +4,8 @@
 // (ref: front_end.cpp:285-305) with the PointCloud2 operations they use (ref: src/open3d/PointCloud2.cpp):
 //   Transform (:71-75) + operator+= (:96-132)  -> k_transform_append
 //   Crop(AxisAlignedBoundingBox) (:551-559)     -> folded into the voxel kernels (inclusive bounds)
-//   VoxelDownSample (:358-403)                  -> k_vox_min / k_vox_accum / k_vox_emit
+//   VoxelDownSample (:358-403)                  -> k_vox_min / k_vox_accum / k_vox_emit (k_vox_keys + sort +
+//                                                  k_vox_emit_sorted for the scan features of processCloud)
 // so that the map never leaves the GPU between frames: per frame only the new scan's submap selection crosses
 // PCIe, instead of the whole 12 MB map (set_target).
 //
@@ -116,6 +117,18 @@ __global__ void __launch_bounds__(256) k_vox_accum(VoxArgs a) {
   atomicAdd(&a.cnt[s], 1u);
 }
 
+// GetAveragePoint of the occupied slot s (c points) into out[0..2]; both emission orders below write it, so their values
+// are the same bits
+__device__ __forceinline__ void vox_average(const VoxArgs& a, unsigned s, unsigned c, double* out) {
+  const unsigned long long key = a.keys[s];
+  const int idx[3] = {(int)((key >> 42) & 0x1FFFFFu), (int)((key >> 21) & 0x1FFFFFu), (int)(key & 0x1FFFFFu)};
+#pragma unroll
+  for (int d = 0; d < 3; ++d) {
+    const double mb = dec_ordered(~a.minenc[d]) - a.voxel * 0.5;
+    out[d] = mb + (double)idx[d] * a.voxel + ((double)a.sums[3ull * s + d] / kVoxFix) / (double)c;
+  }
+}
+
 __global__ void __launch_bounds__(256) k_vox_emit(VoxArgs a) {
   const unsigned s = blockIdx.x * blockDim.x + threadIdx.x;
   const unsigned c = (s <= a.mask) ? a.cnt[s] : 0u;
@@ -135,13 +148,50 @@ __global__ void __launch_bounds__(256) k_vox_emit(VoxArgs a) {
   __syncthreads();
   if (!has) return;
   const unsigned j = s_base + s_w[warp] + incl - 1u;
-  const unsigned long long key = a.keys[s];
-  const int idx[3] = {(int)((key >> 42) & 0x1FFFFFu), (int)((key >> 21) & 0x1FFFFFu), (int)(key & 0x1FFFFFu)};
-#pragma unroll
-  for (int d = 0; d < 3; ++d) {
-    const double mb = dec_ordered(~a.minenc[d]) - a.voxel * 0.5;
-    a.out[3ull * j + d] = mb + (double)idx[d] * a.voxel + ((double)a.sums[3ull * s + d] / kVoxFix) / (double)c;   // GetAveragePoint
+  vox_average(a, s, c, a.out + 3ull * j);
+}
+
+// ---- ordered emission (the scan features of tloam_b200_process_cloud): the occupied voxels come out in ascending packed
+// key ix<<42 | iy<<21 | iz, i.e. ascending (ix, iy, iz) -- the order of the oracle's VoxelDownSample.  The registration caps
+// (*_maxnum) take source features in feature-index order, so a scan cloud must not be ordered by block scheduling.
+// k_vox_keys compacts the occupied slots as (~key, slot) pairs; the rank sort / bitonic network of the PCA selection
+// (feature_extract.cuh: key descending, index ascending) then orders them by ascending key (keys are distinct); k_vox_emit_sorted
+// writes the averages in that order.  The count of occupied voxels lands in *a.out_count (zeroed by k_vox_min).
+__global__ void __launch_bounds__(256) k_vox_keys(VoxArgs a, unsigned long long* key_raw, unsigned* slot_raw) {
+  const unsigned s = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool has = s <= a.mask && a.cnt[s] > 0u;
+  __shared__ unsigned s_w[8], s_base;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned b = __ballot_sync(0xffffffffu, has);
+  if (lane == 0) s_w[warp] = __popc(b);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned tot = 0;
+    for (int wi = 0; wi < 8; ++wi) { const unsigned v = s_w[wi]; s_w[wi] = tot; tot += v; }
+    s_base = tot ? atomicAdd(a.out_count, tot) : 0u;
   }
+  __syncthreads();
+  if (!has) return;
+  const unsigned j = s_base + s_w[warp] + __popc(b & ((1u << lane) - 1u));
+  key_raw[j] = ~a.keys[s];
+  slot_raw[j] = s;
+}
+
+// out[j] = the average of the j-th voxel in key order (slot_sorted: the slots after the sort), j < *a.out_count
+__global__ void __launch_bounds__(256) k_vox_emit_sorted(VoxArgs a, const unsigned* slot_sorted, double* out) {
+  const unsigned j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= *a.out_count) return;
+  const unsigned s = slot_sorted[j];
+  vox_average(a, s, a.cnt[s], out + 3ull * j);
+}
+
+// SelectByIndex (ref: src/open3d/PointCloud2.cpp:198) on the device: out[j] = in[idx[j]] (idx == nullptr: in[j]), j < n
+template <class Index>
+__global__ void __launch_bounds__(256) k_select_by_index(const double* in, const Index* idx, unsigned n, double* out) {
+  const unsigned j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const size_t i = idx ? (size_t)idx[j] : j;
+  out[3ull * j] = in[3ull * i]; out[3ull * j + 1] = in[3ull * i + 1]; out[3ull * j + 2] = in[3ull * i + 2];
 }
 
 // host-known counts of the planar / sphere map clouds -> the device-side count array (cnt[c] = n)

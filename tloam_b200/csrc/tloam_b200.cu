@@ -6,6 +6,7 @@
 #include <string.h>
 
 #include <cmath>
+#include <functional>
 #include <new>
 #include <utility>
 #include <vector>
@@ -121,12 +122,20 @@ struct tloam_b200_handle {
   double* d_acc[2] = {nullptr, nullptr};   size_t cap_acc[2] = {0, 0}, n_acc[2] = {0, 0};     // edge, ground accumulators
   double* d_acc_tmp = nullptr;             size_t cap_acc_tmp = 0;
   // n_acc is the host's UPPER BOUND of each accumulator; the exact counts live on the device (no host round trip per
-  // frame): d_cnt[0..3] unused, [4 + 2k + acc_cur[k]] = points in accumulator k, [8] scratch
+  // frame): d_cnt[0..3] unused, [4 + 2k + acc_cur[k]] = points in accumulator k, [8] scratch, [12] / [13] voxels of the
+  // ground / edge feature of tloam_b200_process_cloud
   unsigned* d_cnt = nullptr;               int acc_cur[2] = {0, 0};
   unsigned long long cum_add[2] = {0, 0}, known_cum[2] = {0, 0};  size_t known_cnt[2] = {0, 0};
   struct CntProbe { cudaEvent_t ev = nullptr; unsigned* h_vals = nullptr; unsigned long long cum[2] = {0, 0}; bool pending = false; };
   CntProbe probes[4];                      int probe_next = 0;
   bool src_staged = false;                 // d_stage_src holds the current source (needed by submap_update)
+  const double* src_ptr[4] = {nullptr, nullptr, nullptr, nullptr};   // where each source cloud is read (tloam_b200_source_download)
+  // ---- FrontEnd::processCloud on the device (tloam_b200_process_cloud / _process_raw_scan): the last processed frame.
+  //      d_frame = raw ground | raw edge | general | planar-submap selection (general[planar_submap_index]); the
+  //      sphere-submap selection is the general cloud's first fr_ns_sub points (the reference's rank lists, SURVEY Q12) ----
+  double* d_frame = nullptr;               size_t cap_frame = 0;
+  size_t fr_ng = 0, fr_ne = 0, fr_nn = 0, fr_np_sub = 0, fr_ns_sub = 0;
+  bool have_frame = false;
   // pipelined results (async_inputs): two pinned result slots + events, so that the host can stay one frame ahead
   cudaEvent_t ev_res[2] = {nullptr, nullptr};
   long long frames_enqueued = 0, frames_fetched = 0;
@@ -360,7 +369,7 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   if (h->ev_planar_in) cudaEventDestroy(h->ev_planar_in);
   if (h->ev_planar_free) cudaEventDestroy(h->ev_planar_free);
   if (h->ev_planar_done) cudaEventDestroy(h->ev_planar_done);
-  cudaFree(h->d_vox1); cudaFree(h->d_acc_tmp1); cudaFree(h->d_up_planar); cudaFree(h->d_chain);
+  cudaFree(h->d_vox1); cudaFree(h->d_acc_tmp1); cudaFree(h->d_up_planar); cudaFree(h->d_chain); cudaFree(h->d_frame);
   for (int i = 0; i < 2; ++i) if (h->ev_stage_free[i]) cudaEventDestroy(h->ev_stage_free[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_fit[i]) cudaEventDestroy(h->ev_fit[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_res[i]) cudaEventDestroy(h->ev_res[i]);
@@ -384,13 +393,16 @@ static void fill_ctx_config(tloam_b200_handle* h) {
   c.st = h->d_state; c.stats = h->d_stats; c.counter = h->d_counter;
 }
 
-static int set_source_impl(tloam_b200_handle* h, const double* const xyz[4], const size_t n[4], bool on_device) {
-  if (!h || !xyz || !n) return TLOAM_B200_ERR_INVALID_ARG;
+// fill (optional): the library writes the source itself -- the clouds are enqueued on the handle's stream straight into the
+// staging buffer (argument: cloud k starts at point n[0] + ... + n[k-1]), xyz is not read (tloam_b200_process_cloud)
+static int set_source_impl(tloam_b200_handle* h, const double* const xyz[4], const size_t n[4], bool on_device,
+                           const std::function<int(double*)>* fill = nullptr) {
+  if (!h || (!xyz && !fill) || !n) return TLOAM_B200_ERR_INVALID_ARG;
   CU_TRY(cudaSetDevice(h->device));
   size_t total = 0, pad = 0;
   int blocks = 0;
   for (int c = 0; c < 4; ++c) {
-    if (n[c] > 0 && !xyz[c]) return TLOAM_B200_ERR_INVALID_ARG;
+    if (n[c] > 0 && !fill && !xyz[c]) return TLOAM_B200_ERR_INVALID_ARG;
     if (n[c] > (size_t)1 << 30) return TLOAM_B200_ERR_INVALID_ARG;
     total += n[c];
     pad += round_up(n[c], kBlk);
@@ -399,7 +411,7 @@ static int set_source_impl(tloam_b200_handle* h, const double* const xyz[4], con
   blocks = (int)(pad / kBlk);
   // host input is staged; device input is read in place -- unless the device-side submap is in use, whose update
   // appends the staged edge / ground features after the frame (tloam_b200_submap_update)
-  const bool stage = !on_device || h->submap_ready;
+  const bool stage = !on_device || h->submap_ready || fill;
   // (re)allocations: a pointer is nulled and its capacity zeroed right after the free, and the new capacity is only
   // committed once the allocation succeeded, so a failed cudaMalloc leaves the handle consistent
   h->have_src = false; h->src_staged = false;
@@ -441,7 +453,8 @@ static int set_source_impl(tloam_b200_handle* h, const double* const xyz[4], con
   c.blk_off[0] = 0;
   for (int k = 0; k < 4; ++k) {
     src[k] = stage ? h->d_stage_src + 3 * off : xyz[k];
-    if (n[k] > 0 && stage)
+    h->src_ptr[k] = src[k];
+    if (n[k] > 0 && stage && !fill)
     {
       static const bool stage_pageable = getenv("TLOAM_B200_NO_HOST_STAGE") == nullptr;
       if (!on_device && stage_pageable && n[k] * 24 >= (128u << 10) && HostStage::pageable(xyz[k])) {
@@ -465,6 +478,10 @@ static int set_source_impl(tloam_b200_handle* h, const double* const xyz[4], con
   c.flags = h->d_flags; c.active = h->d_flags + cp;
   c.blk_count = h->d_blk_count; c.blk_cap = (int)h->cap_blocks; c.partial = h->d_partial;
   h->total_blocks = c.blk_off[4];
+  if (fill) {
+    const int rc = (*fill)(h->d_stage_src);
+    if (rc != TLOAM_B200_OK) return rc;
+  }
   if (!on_device) CU_TRY(cudaEventRecord(h->ev_src, up));             // the uploads are in; the caller's buffers are free
   if (prefetch) CU_TRY(cudaStreamWaitEvent(h->stream, h->ev_src, 0));
   if (h->total_blocks > 0) {
@@ -1795,14 +1812,22 @@ static int ensure_dev(tloam_b200_handle* h, double** p, size_t* cap, size_t need
 // *out_count (device).  The input holds n_bound points at most; its exact count is n_bound itself (n_dev == nullptr)
 // or *n_dev + n_add.  The crop box is lo/hi (host values; nullptr = none) or pose.t +- box_len with the pose in
 // device memory.
+// sorted (optional): the voxels are put in ascending key order instead of being emitted (the scan features of
+// tloam_b200_process_cloud, see submap.cuh); voxel_emit_sorted writes them once the count is known.
+struct VoxSorted { VoxArgs a; unsigned* slots = nullptr; };
 static int voxel_pipeline(tloam_b200_handle* h, const double* d_in, size_t n_bound, const unsigned* n_dev, unsigned n_add,
                           const double* lo, const double* hi, const double* box_pose, double box_len, double voxel,
-                          double* d_out, unsigned* out_count, cudaStream_t stream = nullptr, int scratch = 0) {
+                          double* d_out, unsigned* out_count, cudaStream_t stream = nullptr, int scratch = 0,
+                          VoxSorted* sorted = nullptr) {
   if (!stream) stream = h->stream;
+  if (sorted) sorted->slots = nullptr;
   if (n_bound == 0) { CU_TRY(cudaMemsetAsync(out_count, 0, sizeof(unsigned), stream)); return TLOAM_B200_OK; }
   if (!(voxel > 0.0)) return TLOAM_B200_ERR_INVALID_ARG;
   const unsigned tsize = next_pow2(2 * n_bound + 1);
-  const size_t bytes = 256 + (size_t)tsize * (8 + 24 + 4);
+  size_t npad = 1;                                     // the bitonic network pads the list to a power of two
+  while (npad < n_bound) npad <<= 1;
+  const size_t o_sort = 256 + (size_t)tsize * (8 + 24 + 4);
+  const size_t bytes = o_sort + (sorted ? npad * (8 + 8 + 4 + 4 + 4) : 0);
   unsigned char*& d_vox = scratch ? h->d_vox1 : h->d_vox;
   size_t& cap_vox = scratch ? h->cap_vox1 : h->cap_vox;
   if (bytes > cap_vox) {
@@ -1826,7 +1851,38 @@ static int voxel_pipeline(tloam_b200_handle* h, const double* d_in, size_t n_bou
   const unsigned tb = 256, gb = (unsigned)((n_bound + tb - 1) / tb);
   TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_vox_min<<<(gb < 592u ? gb : 592u), tb, 0, stream>>>(a)));
   TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_vox_accum<<<gb, tb, 0, stream>>>(a)));
-  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_vox_emit<<<(tsize + tb - 1) / tb, tb, 0, stream>>>(a)));
+  if (!sorted) {
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_vox_emit<<<(tsize + tb - 1) / tb, tb, 0, stream>>>(a)));
+    CU_TRY(cudaGetLastError());
+    return TLOAM_B200_OK;
+  }
+  // ordered: (~key, slot) pairs sorted by the PCA selection's rank sort / bitonic network, one list (grid y = 1, one block)
+  unsigned long long* key_raw = reinterpret_cast<unsigned long long*>(d_vox + o_sort);
+  unsigned long long* key_sorted = key_raw + npad;
+  unsigned* slot_raw = reinterpret_cast<unsigned*>(key_sorted + npad);
+  unsigned* slot_sorted = slot_raw + npad;
+  unsigned* rank = slot_sorted + npad;
+  CU_TRY(cudaMemsetAsync(rank, 0, npad * sizeof(unsigned), stream));
+  if (!h->fe_sort_attr_set) {
+    CU_TRY(cudaFuncSetAttribute(k_fe_sort, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFeSortSmemBytes));
+    h->fe_sort_attr_set = true;
+  }
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_vox_keys<<<(tsize + tb - 1) / tb, tb, 0, stream>>>(a, key_raw, slot_raw)));
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_fe_rank<<<dim3(gb, 1, kFeRankSplit), 256, 0, stream>>>(key_raw, slot_raw, key_raw, slot_raw, rank, rank,
+                                                                                           out_count)));
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_fe_rank_scatter<<<dim3(gb, 1), 256, 0, stream>>>(key_raw, slot_raw, key_raw, slot_raw, rank, rank, key_sorted,
+                                                                                   slot_sorted, key_sorted, slot_sorted, out_count)));
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_fe_sort<<<1, 1024, kFeSortSmemBytes, stream>>>(key_sorted, slot_sorted, key_sorted, slot_sorted, out_count)));
+  CU_TRY(cudaGetLastError());
+  sorted->a = a;
+  sorted->slots = slot_sorted;
+  return TLOAM_B200_OK;
+}
+
+// the n voxels sorted by voxel_pipeline into out (n: the count it left in out_count, read back by the caller)
+static int voxel_emit_sorted(tloam_b200_handle* h, const VoxSorted& s, size_t n, double* out) {
+  if (n == 0) return TLOAM_B200_OK;
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_vox_emit_sorted<<<(unsigned)((n + 255) / 256), 256, 0, h->stream>>>(s.a, s.slots, out)));
   CU_TRY(cudaGetLastError());
   return TLOAM_B200_OK;
 }
@@ -1861,7 +1917,7 @@ void tloam_b200_feature_default_config(tloam_feature_config* c) {   // ref: conf
 
 namespace {
 struct FeArena {
-  double* stage; unsigned* scratch; unsigned char* blob; MapHeader hdr;
+  const double* stage; unsigned* scratch; unsigned char* blob; MapHeader hdr;
   FeOut out;
   unsigned long long *key_p_sorted, *key_s_sorted;
   unsigned *val_p_sorted, *val_s_sorted, *counts;
@@ -1869,8 +1925,10 @@ struct FeArena {
 };
 }  // namespace
 
-// carves the arena for n points and enqueues grid build + k_fe_pca (+ classification and sorts when `select`)
-static int fe_run(tloam_b200_handle* h, const tloam_feature_config* cfg, const double* xyz, size_t n, bool select, FeArena& A) {
+// carves the arena for n points and enqueues grid build + k_fe_pca (+ classification and sorts when `select`).
+// on_device: xyz is a device cloud, read in place on the handle's stream (no upload)
+static int fe_run(tloam_b200_handle* h, const tloam_feature_config* cfg, const double* xyz, size_t n, bool select, FeArena& A,
+                  bool on_device = false) {
   if (n == 0 || n > ((size_t)1 << 30)) return TLOAM_B200_ERR_INVALID_ARG;
   if (!(cfg->radius > 0.0) || cfg->K < 3 || cfg->K > kFeK) return TLOAM_B200_ERR_INVALID_ARG;   // :56 asserts K >= 3
   CU_TRY(cudaSetDevice(h->device));
@@ -1888,7 +1946,7 @@ static int fe_run(tloam_b200_handle* h, const tloam_feature_config* cfg, const d
   for (int d = 0; d < 3; ++d) { hd.bbox_enc[d] = ~0ull; hd.bbox_enc[3 + d] = 0ull; }
   size_t off = 0;
   auto take = [&](size_t bytes) { const size_t o = off; off += round_up(bytes, 256); return o; };
-  const size_t o_stage = take(n * 3 * sizeof(double)), o_scr = take(n * 2 * sizeof(unsigned)), o_blob = take(boff);
+  const size_t o_stage = on_device ? 0 : take(n * 3 * sizeof(double)), o_scr = take(n * 2 * sizeof(unsigned)), o_blob = take(boff);
   const size_t o_cvr = take(n * 8), o_flat = take(n * 8), o_sph = take(n * 8), o_nrm = take(n * 24), o_num = take(n * 4),
                o_nei = take(n * kFeK * 4);
   size_t npad = 1;                                     // the bitonic network pads each candidate list to a power of two
@@ -1902,7 +1960,7 @@ static int fe_run(tloam_b200_handle* h, const tloam_feature_config* cfg, const d
     CU_TRY(cudaMalloc(&h->d_fe, h->cap_fe));
   }
   unsigned char* b = h->d_fe;
-  A.stage = (double*)(b + o_stage); A.scratch = (unsigned*)(b + o_scr); A.blob = b + o_blob;
+  A.stage = on_device ? xyz : (const double*)(b + o_stage); A.scratch = (unsigned*)(b + o_scr); A.blob = b + o_blob;
   A.out.cvr = (double*)(b + o_cvr); A.out.flatness = (double*)(b + o_flat); A.out.sphericity = (double*)(b + o_sph);
   A.out.normal = (double*)(b + o_nrm); A.out.num_sum = (int*)(b + o_num); A.out.neigh = (int*)(b + o_nei);
   A.key_p_sorted = (unsigned long long*)(b + o_kps); A.key_s_sorted = (unsigned long long*)(b + o_kss);
@@ -1912,7 +1970,7 @@ static int fe_run(tloam_b200_handle* h, const tloam_feature_config* cfg, const d
   unsigned* val_p_raw = (unsigned*)(b + o_vpr); unsigned* val_s_raw = (unsigned*)(b + o_vsr);
   unsigned* rank_p = (unsigned*)(b + o_rk); unsigned* rank_s = rank_p + npad;
 
-  CU_TRY(cudaMemcpyAsync(A.stage, xyz, n * 3 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  if (!on_device) CU_TRY(cudaMemcpyAsync(b + o_stage, xyz, n * 3 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
   CU_TRY(cudaMemcpyAsync(A.blob, &hd, sizeof(MapHeader), cudaMemcpyHostToDevice, h->stream));
   CU_TRY(cudaMemsetAsync(A.blob + hd.table_off[0], 0, boff - hd.table_off[0], h->stream));
   CU_TRY(cudaMemsetAsync(A.counts, 0, 256, h->stream));
@@ -2050,34 +2108,36 @@ int tloam_b200_voxel_down_sample(tloam_b200_handle* h, const double* pts, size_t
   return TLOAM_B200_OK;
 }
 
-int tloam_b200_submap_init(tloam_b200_handle* h, const tloam_submap_config* cfg, const double* edge, size_t ne,
-                           const double* ground_raw, size_t ng, const double* planar_sub, size_t np,
-                           const double* sphere_sub, size_t ns) {
+// on_device: the four clouds are device buffers (tloam_b200_submap_init_frame: the last processed frame), copied D2D
+static int submap_init_impl(tloam_b200_handle* h, const tloam_submap_config* cfg, const double* edge, size_t ne,
+                            const double* ground_raw, size_t ng, const double* planar_sub, size_t np,
+                            const double* sphere_sub, size_t ns, bool on_device) {
   if (!h || !cfg || (!edge && ne) || (!ground_raw && ng) || (!planar_sub && np) || (!sphere_sub && ns)) return TLOAM_B200_ERR_INVALID_ARG;
   if (cfg->planar_frame_size < 1 || cfg->planar_frame_size > 64) return TLOAM_B200_ERR_INVALID_ARG;
   CU_TRY(cudaSetDevice(h->device));
   h->scfg = *cfg;
   if (!h->d_pose) CU_TRY(cudaMalloc(&h->d_pose, 16 * sizeof(double)));
   int rc;
+  const cudaMemcpyKind kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
   h->acc_cur[0] = h->acc_cur[1] = 0;
   // edge: raw copy (front_end.cpp:286)
   if ((rc = ensure_dev(h, &h->d_acc[0], &h->cap_acc[0], ne, false)) != TLOAM_B200_OK) return rc;
-  if (ne) CU_TRY(cudaMemcpyAsync(h->d_acc[0], edge, ne * 3 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  if (ne) CU_TRY(cudaMemcpyAsync(h->d_acc[0], edge, ne * 3 * sizeof(double), kind, h->stream));
   h->n_acc[0] = ne;
   k_set_counts<<<1, 32, 0, h->stream>>>(h->d_cnt + 4, 0, (unsigned)ne, -1, 0u);
   // ground: VoxelDownSample(ground_down_sample) (:287)
-  if ((rc = upload_points(h, ground_raw, ng)) != TLOAM_B200_OK) return rc;
+  if (!on_device && (rc = upload_points(h, ground_raw, ng)) != TLOAM_B200_OK) return rc;
   if ((rc = ensure_dev(h, &h->d_acc[1], &h->cap_acc[1], ng, false)) != TLOAM_B200_OK) return rc;
-  if ((rc = voxel_pipeline(h, h->d_up, ng, nullptr, 0u, nullptr, nullptr, nullptr, 0.0, cfg->ground_down_sample, h->d_acc[1],
-                           acc_count(h, 1))) != TLOAM_B200_OK) return rc;
+  if ((rc = voxel_pipeline(h, on_device ? ground_raw : h->d_up, ng, nullptr, 0u, nullptr, nullptr, nullptr, 0.0, cfg->ground_down_sample,
+                           h->d_acc[1], acc_count(h, 1))) != TLOAM_B200_OK) return rc;
   // planar / sphere: the submap-index selections (:291-292); the sliding-window buffers stay empty (:285-305)
   if ((rc = ensure_dev(h, &h->d_cat, &h->cap_cat, np, false)) != TLOAM_B200_OK) return rc;
-  if (np) CU_TRY(cudaMemcpyAsync(h->d_cat, planar_sub, np * 3 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  if (np) CU_TRY(cudaMemcpyAsync(h->d_cat, planar_sub, np * 3 * sizeof(double), kind, h->stream));
   h->n_cat = np;
   cudaFree(h->d_sphere0); h->d_sphere0 = nullptr;
   if (ns) {
     CU_TRY(cudaMalloc(&h->d_sphere0, ns * 3 * sizeof(double)));
-    CU_TRY(cudaMemcpyAsync(h->d_sphere0, sphere_sub, ns * 3 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    CU_TRY(cudaMemcpyAsync(h->d_sphere0, sphere_sub, ns * 3 * sizeof(double), kind, h->stream));
   }
   h->n_sphere0 = ns; h->sphere_is_init = true;
   for (double* p : h->ring) cudaFree(p);
@@ -2094,10 +2154,18 @@ int tloam_b200_submap_init(tloam_b200_handle* h, const tloam_submap_config* cfg,
   return submap_set_target(h);
 }
 
+int tloam_b200_submap_init(tloam_b200_handle* h, const tloam_submap_config* cfg, const double* edge, size_t ne,
+                           const double* ground_raw, size_t ng, const double* planar_sub, size_t np,
+                           const double* sphere_sub, size_t ns) {
+  return submap_init_impl(h, cfg, edge, ne, ground_raw, ng, planar_sub, np, sphere_sub, ns, false);
+}
+
 // FrontEnd::updateSubmap (ref: front_end.cpp:201-267) enqueued WITHOUT a host round trip: the voxel counts that size the
 // next map stay on the device (the host only tracks upper bounds, tightened by asynchronous read-backs), and in the
 // chained form the pose is the device-resident result of the frame that was just enqueued.
-static int submap_update_impl(tloam_b200_handle* h, const double* pose_host, const double* planar_sub, size_t np) {
+// planar_on_device: planar_sub is a device buffer written on the handle's stream (the last processed frame's selection), read in place
+static int submap_update_impl(tloam_b200_handle* h, const double* pose_host, const double* planar_sub, size_t np,
+                              bool planar_on_device = false) {
   if (!h || (!planar_sub && np)) return TLOAM_B200_ERR_INVALID_ARG;
   if (!h->submap_ready || !h->have_src) return TLOAM_B200_ERR_NOT_READY;
   if (!h->src_staged) return TLOAM_B200_ERR_NOT_READY;           // the staged source is what gets appended
@@ -2120,7 +2188,9 @@ static int submap_update_impl(tloam_b200_handle* h, const double* pose_host, con
   static const bool no_prefetch = getenv("TLOAM_B200_NO_PREFETCH") != nullptr;
   const bool side = h->async_inputs && !h->profiling && !no_prefetch;
   const double* d_planar_in = nullptr;
-  if (side) {
+  if (planar_on_device) {
+    d_planar_in = planar_sub;                                     // ordered by the fork below (ps waits for the handle's stream)
+  } else if (side) {
     if (np > h->cap_up_planar) {
       CU_TRY(cudaStreamSynchronize(h->stream));
       cudaFree(h->d_up_planar); h->d_up_planar = nullptr; h->cap_up_planar = 0;
@@ -2144,7 +2214,7 @@ static int submap_update_impl(tloam_b200_handle* h, const double* pose_host, con
     CU_TRY(cudaEventRecord(h->ev_sub[0], h->stream));
     CU_TRY(cudaStreamWaitEvent(gs, h->ev_sub[0], 0));
     CU_TRY(cudaStreamWaitEvent(ps, h->ev_sub[0], 0));
-    CU_TRY(cudaStreamWaitEvent(ps, h->ev_planar_in, 0));
+    if (!planar_on_device) CU_TRY(cudaStreamWaitEvent(ps, h->ev_planar_in, 0));
   }
   double* slot = nullptr; size_t slot_cap = 0;
   if ((int)h->ring.size() >= cf.planar_frame_size) {            // recycle the oldest buffer
@@ -2639,11 +2709,14 @@ __global__ void __launch_bounds__(256) k_chain_final(const unsigned* ground, uns
 
 // The one implementation of the chained segmentation.  remove: run RemoveClosedNonFinitePoints(near_dis) on the device
 // first (tloam_b200_segment_raw_scan); tloam_b200_segment_scan runs without that step.  beam / intensity (optional, n
-// values): the channel of every point of the scan as int / FP64 (NaN for removed points).
+// values): the channel of every point of the scan as int / FP64 (NaN for removed points).  keep (optional): the three final
+// lists stay on the device (tloam_b200_process_raw_scan) -- the index arrays are not written, *keep receives the uploaded scan
+// and the lists (valid until the handle's next segmentation call); the counts still land in *n_ground / *n_edge / *n_general.
+struct ChainKeep { const double* scan = nullptr; const unsigned long long *ground = nullptr, *edge = nullptr, *general = nullptr; };
 static int segment_chain(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg, int ring_min_num, bool remove,
                          double near_dis, const double* xyz, size_t n, size_t* ground_index, size_t* n_ground, size_t* edge_index,
                          size_t* n_edge, size_t* general_index, size_t* n_general, int* n_clusters, int* sizes, double* boxes, int* beam,
-                         double* intensity) {
+                         double* intensity, ChainKeep* keep = nullptr) {
   if (!h || !gcfg || !dcfg || !ground_index || !n_ground || !edge_index || !n_edge || !general_index || !n_general || !n_clusters)
     return TLOAM_B200_ERR_INVALID_ARG;
   *n_ground = *n_edge = *n_general = 0; *n_clusters = 0;
@@ -2736,10 +2809,11 @@ static int segment_chain(tloam_b200_handle* h, const tloam_ground_config* gcfg, 
         d_fg, d_fe, d_fn, (double*)(c + o_fi));
     CU_TRY(cudaGetLastError());
     static_assert(sizeof(size_t) == sizeof(unsigned long long), "index lists are copied straight into size_t arrays");
-    if (ng) CU_TRY(cudaMemcpyAsync(ground_index, d_fg, ng * 8, cudaMemcpyDeviceToHost, h->stream));
-    if (ne) CU_TRY(cudaMemcpyAsync(edge_index, d_fe, ne * 8, cudaMemcpyDeviceToHost, h->stream));
-    if (nn) CU_TRY(cudaMemcpyAsync(general_index, d_fn, nn * 8, cudaMemcpyDeviceToHost, h->stream));
+    if (ng && !keep) CU_TRY(cudaMemcpyAsync(ground_index, d_fg, ng * 8, cudaMemcpyDeviceToHost, h->stream));
+    if (ne && !keep) CU_TRY(cudaMemcpyAsync(edge_index, d_fe, ne * 8, cudaMemcpyDeviceToHost, h->stream));
+    if (nn && !keep) CU_TRY(cudaMemcpyAsync(general_index, d_fn, nn * 8, cudaMemcpyDeviceToHost, h->stream));
   }
+  if (keep) { keep->scan = d_scan; keep->ground = d_fg; keep->edge = d_fe; keep->general = d_fn; }
   if (beam) CU_TRY(cudaMemcpyAsync(beam, c + o_beam, n * 4, cudaMemcpyDeviceToHost, h->stream));
   if (intensity) CU_TRY(cudaMemcpyAsync(intensity, c + o_fi, n * 8, cudaMemcpyDeviceToHost, h->stream));
   CU_TRY(cudaStreamSynchronize(h->stream));
@@ -2760,6 +2834,164 @@ int tloam_b200_segment_raw_scan(tloam_b200_handle* h, const tloam_ground_config*
                                 double* intensity) {
   return segment_chain(h, gcfg, dcfg, ring_min_num, true, near_dis, xyz, n, ground_index, n_ground, edge_index, n_edge, general_index, n_general,
                        n_clusters, sizes, boxes, nullptr, intensity);
+}
+
+// ---------------------------------------------------------------------------------------------
+// FrontEnd::processCloud (ref: src/front_end/front_end.cpp:181-199) + setInputSource on the device: the frame's ground /
+// edge / general clouds sit in h->d_frame, and the four features are written straight into the registration's staging
+// buffer.  Every launch and copy goes on the handle's stream.  That stream order is what lets process_* of frame k+1
+// overwrite d_frame (the planar-submap selection of frame k) and the staging buffer: the submap update of frame k reads
+// them on side streams that it joins back into the handle's stream before it returns.
+// ---------------------------------------------------------------------------------------------
+static int reserve_frame(tloam_b200_handle* h, size_t ng, size_t ne, size_t nn) {
+  const size_t need = ng + ne + 2 * nn;                   // raw ground | raw edge | general | planar-submap selection (<= nn)
+  if (need <= h->cap_frame) return TLOAM_B200_OK;
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  cudaFree(h->d_frame); h->d_frame = nullptr; h->cap_frame = 0;
+  const size_t ncap = need + need / 4 + 1024;
+  CU_TRY(cudaMalloc(&h->d_frame, ncap * 3 * sizeof(double)));
+  h->cap_frame = ncap;
+  return TLOAM_B200_OK;
+}
+
+static int process_frame(tloam_b200_handle* h, const tloam_feature_config* fcfg, double ground_down_sample, double edge_down_sample,
+                         size_t ng, size_t ne, size_t nn, size_t n_source[4]) {
+  const double* d_ground = h->d_frame;
+  const double* d_edge = d_ground + 3 * ng;
+  const double* d_general = d_edge + 3 * ne;
+  double* d_planar_sub = h->d_frame + 3 * (ng + ne + nn);
+  int rc;
+  // VoxelDownSample of the ground (:183) and edge (:186) clouds, sorted by voxel key (the caps take features in index
+  // order); each keeps its own voxel scratch until the emission below
+  VoxSorted vg, ve;
+  if ((rc = voxel_pipeline(h, d_ground, ng, nullptr, 0u, nullptr, nullptr, nullptr, 0.0, ground_down_sample, nullptr, h->d_cnt + 12,
+                           h->stream, 0, &vg)) != TLOAM_B200_OK) return rc;
+  if ((rc = voxel_pipeline(h, d_edge, ne, nullptr, 0u, nullptr, nullptr, nullptr, 0.0, edge_down_sample, nullptr, h->d_cnt + 13,
+                           h->stream, 1, &ve)) != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaMemcpyAsync(h->h_result + 22, h->d_cnt + 12, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+  // extractPlanarSphere (:194); an empty general cloud selects nothing (feature_extract.cpp:49-54, 140).  fe_run ends with
+  // the one synchronisation of the call.
+  FeArena A;
+  unsigned fc[4] = {0u, 0u, 0u, 0u};                     // planar_submap, sphere_submap, planar_scan, sphere_scan counts
+  if (nn) {
+    if ((rc = fe_run(h, fcfg, d_general, nn, true, A, true)) != TLOAM_B200_OK) return rc;
+    memcpy(fc, h->h_result + 28, sizeof(fc));
+  } else {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+  }
+  unsigned vc[2];
+  memcpy(vc, h->h_result + 22, sizeof(vc));
+  const size_t n[4] = {vc[1], fc[3], fc[2], vc[0]};     // edge, sphere, planar, ground
+  const unsigned tb = 256;
+  // SelectByIndex (:197-198): planar = general[planar_scan_index]; sphere = general[sphere_scan_index] where the reference's
+  // sphere list holds RANKS 0..n-1 (feature_extract.cpp:183-188, SURVEY Q12), so the sphere feature is the general cloud's
+  // first n points -- restated literally, like tloam_b200_extract_planar_sphere's lists
+  const std::function<int(double*)> fill = [&](double* stage) -> int {
+    int r;
+    if ((r = voxel_emit_sorted(h, ve, n[0], stage)) != TLOAM_B200_OK) return r;
+    if (n[1]) TL_LAUNCH(TLOAM_B200_K_FEATURE, (k_select_by_index<unsigned><<<(unsigned)((n[1] + tb - 1) / tb), tb, 0, h->stream>>>(
+                                                   d_general, nullptr, (unsigned)n[1], stage + 3 * n[0])));
+    if (n[2]) TL_LAUNCH(TLOAM_B200_K_FEATURE, (k_select_by_index<unsigned><<<(unsigned)((n[2] + tb - 1) / tb), tb, 0, h->stream>>>(
+                                                   d_general, A.val_p_sorted, (unsigned)n[2], stage + 3 * (n[0] + n[1]))));
+    if ((r = voxel_emit_sorted(h, vg, n[3], stage + 3 * (n[0] + n[1] + n[2]))) != TLOAM_B200_OK) return r;
+    // the frame's planar-submap selection general[planar_submap_index] (:291, :207), kept for submap_init_frame / _update_frame
+    if (fc[0]) TL_LAUNCH(TLOAM_B200_K_FEATURE, (k_select_by_index<unsigned><<<(fc[0] + tb - 1) / tb, tb, 0, h->stream>>>(
+                                                    d_general, A.val_p_sorted, fc[0], d_planar_sub)));
+    CU_TRY(cudaGetLastError());
+    return TLOAM_B200_OK;
+  };
+  if ((rc = set_source_impl(h, nullptr, n, true, &fill)) != TLOAM_B200_OK) return rc;
+  h->fr_ng = ng; h->fr_ne = ne; h->fr_nn = nn; h->fr_np_sub = fc[0]; h->fr_ns_sub = fc[1];
+  h->have_frame = true;
+  for (int k = 0; k < 4; ++k) n_source[k] = n[k];
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_process_cloud(tloam_b200_handle* h, const tloam_feature_config* fcfg, double ground_down_sample, double edge_down_sample,
+                             const double* ground, size_t ng, const double* edge, size_t ne, const double* general, size_t nn,
+                             size_t n_source[4]) {
+  if (!h || !fcfg || !n_source || (!ground && ng) || (!edge && ne) || (!general && nn)) return TLOAM_B200_ERR_INVALID_ARG;
+  for (int k = 0; k < 4; ++k) n_source[k] = 0;
+  if (!(ground_down_sample > 0.0) || !(edge_down_sample > 0.0)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (ng > ((size_t)1 << 30) || ne > ((size_t)1 << 30) || nn > ((size_t)1 << 30)) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  h->have_frame = false;
+  int rc = reserve_frame(h, ng, ne, nn);
+  if (rc != TLOAM_B200_OK) return rc;
+  const double* src[3] = {ground, edge, general};
+  const size_t cnt[3] = {ng, ne, nn};
+  size_t off = 0;
+  for (int c = 0; c < 3; ++c) {                           // the only point data that crosses PCIe
+    if (cnt[c]) {
+      if (HostStage::pageable(src[c]) && getenv("TLOAM_B200_NO_HOST_STAGE") == nullptr)
+        CU_TRY(h->hstage.upload(h->d_frame + 3 * off, src[c], cnt[c] * 24, h->stream));
+      else
+        CU_TRY(cudaMemcpyAsync(h->d_frame + 3 * off, src[c], cnt[c] * 24, cudaMemcpyHostToDevice, h->stream));
+    }
+    off += cnt[c];
+  }
+  return process_frame(h, fcfg, ground_down_sample, edge_down_sample, ng, ne, nn, n_source);
+}
+
+int tloam_b200_process_raw_scan(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg, int ring_min_num,
+                                double near_dis, const tloam_feature_config* fcfg, double ground_down_sample, double edge_down_sample,
+                                const double* xyz, size_t n, size_t n_source[4]) {
+  if (!h || !gcfg || !dcfg || !fcfg || !n_source || (!xyz && n)) return TLOAM_B200_ERR_INVALID_ARG;
+  for (int k = 0; k < 4; ++k) n_source[k] = 0;
+  if (!(ground_down_sample > 0.0) || !(edge_down_sample > 0.0)) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  h->have_frame = false;
+  size_t unused[1];                                       // the index lists stay on the device (ChainKeep)
+  size_t ng = 0, ne = 0, nn = 0;
+  int n_clusters = 0;
+  ChainKeep keep;
+  int rc = segment_chain(h, gcfg, dcfg, ring_min_num, true, near_dis, xyz, n, unused, &ng, unused, &ne, unused, &nn, &n_clusters, nullptr,
+                         nullptr, nullptr, nullptr, &keep);
+  if (rc != TLOAM_B200_OK) return rc;
+  if ((rc = reserve_frame(h, ng, ne, nn)) != TLOAM_B200_OK) return rc;
+  const unsigned long long* lists[3] = {keep.ground, keep.edge, keep.general};
+  const size_t cnt[3] = {ng, ne, nn};
+  size_t off = 0;
+  for (int c = 0; c < 3; ++c) {                           // ground / edge / general clouds gathered from the uploaded raw scan
+    if (cnt[c]) TL_LAUNCH(TLOAM_B200_K_FEATURE, (k_select_by_index<unsigned long long><<<(unsigned)((cnt[c] + 255) / 256), 256, 0, h->stream>>>(
+                                                    keep.scan, lists[c], (unsigned)cnt[c], h->d_frame + 3 * off)));
+    off += cnt[c];
+  }
+  CU_TRY(cudaGetLastError());
+  return process_frame(h, fcfg, ground_down_sample, edge_down_sample, ng, ne, nn, n_source);
+}
+
+int tloam_b200_source_download(tloam_b200_handle* h, int cloud, double* out, size_t capacity_points) {
+  if (!h || !out || cloud < 0 || cloud > 3) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->have_src) return TLOAM_B200_ERR_NOT_READY;
+  if (capacity_points < h->n_src[cloud]) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  if (h->n_src[cloud]) CU_TRY(cudaMemcpyAsync(out, h->src_ptr[cloud], h->n_src[cloud] * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+// first-frame seeding (ref: front_end.cpp:285-305) from the last processed frame, through submap_init's body
+int tloam_b200_submap_init_frame(tloam_b200_handle* h, const tloam_submap_config* scfg) {
+  if (!h || !scfg) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->have_frame) return TLOAM_B200_ERR_NOT_READY;
+  const double* ground = h->d_frame;
+  const double* edge = ground + 3 * h->fr_ng;
+  const double* general = edge + 3 * h->fr_ne;
+  const double* planar_sub = general + 3 * h->fr_nn;
+  return submap_init_impl(h, scfg, edge, h->fr_ne, ground, h->fr_ng, planar_sub, h->fr_np_sub, general, h->fr_ns_sub, true);
+}
+
+int tloam_b200_submap_update_frame(tloam_b200_handle* h, const double pose[16]) {
+  if (!h || !pose) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->have_frame) return TLOAM_B200_ERR_NOT_READY;
+  return submap_update_impl(h, pose, h->d_frame + 3 * (h->fr_ng + h->fr_ne + h->fr_nn), h->fr_np_sub, true);
+}
+
+int tloam_b200_submap_update_frame_chained(tloam_b200_handle* h) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->have_frame) return TLOAM_B200_ERR_NOT_READY;
+  return submap_update_impl(h, nullptr, h->d_frame + 3 * (h->fr_ng + h->fr_ne + h->fr_nn), h->fr_np_sub, true);
 }
 
 int tloam_b200_host_alloc(void** p, size_t bytes) {

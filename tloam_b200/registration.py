@@ -464,6 +464,67 @@ class LocalRegistration:
         return dict(ground=g[:ng.value].copy(), edge=e[:ne.value].copy(), general=o[:no.value].copy(), sizes=sizes[:k].copy(),
                     boxes=boxes[:k].copy(), intensity=inten[:n].copy())
 
+    # ---- FrontEnd::processCloud on the device (ref: src/front_end/front_end.cpp:181-199) ----
+    def _submap_config(self, overrides):
+        cfg = _lib.SubmapConfig()
+        self._L.tloam_b200_submap_default_config(C.byref(cfg))
+        for k, v in overrides.items():
+            setattr(cfg, k, v)
+        return cfg
+
+    def process_cloud(self, ground, edge, general, ground_down_sample=0.3, edge_down_sample=0.1, **feature):
+        """VoxelDownSample(ground / edge), extractPlanarSphere(general) and the SelectByIndex gathers on the device; the four
+        features become the source (as set_input_source would).  feature: tloam_feature_config overrides.  Returns the four
+        source sizes (edge, sphere, planar, ground)."""
+        a = [_f64(x).reshape(-1, 3) for x in (ground, edge, general)]
+        c = self._feature_config(feature)
+        ns = (C.c_size_t * 4)()
+        self._check(self._L.tloam_b200_process_cloud(self._h, C.byref(c), float(ground_down_sample), float(edge_down_sample), _dp(a[0]),
+                                                     a[0].shape[0], _dp(a[1]), a[1].shape[0], _dp(a[2]), a[2].shape[0], ns),
+                    "process_cloud")
+        self.n_source = [int(v) for v in ns]
+        return list(self.n_source)
+
+    def process_raw_scan(self, scan, near_dis=3.0, ring_min_num=131, ground=None, dcvc=None, feature=None, ground_down_sample=0.3,
+                         edge_down_sample=0.1):
+        """segment_raw_scan -> process_cloud on the device with one upload of the raw scan and no index list going home.
+        ground / dcvc / feature: dicts of configuration overrides.  Returns the four source sizes."""
+        a = _f64(scan).reshape(-1, 3)
+        gc, dc = _lib.GroundConfig(), _lib.DcvcConfig()
+        self._L.tloam_b200_ground_default_config(C.byref(gc))
+        self._L.tloam_b200_dcvc_default_config(C.byref(dc))
+        for k, v in (ground or {}).items():
+            setattr(gc, k, v)
+        for k, v in (dcvc or {}).items():
+            setattr(dc, k, v)
+        fc = self._feature_config(feature or {})
+        ns = (C.c_size_t * 4)()
+        self._check(self._L.tloam_b200_process_raw_scan(self._h, C.byref(gc), C.byref(dc), ring_min_num, float(near_dis), C.byref(fc),
+                                                        float(ground_down_sample), float(edge_down_sample), _dp(a), a.shape[0], ns),
+                    "process_raw_scan")
+        self.n_source = [int(v) for v in ns]
+        return list(self.n_source)
+
+    def source_cloud(self, cloud):
+        """the current source cloud `cloud` (0 edge, 1 sphere, 2 planar, 3 ground), sensor frame"""
+        out = np.zeros((self.n_source[cloud], 3))
+        self._check(self._L.tloam_b200_source_download(self._h, cloud, _dp(out), out.shape[0]), "source_download")
+        return out
+
+    def submap_init_frame(self, **cfg_overrides):
+        """the first-frame seeding (ref: front_end.cpp:285-305) from the last processed frame"""
+        cfg = self._submap_config(cfg_overrides)
+        self._check(self._L.tloam_b200_submap_init_frame(self._h, C.byref(cfg)), "submap_init_frame")
+
+    def submap_update_frame(self, pose):
+        """submap_update with the last processed frame's planar-submap selection, read on the device"""
+        p = _f64(np.asarray(pose).T).reshape(16)
+        self._check(self._L.tloam_b200_submap_update_frame(self._h, _dp(p)), "submap_update_frame")
+
+    def submap_update_frame_chained(self):
+        """submap_update_chained with the last processed frame's planar-submap selection: no host input at all"""
+        self._check(self._L.tloam_b200_submap_update_frame_chained(self._h), "submap_update_frame_chained")
+
     # ---- shared map (multi-GPU) ----
     def map_blob_size(self):
         n = C.c_size_t(0)

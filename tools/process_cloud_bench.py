@@ -1,0 +1,113 @@
+"""FrontEnd::processCloud on the device, on a 116k-point synthetic HDL-64E raw scan (the street scene of synth.raw_scan):
+  (a) one tloam_b200_process_cloud call on the scan's segmented ground / edge / general clouds (host clouds in);
+  (b) one tloam_b200_process_raw_scan call (raw scan in, nothing but counts out);
+  (c) the host-glue path (b) replaces: segment_raw_scan, numpy gathers, voxel_down_sample x 2, extract_planar_sphere, numpy
+      gathers, set_input_source;
+  (d) frames/s of the per-frame loop process_raw_scan -> scan_match_predicted_async -> submap_update_frame_chained ->
+      get_result against the same loop with the host glue of (c) and submap_update_chained.
+It checks that (b) and (c) give the same source apart from the voxel order and the fixed-point voxel averages (planar /
+sphere bit-identical, ground / edge the same rows to 1e-10 m), and prints the card and its power limit with the numbers.
+
+    python tools/process_cloud_bench.py [reps]
+"""
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
+sys.path.insert(0, ROOT)
+import tloam_b200  # noqa: E402
+from tloam_b200 import synth  # noqa: E402
+
+FE = dict(cvr_submap=0.005, cvr_scan=0.01)        # the street scene has few curvature maxima (tests/test_front_end_chain.py)
+
+
+def host_glue(reg, raw):
+    """(c): what a caller does today to turn a raw scan into the registration source; returns the planar-submap selection"""
+    s = reg.segment_raw_scan(raw)
+    ground, edge, general = (np.ascontiguousarray(raw[s[k]]) for k in ("ground", "edge", "general"))
+    g = reg.voxel_down_sample(ground, 0.3)
+    e = reg.voxel_down_sample(edge, 0.1)
+    p_scan, p_sub, s_scan, s_sub, _ = reg.extract_planar_sphere(general, **FE)
+    reg.set_input_source([e, general[:len(s_scan)], general[p_scan], g])          # sphere: the rank list taken literally (Q12)
+    return general[p_sub]
+
+
+def timed(fn, reps):
+    fn()
+    passes = []
+    for _ in range(3):
+        t0 = time.perf_counter()
+        for _ in range(reps):
+            fn()
+        passes.append(1e3 * (time.perf_counter() - t0) / reps)           # every call ends in a synchronisation
+    return float(np.median(passes)), passes
+
+
+def sorted_rows(a):
+    return a[np.lexsort(a.T[::-1])]
+
+
+def main():
+    reps = int(sys.argv[1]) if len(sys.argv) > 1 else 20
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    raw = synth.raw_scan()
+    reg = tloam_b200.LocalRegistration()
+    s = reg.segment_raw_scan(raw)
+    clouds = [np.ascontiguousarray(raw[s[k]]) for k in ("ground", "edge", "general")]
+    res = {"gpu": card, "raw_points": int(len(raw)), "ground": len(clouds[0]), "edge": len(clouds[1]), "general": len(clouds[2])}
+    res["a_process_cloud_ms"], _ = timed(lambda: reg.process_cloud(*clouds, **FE), reps)
+    res["b_process_raw_scan_ms"], _ = timed(lambda: reg.process_raw_scan(raw, feature=FE), reps)
+    res["source_sizes"] = reg.process_raw_scan(raw, feature=FE)
+    dev = [reg.source_cloud(c) for c in range(4)]
+    res["c_host_glue_ms"], _ = timed(lambda: host_glue(reg, raw), reps)
+    host_glue(reg, raw)
+    host = [reg.source_cloud(c) for c in range(4)]
+    same = np.array_equal(dev[1], host[1]) and np.array_equal(dev[2], host[2])
+    for c in (0, 3):
+        a, b = sorted_rows(dev[c]), sorted_rows(host[c])
+        same = same and a.shape == b.shape and bool(np.allclose(a, b, rtol=0, atol=1e-10))
+    res["b_equals_c_up_to_voxel_order"] = bool(same)
+
+    # (d) the per-frame loop over rigid motions of the scan, seeded from frame 0
+    xis = [np.array([0.3 * k, 0.02 * k, 0.0, 0.0, 0.0, 0.004 * k]) for k in range(reps + 1)]
+    scans = [raw]
+    for k in range(1, reps + 1):
+        Ti = np.linalg.inv(synth.se3_exp(xis[k]))
+        scans.append(np.ascontiguousarray(raw @ Ti[:3, :3].T + Ti[:3, 3]))
+    prev = synth.se3_exp(-xis[1])
+    for mode in ("device", "host_glue"):
+        r = tloam_b200.LocalRegistration(fitness_thres=0.3)
+        if mode == "device":
+            r.process_raw_scan(scans[0], feature=FE)
+            r.submap_init_frame()
+        else:
+            s0 = r.segment_raw_scan(scans[0])
+            ground, edge, general = (np.ascontiguousarray(scans[0][s0[k]]) for k in ("ground", "edge", "general"))
+            p_scan, p_sub, s_scan, s_sub, _ = r.extract_planar_sphere(general, **FE)
+            r.submap_init(edge, ground, general[p_sub], general[:len(s_sub)])
+        r.set_pose_history(prev, np.eye(4))
+        t0 = time.perf_counter()
+        for sc in scans[1:]:
+            if mode == "device":
+                r.process_raw_scan(sc, feature=FE)
+                r.scan_matching_predicted_async()
+                r.submap_update_frame_chained()
+            else:
+                planar_sub = host_glue(r, sc)
+                r.scan_matching_predicted_async()
+                r.submap_update_chained(planar_sub)
+            T = r.get_result()
+        res[f"d_{mode}_frames_per_s"] = reps / (time.perf_counter() - t0)
+        res[f"d_{mode}_last_pose_t"] = [float(v) for v in T[:3, 3]]
+        r.close()
+    reg.close()
+    print(json.dumps(res))
+
+
+if __name__ == "__main__":
+    main()
