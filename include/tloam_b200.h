@@ -57,7 +57,8 @@ typedef enum tloam_b200_status {
   TLOAM_B200_ERR_NO_DEVICE = 5,
   TLOAM_B200_ERR_NOT_READY = 6,      /* scan_match before set_source / set_target */
   TLOAM_B200_ERR_NUMERIC = 7,        /* non-finite value met inside the solve */
-  TLOAM_B200_ERR_MAP_DENSITY = 8     /* a map cell (edge = search radius) holds more than 65535 points */
+  TLOAM_B200_ERR_MAP_DENSITY = 8,    /* a map cell (edge = search radius) holds more than 65535 points */
+  TLOAM_B200_ERR_VOXEL_RANGE = 9     /* a global-map frame spans 2^21 or more voxels on an axis (voxel too small): not appended */
 } tloam_b200_status;
 
 /* The "TLS:" YAML block (ref: config/mapping/lidar_odometry.yaml:23-39, read at registration.cpp:212-230)
@@ -451,6 +452,50 @@ int tloam_b200_submap_init_frame(tloam_b200_handle* h, const tloam_submap_config
  * device.  NOT_READY before any processed frame. */
 int tloam_b200_submap_update_frame(tloam_b200_handle* h, const double pose[16]);
 int tloam_b200_submap_update_frame_chained(tloam_b200_handle* h);
+
+/* ---- Global map (FrontEnd::updateSubmap with mapping_flag, ref: src/front_end/front_end.cpp:269-274): every appended
+ * raw scan is transformed by its pose, voxel-down-sampled ON ITS OWN and concatenated to a map kept on the device:
+ *     global_map += raw.Transform(pose).VoxelDownSample(voxel)
+ *   - Frames are never merged: each is down-sampled on its own grid (min bound of its transformed finite rows - voxel/2).
+ *     Its voxels come out in ascending voxel index (ix, iy, iz), with the fixed-point averages of
+ *     tloam_b200_voxel_down_sample; frames follow in call order.  The map is fully deterministic.
+ *   - Non-finite rows are left out of the map (the reference feeds them to GetMinBound / floor: undefined behaviour).
+ *   - The registered scan is T.p of every raw row, in raw order (non-finite rows stay non-finite).  The reference with
+ *     mapping_flag on publishes T.T.p (Transform works in place); T.p is what it publishes with mapping_flag off.
+ *   - The first frame of FrontEnd is not in the reference's map (front_end.cpp:285-305 returns before updateSubmap):
+ *     append from frame 1 on to restate it.
+ *   - Appends are enqueued on the handle's stream with no host round trip; the host sizes the map from an upper bound
+ *     and synchronises only when the buffer has to grow (x1.5).  A frame whose finite extent reaches 2^21 voxels on an
+ *     axis is refused on the device (map unchanged); the next call below that synchronises returns VOXEL_RANGE once.
+ *   - Mapping is off until tloam_b200_global_map_enable; with it off none of this launches anything. */
+typedef struct tloam_global_map_config {
+  double voxel;                        /* VoxelDownSample size of every frame (the reference's literal 1.0) */
+  size_t initial_capacity_points;      /* map buffer before the first growth */
+} tloam_global_map_config;
+void tloam_b200_global_map_default_config(tloam_global_map_config* c);
+/* (re)starts an empty map with this configuration.  INVALID_ARG: cfg null, voxel <= 0 or not finite. */
+int tloam_b200_global_map_enable(tloam_b200_handle* h, const tloam_global_map_config* cfg);
+/* empties the map and forgets the registered scan (the configuration and the buffers stay).  NOT_READY if not enabled. */
+int tloam_b200_global_map_reset(tloam_b200_handle* h);
+/* appends a HOST raw cloud (n x 3 FP64 AoS, may hold NaN / Inf rows) with pose[16] (column-major, host) or, _chained, the
+ * pose of the frame just enqueued on the handle (tloam_b200_scan_match_predicted_async).  n == 0 appends an empty frame. */
+int tloam_b200_global_map_append(tloam_b200_handle* h, const double pose[16], const double* xyz, size_t n);
+int tloam_b200_global_map_append_chained(tloam_b200_handle* h, const double* xyz, size_t n);
+/* the same for the raw scan that the last tloam_b200_process_raw_scan uploaded (no upload).  NOT_READY when there is none,
+ * or when any segmentation or process call has run since (its buffer may have been reused). */
+int tloam_b200_global_map_append_frame(tloam_b200_handle* h, const double pose[16]);
+int tloam_b200_global_map_append_frame_chained(tloam_b200_handle* h);
+/* exact points and frames in the map (synchronises); returns VOXEL_RANGE once after a refused frame */
+int tloam_b200_global_map_size(tloam_b200_handle* h, size_t* n_points, size_t* n_frames);
+/* map points [first, first + count) to out (count x 3 FP64, synchronises).  INVALID_ARG past the end. */
+int tloam_b200_global_map_download(tloam_b200_handle* h, size_t first, size_t count, double* out);
+/* offsets[0 .. n_frames]: the first point of every frame, then the map size (capacity >= n_frames + 1, synchronises) */
+int tloam_b200_global_map_frame_offsets(tloam_b200_handle* h, size_t* offsets, size_t capacity);
+/* map buffer capacity in points and the number of growths since enable (each growth synchronised once) */
+int tloam_b200_global_map_capacity(tloam_b200_handle* h, size_t* capacity_points, size_t* growths);
+/* T.p of every row of the last append, raw order, to out (synchronises).  *n receives the row count; NOT_READY before the
+ * first append, INVALID_ARG if capacity_points < *n. */
+int tloam_b200_registered_scan_download(tloam_b200_handle* h, double* out, size_t capacity_points, size_t* n);
 
 /* Pinned host memory helpers (optional; pinned inputs make set_* a direct DMA, no staging threads). */
 int tloam_b200_host_alloc(void** p, size_t bytes);

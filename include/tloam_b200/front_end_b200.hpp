@@ -9,6 +9,9 @@
 //     updateSubmap(pose)                      replaces updateSubmap() + setInputTarget(submap)
 // and on the first frame processCloud + initSubmap() replace the `!odometry_inited` branch.  The scan features, the frame's
 // submap selections and the submap itself stay on the GPU; the caller reads a source cloud back only to inspect it.
+// With mapping_flag (ref: front_end.cpp:57, :269-274) updateGlobalMap(raw, pose) after updateSubmap appends the frame's raw
+// scan, transformed and VoxelDownSample(1.0)'d on its own, to a global map kept on the GPU (globalMap / registeredScan read
+// it back); frame 0 has no append, as in the reference.
 // Without the reference headers (this repository's tests) define TLOAM_B200_MOCK_HOST_TYPES and provide the host types
 // (tests/mock/mock_tloam.hpp).
 #ifndef TLOAM_B200_FRONT_END_B200_HPP
@@ -63,8 +66,44 @@ class FrontEndB200 {
     fcfg_.planar_scan_thres = fe["planar_scan_thres"].as<double>();
     fcfg_.planar_submap_thres = fe["planar_submap_thres"].as<double>();
     fcfg_.planar_vertic_thres = fe["planar_vertic_thres"].as<double>();
+    if (lo["mapping_flag"].as<bool>()) enableGlobalMap();   // front_end.cpp:57
   }
 #endif
+
+  // mapping_flag on: an empty global map with VoxelDownSample(voxel) per frame (the reference's literal 1.0)
+  bool enableGlobalMap(double voxel = 1.0) {
+    tloam_global_map_config c;
+    tloam_b200_global_map_default_config(&c);
+    c.voxel = voxel;
+    mapping_ = report(tloam_b200_global_map_enable(h_, &c), "enableGlobalMap");
+    return mapping_;
+  }
+  bool mappingFlag() const { return mapping_; }
+  // global_map += raw.Transform(pose).VoxelDownSample(voxel) (ref: front_end.cpp:269-274): raw = the driver's scan, NaN rows
+  // allowed (left out of the map).  No-ops returning true when mapping is off, like the reference.
+  bool updateGlobalMap(const CloudData& raw, const Eigen::Isometry3d& pose) {
+    if (!mapping_) return true;
+    return report(tloam_b200_global_map_append(h_, pose.matrix().data(), data(raw), size(raw)), "updateGlobalMap");
+  }
+  // the same with the pose of the frame just enqueued on the handle (tloam_b200_scan_match_predicted_async)
+  bool updateGlobalMapChained(const CloudData& raw) {
+    if (!mapping_) return true;
+    return report(tloam_b200_global_map_append_chained(h_, data(raw), size(raw)), "updateGlobalMapChained");
+  }
+  // the whole map (synchronises) and T.p of the last appended raw scan, raw order (the reference's /raw_cloud, :84-86)
+  bool globalMap(std::vector<Eigen::Vector3d>& out) {
+    size_t n = 0, frames = 0;
+    if (!report(tloam_b200_global_map_size(h_, &n, &frames), "globalMap")) return false;
+    out.resize(n);
+    return report(tloam_b200_global_map_download(h_, 0, n, reinterpret_cast<double*>(out.data())), "globalMap");
+  }
+  bool registeredScan(std::vector<Eigen::Vector3d>& out) {
+    size_t n = 0;
+    const int rc = tloam_b200_registered_scan_download(h_, nullptr, 0, &n);
+    if (rc != TLOAM_B200_OK && rc != TLOAM_B200_ERR_INVALID_ARG) return report(rc, "registeredScan");
+    out.resize(n);
+    return report(tloam_b200_registered_scan_download(h_, reinterpret_cast<double*>(out.data()), out.size(), &n), "registeredScan");
+  }
 
   // processCloud + setInputSource (ref: front_end.cpp:181-199, :313): the three clouds the segmentation nodelet publishes
   bool processCloud(CloudData& ground, CloudData& edge, CloudData& general) {
@@ -106,6 +145,7 @@ class FrontEndB200 {
   tloam_submap_config scfg_;
   double ground_down_sample_ = 0.3, edge_down_sample_ = 0.1;
   size_t n_source_[4] = {0, 0, 0, 0};
+  bool mapping_ = false;
   int last_status_ = TLOAM_B200_OK;
 };
 

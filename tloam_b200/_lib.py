@@ -9,7 +9,8 @@ LIB_PATH = os.environ.get("TLOAM_B200_LIB") or os.path.join(HERE, "libtloam_b200
 MAX_OUTER = 16
 MAX_INNER = 8
 
-OK, ERR_INVALID_ARG, ERR_TOO_FEW_POINTS, ERR_BAD_POSE, ERR_CUDA, ERR_NO_DEVICE, ERR_NOT_READY, ERR_NUMERIC, ERR_MAP_DENSITY = range(9)
+(OK, ERR_INVALID_ARG, ERR_TOO_FEW_POINTS, ERR_BAD_POSE, ERR_CUDA, ERR_NO_DEVICE, ERR_NOT_READY, ERR_NUMERIC, ERR_MAP_DENSITY,
+ ERR_VOXEL_RANGE) = range(10)
 
 
 class TlsConfig(C.Structure):
@@ -34,6 +35,11 @@ class SubmapConfig(C.Structure):
     _fields_ = [("ground_down_sample", C.c_double), ("ground_down_sample_submap", C.c_double),
                 ("edge_down_sample_submap", C.c_double), ("planar_frame_size", C.c_int), ("sphere_frame_size", C.c_int),
                 ("edge_crop_box_length", C.c_double), ("ground_crop_box_length", C.c_double)]
+
+
+class GlobalMapConfig(C.Structure):
+    """tloam_global_map_config (the reference's global map: front_end.cpp:269-274, VoxelDownSample(1.0))."""
+    _fields_ = [("voxel", C.c_double), ("initial_capacity_points", C.c_size_t)]
 
 
 class InnerTrace(C.Structure):
@@ -121,6 +127,10 @@ EXPORTS = [
     "tloam_b200_map_send_buffer", "tloam_b200_map_recv_buffer", "tloam_b200_map_adopt", "tloam_b200_signal_stream",
     "tloam_b200_process_cloud", "tloam_b200_process_raw_scan", "tloam_b200_source_download", "tloam_b200_submap_init_frame",
     "tloam_b200_submap_update_frame", "tloam_b200_submap_update_frame_chained",
+    "tloam_b200_global_map_default_config", "tloam_b200_global_map_enable", "tloam_b200_global_map_reset",
+    "tloam_b200_global_map_append", "tloam_b200_global_map_append_chained", "tloam_b200_global_map_append_frame",
+    "tloam_b200_global_map_append_frame_chained", "tloam_b200_global_map_size", "tloam_b200_global_map_download",
+    "tloam_b200_global_map_frame_offsets", "tloam_b200_global_map_capacity", "tloam_b200_registered_scan_download",
 ]
 
 _lib = None
@@ -244,5 +254,18 @@ def load():
     L.tloam_b200_submap_init_frame.argtypes = [vp, C.POINTER(SubmapConfig)]
     L.tloam_b200_submap_update_frame.argtypes = [vp, dp]
     L.tloam_b200_submap_update_frame_chained.argtypes = [vp]
+    L.tloam_b200_global_map_default_config.argtypes = [C.POINTER(GlobalMapConfig)]
+    L.tloam_b200_global_map_default_config.restype = None
+    L.tloam_b200_global_map_enable.argtypes = [vp, C.POINTER(GlobalMapConfig)]
+    L.tloam_b200_global_map_reset.argtypes = [vp]
+    L.tloam_b200_global_map_append.argtypes = [vp, dp, dp, C.c_size_t]
+    L.tloam_b200_global_map_append_chained.argtypes = [vp, dp, C.c_size_t]
+    L.tloam_b200_global_map_append_frame.argtypes = [vp, dp]
+    L.tloam_b200_global_map_append_frame_chained.argtypes = [vp]
+    L.tloam_b200_global_map_size.argtypes = [vp, szp, szp]
+    L.tloam_b200_global_map_download.argtypes = [vp, C.c_size_t, C.c_size_t, dp]
+    L.tloam_b200_global_map_frame_offsets.argtypes = [vp, szp, C.c_size_t]
+    L.tloam_b200_global_map_capacity.argtypes = [vp, szp, szp]
+    L.tloam_b200_registered_scan_download.argtypes = [vp, dp, C.c_size_t, szp]
     _lib = L
     return L

@@ -199,4 +199,110 @@ __global__ void k_set_counts(unsigned* cnt, int c0, unsigned n0, int c1, unsigne
   if (threadIdx.x == 0) { if (c0 >= 0) cnt[c0] = n0; if (c1 >= 0) cnt[c1] = n1; }
 }
 
+// ---- global map (FrontEnd::updateSubmap with mapping_flag, ref: front_end.cpp:269-274):
+//        curr_map = raw.Transform(pose); global_map += curr_map->VoxelDownSample(voxel)
+// per frame on the handle's stream: k_gmap_transform (T.p of every raw row + the finite rows compacted + their bounds) ->
+// k_gmap_guard (key range) -> voxel_pipeline(sorted) over the finite rows -> k_gmap_emit (ascending key, at the map's
+// device-side end) -> k_gmap_commit (count, frame table).  No host round trip: the map's size lives in GMapState.
+struct GMapState {
+  unsigned long long count;       // points in the map
+  unsigned long long frames;      // frames in the map (offsets[0 .. frames] are valid)
+  unsigned flags;                 // sticky until the host reads it: kGMapKeyRange | kGMapOverflow
+  // ---- per frame (cleared by one memset before k_gmap_transform) ----
+  unsigned n_fin;                 // finite rows compacted into the voxel input (0 when the frame is refused)
+  unsigned n_vox;                 // voxels of the frame (voxel_pipeline's out_count)
+  unsigned refused;
+  unsigned long long lo[3];       // complemented ordered encodings of the finite rows' min (0 = none yet)
+  unsigned long long hi[3];       // ordered encodings of their max (0 = none yet)
+};
+constexpr unsigned kGMapKeyRange = 1u, kGMapOverflow = 2u;
+constexpr unsigned kGMapKeyBits = 21;   // per axis of the packed voxel key (cell_key)
+
+// reg[i] = T.p_i for every row (non-finite rows stay non-finite, like Transform); the finite rows also go to fin[] (order
+// irrelevant: the voxel sums are fixed point and the emission is sorted), with their count and bounds in st.
+// Same expression as k_transform_append, so both transforms round alike.  in may alias reg (each thread reads its row first).
+__global__ void __launch_bounds__(256) k_gmap_transform(const double* in, unsigned n, const double* pose, double* reg, double* fin,
+                                                        GMapState* st) {
+  const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+  double p[3] = {0.0, 0.0, 0.0};
+  bool ok = false;
+  if (i < n) {
+    const double x = in[3ull * i], y = in[3ull * i + 1], z = in[3ull * i + 2];
+    p[0] = pose[0] * x + pose[4] * y + pose[8] * z + pose[12];
+    p[1] = pose[1] * x + pose[5] * y + pose[9] * z + pose[13];
+    p[2] = pose[2] * x + pose[6] * y + pose[10] * z + pose[14];
+    reg[3ull * i] = p[0]; reg[3ull * i + 1] = p[1]; reg[3ull * i + 2] = p[2];
+    ok = isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]);
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned b = __ballot_sync(0xffffffffu, ok);
+  unsigned base = 0u;
+  if (lane == 0 && b) base = atomicAdd(&st->n_fin, (unsigned)__popc(b));
+  base = __shfl_sync(0xffffffffu, base, 0);
+  if (ok) {
+    const unsigned j = base + __popc(b & ((1u << lane) - 1u));
+    fin[3ull * j] = p[0]; fin[3ull * j + 1] = p[1]; fin[3ull * j + 2] = p[2];
+  }
+  double mn[3], mx[3];
+#pragma unroll
+  for (int d = 0; d < 3; ++d) { mn[d] = ok ? p[d] : DBL_MAX; mx[d] = ok ? p[d] : -DBL_MAX; }
+#pragma unroll
+  for (int d = 0; d < 3; ++d)
+    for (int o = 16; o > 0; o >>= 1) {
+      mn[d] = fmin(mn[d], __shfl_xor_sync(0xffffffffu, mn[d], o));
+      mx[d] = fmax(mx[d], __shfl_xor_sync(0xffffffffu, mx[d], o));
+    }
+  __shared__ double s_b[8][6];
+  __shared__ unsigned s_any;
+  if (threadIdx.x == 0) s_any = 0u;
+  __syncthreads();
+  if (lane == 0) {
+    for (int d = 0; d < 3; ++d) { s_b[warp][d] = mn[d]; s_b[warp][3 + d] = mx[d]; }
+    if (b) atomicOr(&s_any, 1u);
+  }
+  __syncthreads();
+  if (threadIdx.x < 6 && s_any) {
+    const int d = threadIdx.x;
+    double v = s_b[0][d];
+    for (int wi = 1; wi < 8; ++wi) v = d < 3 ? fmin(v, s_b[wi][d]) : fmax(v, s_b[wi][d]);
+    if (d < 3) atomicMax(&st->lo[d], ~enc_ordered(v));
+    else atomicMax(&st->hi[d - 3], enc_ordered(v));
+  }
+}
+
+// a frame whose finite extent reaches 2^21 voxels on an axis cannot be keyed (the reference's "voxel_size is too small"):
+// it is refused -- no voxel input, no append -- and the sticky flag reports it.  floor((p - min_bound) / voxel) as in
+// k_vox_accum is monotone in p, so the max row gives the largest index.
+__global__ void k_gmap_guard(GMapState* st, double voxel) {
+  if (threadIdx.x != 0 || st->n_fin == 0u) return;
+  bool bad = false;
+  for (int d = 0; d < 3; ++d) {
+    const double mb = dec_ordered(~st->lo[d]) - voxel * 0.5;
+    const double ref = (dec_ordered(st->hi[d]) - mb) / voxel;
+    bad |= !(ref < (double)(1u << kGMapKeyBits));
+  }
+  if (bad) { st->refused = 1u; st->n_fin = 0u; st->flags |= kGMapKeyRange; }
+}
+
+// map[count + j] = the average of the j-th voxel in key order (k_vox_emit_sorted with the output base read on the device);
+// nothing is written unless the whole frame fits below cap (k_gmap_commit then flags the overflow)
+__global__ void __launch_bounds__(256) k_gmap_emit(VoxArgs a, const unsigned* slot_sorted, double* map, const GMapState* st,
+                                                   unsigned long long cap) {
+  const unsigned j = blockIdx.x * blockDim.x + threadIdx.x;
+  const unsigned nv = *a.out_count;
+  if (j >= nv || st->refused || st->count + nv > cap) return;
+  const unsigned s = slot_sorted[j];
+  vox_average(a, s, a.cnt[s], map + 3ull * (st->count + j));
+}
+
+// offsets[f] = first point of frame f; offsets[frames] = count
+__global__ void k_gmap_commit(GMapState* st, unsigned long long* offsets, unsigned long long cap, unsigned long long frame_cap) {
+  if (threadIdx.x != 0 || st->refused) return;
+  const unsigned long long end = st->count + st->n_vox;
+  if (end > cap || st->frames + 1ull >= frame_cap) { st->flags |= kGMapOverflow; return; }
+  st->count = end;
+  st->frames += 1ull;
+  offsets[st->frames] = end;
+}
+
 }  // namespace tloam

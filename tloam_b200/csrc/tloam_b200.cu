@@ -179,6 +179,25 @@ struct tloam_b200_handle {
   bool fe_sort_attr_set = false, ge_attr_set = false, ee_attr_set = false, os_attr_set = false;   // per handle: function attributes are per device
   bool dense_check = false;                // TLOAM_B200_DENSE_CHECK=1: every dense query is re-searched by the plain path and compared
   int num_sms = 132;                       // H100 SXM; replaced by the device's count at create
+  // ---- the raw scan of the last tloam_b200_process_raw_scan (in d_chain): valid while no segmentation / process call
+  //      has run since, i.e. while seg_gen == raw_gen ----
+  unsigned long long seg_gen = 0, raw_gen = ~0ull;
+  const double* raw_scan = nullptr;        size_t raw_n = 0;
+  // ---- global map (tloam_b200_global_map_*, submap.cuh): nothing is allocated or launched until it is enabled ----
+  bool gmap_on = false;
+  double gmap_voxel = 1.0;
+  GMapState* d_gmap_st = nullptr;
+  double* d_gmap_pose = nullptr;
+  double* d_gmap = nullptr;                size_t cap_gmap = 0;                                 // map points
+  unsigned long long* d_gmap_off = nullptr; size_t cap_gmap_off = 0;                            // frame table entries
+  double* d_gmap_reg = nullptr;            size_t cap_gmap_reg = 0, gmap_reg_n = 0; bool gmap_reg_valid = false;
+  double* d_gmap_fin = nullptr;            size_t cap_gmap_fin = 0;                             // finite rows (voxel input)
+  // the host's upper bound of the map size = gmap_known (an exact count, read asynchronously) + the rows appended since
+  // (gmap_cum - gmap_known_cum); gmap_calls bounds the frame count
+  unsigned long long gmap_cum = 0, gmap_known_cum = 0, gmap_known = 0, gmap_calls = 0;
+  size_t gmap_growths = 0;
+  struct GMapProbe { cudaEvent_t ev = nullptr; unsigned long long* h_count = nullptr; unsigned long long cum = 0; bool pending = false; };
+  GMapProbe gmap_probes[4];                int gmap_probe_next = 0;
 };
 
 // launch bookkeeping: counts the kernel and, in profiling mode, brackets it with events
@@ -233,6 +252,7 @@ const char* tloam_b200_status_string(int s) {
     case TLOAM_B200_ERR_NOT_READY: return "source or target not set";
     case TLOAM_B200_ERR_NUMERIC: return "non-finite value in the solve";
     case TLOAM_B200_ERR_MAP_DENSITY: return "a map cell holds more than 65535 points";
+    case TLOAM_B200_ERR_VOXEL_RANGE: return "a global-map frame spans 2^21 or more voxels on an axis (voxel size too small)";
     default: return "unknown status";
   }
 }
@@ -370,6 +390,9 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   if (h->ev_planar_free) cudaEventDestroy(h->ev_planar_free);
   if (h->ev_planar_done) cudaEventDestroy(h->ev_planar_done);
   cudaFree(h->d_vox1); cudaFree(h->d_acc_tmp1); cudaFree(h->d_up_planar); cudaFree(h->d_chain); cudaFree(h->d_frame);
+  cudaFree(h->d_gmap_st); cudaFree(h->d_gmap_pose); cudaFree(h->d_gmap); cudaFree(h->d_gmap_off); cudaFree(h->d_gmap_reg);
+  cudaFree(h->d_gmap_fin);
+  for (auto& pr : h->gmap_probes) { if (pr.ev) cudaEventDestroy(pr.ev); if (pr.h_count) cudaFreeHost(pr.h_count); }
   for (int i = 0; i < 2; ++i) if (h->ev_stage_free[i]) cudaEventDestroy(h->ev_stage_free[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_fit[i]) cudaEventDestroy(h->ev_fit[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_res[i]) cudaEventDestroy(h->ev_res[i]);
@@ -2373,6 +2396,7 @@ static int ground_run(tloam_b200_handle* h, const tloam_ground_config* cfg, cons
                       size_t* n_ground, size_t* object_index, size_t* n_object, int* beam, double* intensity, int* region,
                       double* height_threshold, double* planes) {
   if (!h || !cfg || !ground_index || !n_ground || !object_index || !n_object) return TLOAM_B200_ERR_INVALID_ARG;
+  h->seg_gen++;                                                            // the last raw scan may no longer be in place
   *n_ground = *n_object = 0;
   if ((cfg->sensor_model != 64 && cfg->sensor_model != 16) || cfg->quadrant != 4 || cfg->num_sec < 1 || cfg->num_sec > 3 ||
       cfg->max_iter < 1 || cfg->max_iter > kGeMaxIter || cfg->ground_seed_num < 1)
@@ -2470,6 +2494,7 @@ int tloam_b200_ground_extract(tloam_b200_handle* h, const tloam_ground_config* c
 int tloam_b200_extract_edge(tloam_b200_handle* h, int sensor_model, int ring_min_num, const double* xyz, const double* intensity,
                             size_t n, size_t* edge_index, size_t* n_edge, size_t* non_edge_index, size_t* n_non_edge) {
   if (!h || !edge_index || !n_edge || !non_edge_index || !n_non_edge) return TLOAM_B200_ERR_INVALID_ARG;
+  h->seg_gen++;
   *n_edge = *n_non_edge = 0;
   if (sensor_model < 1 || sensor_model > kEeKeys || ring_min_num < 0) return TLOAM_B200_ERR_INVALID_ARG;
   if (n == 0) return TLOAM_B200_OK;                                        // ref: :1222-1225 (empty input: nothing extracted)
@@ -2550,6 +2575,7 @@ int tloam_b200_object_segmentation(tloam_b200_handle* h, const tloam_dcvc_config
                                    size_t* seg_index, size_t* n_seg, int* n_clusters, int* sizes, double* boxes, int* root,
                                    int* cluster, int* voxel, double* polar) {
   if (!h || !cfg || !seg_index || !n_seg || !n_clusters) return TLOAM_B200_ERR_INVALID_ARG;
+  h->seg_gen++;
   *n_seg = 0; *n_clusters = 0;
   if (!(cfg->delta_p > 0.0) || !(cfg->delta_a > 0.0)) return TLOAM_B200_ERR_INVALID_ARG;
   if (n == 0) return TLOAM_B200_OK;                                         // ref: :1088-1093 (nothing to convert)
@@ -2719,6 +2745,7 @@ static int segment_chain(tloam_b200_handle* h, const tloam_ground_config* gcfg, 
                          double* intensity, ChainKeep* keep = nullptr) {
   if (!h || !gcfg || !dcfg || !ground_index || !n_ground || !edge_index || !n_edge || !general_index || !n_general || !n_clusters)
     return TLOAM_B200_ERR_INVALID_ARG;
+  h->seg_gen++;                                           // d_chain (the raw scan of the last process_raw_scan) is rewritten
   *n_ground = *n_edge = *n_general = 0; *n_clusters = 0;
   if (remove && gcfg->sensor_model != 64 && gcfg->sensor_model != 16) return TLOAM_B200_ERR_INVALID_ARG;
   if (n == 0) return TLOAM_B200_OK;
@@ -2911,6 +2938,7 @@ int tloam_b200_process_cloud(tloam_b200_handle* h, const tloam_feature_config* f
                              const double* ground, size_t ng, const double* edge, size_t ne, const double* general, size_t nn,
                              size_t n_source[4]) {
   if (!h || !fcfg || !n_source || (!ground && ng) || (!edge && ne) || (!general && nn)) return TLOAM_B200_ERR_INVALID_ARG;
+  h->seg_gen++;                                           // the last raw scan no longer belongs to the processed frame
   for (int k = 0; k < 4; ++k) n_source[k] = 0;
   if (!(ground_down_sample > 0.0) || !(edge_down_sample > 0.0)) return TLOAM_B200_ERR_INVALID_ARG;
   if (ng > ((size_t)1 << 30) || ne > ((size_t)1 << 30) || nn > ((size_t)1 << 30)) return TLOAM_B200_ERR_INVALID_ARG;
@@ -2958,7 +2986,9 @@ int tloam_b200_process_raw_scan(tloam_b200_handle* h, const tloam_ground_config*
     off += cnt[c];
   }
   CU_TRY(cudaGetLastError());
-  return process_frame(h, fcfg, ground_down_sample, edge_down_sample, ng, ne, nn, n_source);
+  if ((rc = process_frame(h, fcfg, ground_down_sample, edge_down_sample, ng, ne, nn, n_source)) != TLOAM_B200_OK) return rc;
+  h->raw_scan = keep.scan; h->raw_n = n; h->raw_gen = h->seg_gen;   // for tloam_b200_global_map_append_frame*
+  return TLOAM_B200_OK;
 }
 
 int tloam_b200_source_download(tloam_b200_handle* h, int cloud, double* out, size_t capacity_points) {
@@ -2992,6 +3022,259 @@ int tloam_b200_submap_update_frame_chained(tloam_b200_handle* h) {
   if (!h) return TLOAM_B200_ERR_INVALID_ARG;
   if (!h->have_frame) return TLOAM_B200_ERR_NOT_READY;
   return submap_update_impl(h, nullptr, h->d_frame + 3 * (h->fr_ng + h->fr_ne + h->fr_nn), h->fr_np_sub, true);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Global map (FrontEnd::updateSubmap with mapping_flag, ref: front_end.cpp:269-274; kernels in submap.cuh).  Every append
+// is enqueued on the handle's stream.  The map's size stays on the device; the host keeps an upper bound (an exact count
+// read back asynchronously, plus the rows appended since) and synchronises only to grow the buffer.
+// ---------------------------------------------------------------------------------------------
+void tloam_b200_global_map_default_config(tloam_global_map_config* c) {
+  c->voxel = 1.0;                          // front_end.cpp:273: VoxelDownSample(1.0)
+  c->initial_capacity_points = (size_t)1 << 20;
+}
+
+static void gmap_harvest(tloam_b200_handle* h) {
+  for (auto& pr : h->gmap_probes) {
+    if (!pr.pending) continue;
+    if (cudaEventQuery(pr.ev) != cudaSuccess) { cudaGetLastError(); continue; }
+    pr.pending = false;
+    if (pr.cum >= h->gmap_known_cum) { h->gmap_known_cum = pr.cum; h->gmap_known = *pr.h_count; }
+  }
+}
+
+static int gmap_clear(tloam_b200_handle* h) {
+  CU_TRY(cudaMemsetAsync(h->d_gmap_st, 0, sizeof(GMapState), h->stream));
+  CU_TRY(cudaMemsetAsync(h->d_gmap_off, 0, sizeof(unsigned long long), h->stream));
+  h->gmap_cum = h->gmap_known_cum = h->gmap_known = h->gmap_calls = 0;
+  for (auto& pr : h->gmap_probes) pr.pending = false;
+  h->gmap_reg_valid = false; h->gmap_reg_n = 0;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_global_map_enable(tloam_b200_handle* h, const tloam_global_map_config* cfg) {
+  if (!h || !cfg || !(cfg->voxel > 0.0) || !std::isfinite(cfg->voxel)) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (!h->d_gmap_st) {
+    CU_TRY(cudaMalloc(&h->d_gmap_st, sizeof(GMapState)));
+    CU_TRY(cudaMalloc(&h->d_gmap_pose, 16 * sizeof(double)));
+    for (auto& pr : h->gmap_probes) {
+      CU_TRY(cudaEventCreateWithFlags(&pr.ev, cudaEventDisableTiming));
+      CU_TRY(cudaMallocHost(&pr.h_count, sizeof(unsigned long long)));
+    }
+  }
+  const size_t cap = cfg->initial_capacity_points ? cfg->initial_capacity_points : 1;
+  if (cap != h->cap_gmap) {
+    cudaFree(h->d_gmap); h->d_gmap = nullptr; h->cap_gmap = 0;
+    CU_TRY(cudaMalloc(&h->d_gmap, cap * 3 * sizeof(double)));
+    h->cap_gmap = cap;
+  }
+  if (!h->d_gmap_off) {
+    CU_TRY(cudaMalloc(&h->d_gmap_off, 1024 * sizeof(unsigned long long)));
+    h->cap_gmap_off = 1024;
+  }
+  h->gmap_voxel = cfg->voxel;
+  h->gmap_growths = 0;
+  h->gmap_on = true;
+  return gmap_clear(h);
+}
+
+int tloam_b200_global_map_reset(tloam_b200_handle* h) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on) return TLOAM_B200_ERR_NOT_READY;
+  CU_TRY(cudaSetDevice(h->device));
+  return gmap_clear(h);
+}
+
+// the one place an append synchronises: the map (or its frame table) may not hold the next frame.  The exact size is read,
+// and the buffer grows to max(1.5 x capacity, exact size + n rows); the frame table likewise.
+static int gmap_grow(tloam_b200_handle* h, size_t n) {
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  GMapState st;
+  CU_TRY(cudaMemcpyAsync(&st, h->d_gmap_st, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  h->gmap_known = st.count; h->gmap_known_cum = h->gmap_cum;
+  for (auto& pr : h->gmap_probes) pr.pending = false;
+  if (st.count + n > h->cap_gmap) {
+    size_t ncap = h->cap_gmap + h->cap_gmap / 2;
+    if (ncap < st.count + n) ncap = st.count + n;
+    double* q = nullptr;
+    CU_TRY(cudaMalloc(&q, ncap * 3 * sizeof(double)));
+    if (st.count) CU_TRY(cudaMemcpyAsync(q, h->d_gmap, st.count * 3 * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_gmap);
+    h->d_gmap = q; h->cap_gmap = ncap;
+  }
+  if (h->gmap_calls + 2 > h->cap_gmap_off) {
+    size_t ncap = h->cap_gmap_off + h->cap_gmap_off / 2;
+    if (ncap < h->gmap_calls + 2) ncap = h->gmap_calls + 2;
+    unsigned long long* q = nullptr;
+    CU_TRY(cudaMalloc(&q, ncap * sizeof(unsigned long long)));
+    CU_TRY(cudaMemcpyAsync(q, h->d_gmap_off, (st.frames + 1) * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_gmap_off);
+    h->d_gmap_off = q; h->cap_gmap_off = ncap;
+  }
+  h->gmap_growths++;
+  return TLOAM_B200_OK;
+}
+
+// global_map += (T . raw).VoxelDownSample(voxel).  d_raw: a device raw scan read in place, or nullptr: xyz_host is uploaded
+// into the registered-scan buffer and transformed there.  pose_host == nullptr: the device-side result of the frame just
+// enqueued (as submap_update_impl's chained form).
+static int gmap_append_impl(tloam_b200_handle* h, const double* pose_host, const double* xyz_host, const double* d_raw, size_t n) {
+  if (n > ((size_t)1 << 30)) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  gmap_harvest(h);
+  int rc;
+  const unsigned long long bound = h->gmap_known + (h->gmap_cum - h->gmap_known_cum) + n;   // voxels <= finite rows <= rows
+  if (bound > h->cap_gmap || h->gmap_calls + 2 > h->cap_gmap_off)
+    if ((rc = gmap_grow(h, n)) != TLOAM_B200_OK) return rc;
+  if ((rc = ensure_dev(h, &h->d_gmap_reg, &h->cap_gmap_reg, n, false)) != TLOAM_B200_OK) return rc;
+  if ((rc = ensure_dev(h, &h->d_gmap_fin, &h->cap_gmap_fin, n, false)) != TLOAM_B200_OK) return rc;
+  const double* d_in = d_raw;
+  if (!d_raw && n) {                       // the only point data that crosses PCIe
+    if (HostStage::pageable(xyz_host) && getenv("TLOAM_B200_NO_HOST_STAGE") == nullptr)
+      CU_TRY(h->hstage.upload(h->d_gmap_reg, xyz_host, n * 24, h->stream));
+    else
+      CU_TRY(cudaMemcpyAsync(h->d_gmap_reg, xyz_host, n * 24, cudaMemcpyHostToDevice, h->stream));
+    d_in = h->d_gmap_reg;
+  }
+  const double* d_pose = h->d_gmap_pose;
+  if (pose_host) {
+    double tmp[16];
+    memcpy(tmp, pose_host, sizeof(tmp));
+    CU_TRY(cudaMemcpyAsync(h->d_gmap_pose, tmp, sizeof(tmp), cudaMemcpyHostToDevice, h->stream));   // pageable source: staged before return
+  } else {
+    d_pose = reinterpret_cast<const double*>(reinterpret_cast<const char*>(h->d_state) + offsetof(FrameState, result));
+  }
+  GMapState* st = h->d_gmap_st;
+  CU_TRY(cudaMemsetAsync(&st->n_fin, 0, sizeof(GMapState) - offsetof(GMapState, n_fin), h->stream));
+  const unsigned tb = 256, gb = (unsigned)((n + tb - 1) / tb);
+  if (n) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_transform<<<gb, tb, 0, h->stream>>>(d_in, (unsigned)n, d_pose, h->d_gmap_reg, h->d_gmap_fin, st)));
+  if (n) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_guard<<<1, 32, 0, h->stream>>>(st, h->gmap_voxel)));
+  VoxSorted vs;
+  if ((rc = voxel_pipeline(h, h->d_gmap_fin, n, &st->n_fin, 0u, nullptr, nullptr, nullptr, 0.0, h->gmap_voxel, nullptr, &st->n_vox,
+                           h->stream, 0, &vs)) != TLOAM_B200_OK) return rc;
+  if (n) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_emit<<<gb, tb, 0, h->stream>>>(vs.a, vs.slots, h->d_gmap, st, h->cap_gmap)));
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_commit<<<1, 32, 0, h->stream>>>(st, h->d_gmap_off, h->cap_gmap, h->cap_gmap_off)));
+  CU_TRY(cudaGetLastError());
+  h->gmap_cum += n;
+  h->gmap_calls++;
+  h->gmap_reg_n = n; h->gmap_reg_valid = true;
+  // asynchronous read-back of the exact size (tightens the bound of later frames)
+  tloam_b200_handle::GMapProbe& pr = h->gmap_probes[h->gmap_probe_next];
+  if (!pr.pending) {
+    CU_TRY(cudaMemcpyAsync(pr.h_count, &st->count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaEventRecord(pr.ev, h->stream));
+    pr.cum = h->gmap_cum; pr.pending = true;
+    h->gmap_probe_next = (h->gmap_probe_next + 1) & 3;
+  }
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_global_map_append(tloam_b200_handle* h, const double pose[16], const double* xyz, size_t n) {
+  if (!h || !pose || (!xyz && n)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on) return TLOAM_B200_ERR_NOT_READY;
+  return gmap_append_impl(h, pose, xyz, nullptr, n);
+}
+
+int tloam_b200_global_map_append_chained(tloam_b200_handle* h, const double* xyz, size_t n) {
+  if (!h || (!xyz && n)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on) return TLOAM_B200_ERR_NOT_READY;
+  return gmap_append_impl(h, nullptr, xyz, nullptr, n);
+}
+
+// the raw scan is read where process_raw_scan uploaded it (d_chain); any segmentation / process call since may have
+// reused that buffer, so the generation must still match
+static int gmap_append_frame(tloam_b200_handle* h, const double* pose) {
+  if (!h->gmap_on || h->raw_gen != h->seg_gen) return TLOAM_B200_ERR_NOT_READY;
+  return gmap_append_impl(h, pose, nullptr, h->raw_scan, h->raw_n);
+}
+
+int tloam_b200_global_map_append_frame(tloam_b200_handle* h, const double pose[16]) {
+  if (!h || !pose) return TLOAM_B200_ERR_INVALID_ARG;
+  return gmap_append_frame(h, pose);
+}
+
+int tloam_b200_global_map_append_frame_chained(tloam_b200_handle* h) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  return gmap_append_frame(h, nullptr);
+}
+
+// synchronises and reads the device-side state; a pending refusal / overflow flag is cleared and returned as a status
+static int gmap_read(tloam_b200_handle* h, GMapState* st, int* flag_status) {
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaMemcpyAsync(st, h->d_gmap_st, sizeof(*st), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  *flag_status = TLOAM_B200_OK;
+  if (st->flags) {
+    CU_TRY(cudaMemsetAsync(&h->d_gmap_st->flags, 0, sizeof(unsigned), h->stream));
+    if (st->flags & kGMapOverflow) {       // the host sizes the buffer from an upper bound: this is a bug, not an input error
+      snprintf(h->last_error, sizeof(h->last_error), "global map: the device-side capacity check refused a frame");
+      *flag_status = TLOAM_B200_ERR_CUDA;
+    } else {
+      *flag_status = TLOAM_B200_ERR_VOXEL_RANGE;
+    }
+  }
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_global_map_size(tloam_b200_handle* h, size_t* n_points, size_t* n_frames) {
+  if (!h || !n_points || !n_frames) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on) return TLOAM_B200_ERR_NOT_READY;
+  GMapState st;
+  int flag = TLOAM_B200_OK;
+  const int rc = gmap_read(h, &st, &flag);
+  if (rc != TLOAM_B200_OK) return rc;
+  *n_points = st.count; *n_frames = st.frames;
+  return flag;
+}
+
+int tloam_b200_global_map_download(tloam_b200_handle* h, size_t first, size_t count, double* out) {
+  if (!h || (!out && count)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on) return TLOAM_B200_ERR_NOT_READY;
+  GMapState st;
+  int flag = TLOAM_B200_OK;
+  const int rc = gmap_read(h, &st, &flag);
+  if (rc != TLOAM_B200_OK) return rc;
+  if (first > st.count || count > st.count - first) return TLOAM_B200_ERR_INVALID_ARG;
+  if (count) CU_TRY(cudaMemcpyAsync(out, h->d_gmap + 3 * first, count * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return flag;
+}
+
+int tloam_b200_global_map_frame_offsets(tloam_b200_handle* h, size_t* offsets, size_t capacity) {
+  if (!h || !offsets) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on) return TLOAM_B200_ERR_NOT_READY;
+  GMapState st;
+  int flag = TLOAM_B200_OK;
+  const int rc = gmap_read(h, &st, &flag);
+  if (rc != TLOAM_B200_OK) return rc;
+  if (capacity < st.frames + 1) return TLOAM_B200_ERR_INVALID_ARG;
+  static_assert(sizeof(size_t) == sizeof(unsigned long long), "the frame table is copied straight into a size_t array");
+  CU_TRY(cudaMemcpyAsync(offsets, h->d_gmap_off, (st.frames + 1) * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return flag;
+}
+
+int tloam_b200_global_map_capacity(tloam_b200_handle* h, size_t* capacity_points, size_t* growths) {
+  if (!h || !capacity_points || !growths) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on) return TLOAM_B200_ERR_NOT_READY;
+  *capacity_points = h->cap_gmap; *growths = h->gmap_growths;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_registered_scan_download(tloam_b200_handle* h, double* out, size_t capacity_points, size_t* n) {
+  if (!h || !n) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on || !h->gmap_reg_valid) return TLOAM_B200_ERR_NOT_READY;
+  *n = h->gmap_reg_n;
+  if (capacity_points < h->gmap_reg_n || (!out && h->gmap_reg_n)) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  if (h->gmap_reg_n) CU_TRY(cudaMemcpyAsync(out, h->d_gmap_reg, h->gmap_reg_n * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
 }
 
 int tloam_b200_host_alloc(void** p, size_t bytes) {

@@ -525,6 +525,73 @@ class LocalRegistration:
         """submap_update_chained with the last processed frame's planar-submap selection: no host input at all"""
         self._check(self._L.tloam_b200_submap_update_frame_chained(self._h), "submap_update_frame_chained")
 
+    # ---- global map (FrontEnd::updateSubmap with mapping_flag, ref: src/front_end/front_end.cpp:269-274) ----
+    def enable_global_map(self, voxel=1.0, initial_capacity=1 << 20):
+        """start an empty map: every appended raw scan is transformed, VoxelDownSample(voxel)'d on its own and concatenated"""
+        cfg = _lib.GlobalMapConfig(float(voxel), int(initial_capacity))
+        self._check(self._L.tloam_b200_global_map_enable(self._h, C.byref(cfg)), "global_map_enable")
+
+    def reset_global_map(self):
+        self._check(self._L.tloam_b200_global_map_reset(self._h), "global_map_reset")
+
+    def global_map_append(self, scan, pose=None):
+        """append a host raw scan (NaN / Inf rows allowed) with `pose` (4x4), or with the pose of the frame just enqueued on
+        this handle when pose is None (no host round trip)"""
+        a = _f64(scan).reshape(-1, 3)
+        if pose is None:
+            rc = self._L.tloam_b200_global_map_append_chained(self._h, _dp(a), a.shape[0])
+        else:
+            p = _f64(np.asarray(pose).T).reshape(16)
+            rc = self._L.tloam_b200_global_map_append(self._h, _dp(p), _dp(a), a.shape[0])
+        self._check(rc, "global_map_append")
+
+    def global_map_append_frame(self, pose=None):
+        """append the raw scan the last process_raw_scan uploaded (read on the device); pose None = chained"""
+        if pose is None:
+            rc = self._L.tloam_b200_global_map_append_frame_chained(self._h)
+        else:
+            p = _f64(np.asarray(pose).T).reshape(16)
+            rc = self._L.tloam_b200_global_map_append_frame(self._h, _dp(p))
+        self._check(rc, "global_map_append_frame")
+
+    def global_map_size(self):
+        """(points, frames) of the map; raises RegistrationError(ERR_VOXEL_RANGE) once after a refused frame"""
+        n, f = C.c_size_t(0), C.c_size_t(0)
+        self._check(self._L.tloam_b200_global_map_size(self._h, C.byref(n), C.byref(f)), "global_map_size")
+        return n.value, f.value
+
+    def global_map(self, first=0, count=None):
+        """map points [first, first + count) (all from `first` when count is None), (count, 3) float64"""
+        if count is None:
+            count = self.global_map_size()[0] - first
+        out = np.zeros((max(count, 0), 3))
+        self._check(self._L.tloam_b200_global_map_download(self._h, int(first), int(count), _dp(out)), "global_map_download")
+        return out
+
+    def global_map_frames(self):
+        """frame offsets: n_frames + 1 entries, frame f is map[offsets[f]:offsets[f + 1]]"""
+        nf = self.global_map_size()[1]
+        out = np.zeros(nf + 1, dtype=np.uint64)
+        self._check(self._L.tloam_b200_global_map_frame_offsets(self._h, out.ctypes.data_as(C.POINTER(C.c_size_t)), nf + 1),
+                    "global_map_frame_offsets")
+        return out.astype(np.int64)
+
+    def global_map_capacity(self):
+        """(capacity in points, growths since enable_global_map)"""
+        c, g = C.c_size_t(0), C.c_size_t(0)
+        self._check(self._L.tloam_b200_global_map_capacity(self._h, C.byref(c), C.byref(g)), "global_map_capacity")
+        return c.value, g.value
+
+    def registered_scan(self):
+        """T.p of every row of the last appended raw scan, raw order (non-finite rows stay non-finite)"""
+        n = C.c_size_t(0)
+        rc = self._L.tloam_b200_registered_scan_download(self._h, None, 0, C.byref(n))
+        if rc != _lib.ERR_INVALID_ARG or n.value == 0:
+            self._check(rc, "registered_scan_download")
+        out = np.zeros((n.value, 3))
+        self._check(self._L.tloam_b200_registered_scan_download(self._h, _dp(out), n.value, C.byref(n)), "registered_scan_download")
+        return out
+
     # ---- shared map (multi-GPU) ----
     def map_blob_size(self):
         n = C.c_size_t(0)

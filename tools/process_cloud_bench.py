@@ -8,7 +8,11 @@
 It checks that (b) and (c) give the same source apart from the voxel order and the fixed-point voxel averages (planar /
 sphere bit-identical, ground / edge the same rows to 1e-10 m), and prints the card and its power limit with the numbers.
 
-    python tools/process_cloud_bench.py [reps]
+With --mapping it measures the global map instead: frames/s of the loop (d) with global_map_append_frame_chained after the
+submap update against the same loop without it, three alternating runs each, the voxels appended per frame, and the time
+per frame of the same work on the CPU (numpy: transform, finite rows, VoxelDownSample(1.0) by np.unique and a group mean).
+
+    python tools/process_cloud_bench.py [reps] [--mapping]
 """
 import json
 import os
@@ -52,9 +56,86 @@ def sorted_rows(a):
     return a[np.lexsort(a.T[::-1])]
 
 
+def moved_scans(raw, reps):
+    xis = [np.array([0.3 * k, 0.02 * k, 0.0, 0.0, 0.0, 0.004 * k]) for k in range(reps + 1)]
+    scans = [raw]
+    for k in range(1, reps + 1):
+        Ti = np.linalg.inv(synth.se3_exp(xis[k]))
+        scans.append(np.ascontiguousarray(raw @ Ti[:3, :3].T + Ti[:3, 3]))
+    return scans, synth.se3_exp(-xis[1])
+
+
+def cpu_map_frame(raw, T, voxel=1.0):
+    """what a caller without the device map does per frame: T.p, finite rows, VoxelDownSample(voxel) of the frame"""
+    reg = raw @ T[:3, :3].T + T[:3, 3]
+    fin = reg[np.isfinite(reg).all(axis=1)]
+    idx = np.floor((fin - (fin.min(0) - 0.5 * voxel)) / voxel).astype(np.int64)
+    uniq, inv, cnt = np.unique(idx, axis=0, return_inverse=True, return_counts=True)
+    out = np.zeros((cnt.size, 3))
+    np.add.at(out, inv.reshape(-1), fin)
+    return out / cnt[:, None]
+
+
+def mapping_main(reps, card):
+    raw = synth.raw_scan()
+    scans, prev = moved_scans(raw, reps)
+    res = {"gpu": card, "raw_points": int(len(raw)), "frames": reps, "voxel": 1.0}
+    runs = {"without_mapping": [], "with_mapping": []}
+    for _ in range(3):
+        for mode in ("without_mapping", "with_mapping"):                 # alternating: the shared card drifts
+            r = tloam_b200.LocalRegistration(fitness_thres=0.3)
+            if mode == "with_mapping":
+                r.enable_global_map()
+            r.process_raw_scan(scans[0], feature=FE)
+            r.submap_init_frame()
+            r.set_pose_history(prev, np.eye(4))
+            t0 = time.perf_counter()
+            for sc in scans[1:]:
+                r.process_raw_scan(sc, feature=FE)
+                r.scan_matching_predicted_async()
+                r.submap_update_frame_chained()
+                if mode == "with_mapping":
+                    r.global_map_append_frame()
+                T = r.get_result()
+            runs[mode].append(reps / (time.perf_counter() - t0))
+            if mode == "with_mapping":
+                n, f = r.global_map_size()
+                res["voxels_per_frame"] = n / f
+                res["growths"] = r.global_map_capacity()[1]
+            r.close()
+    for mode, v in runs.items():
+        res[f"{mode}_frames_per_s"] = [round(x, 1) for x in v]
+    res["mapping_ms_per_frame"] = [round(1e3 / w - 1e3 / wo, 3) for wo, w in zip(runs["without_mapping"], runs["with_mapping"])]
+    # the append alone: back-to-back global_map_append_frame calls on one processed scan, ending in a synchronise
+    r = tloam_b200.LocalRegistration()
+    r.enable_global_map()
+    r.process_raw_scan(raw, feature=FE)
+    T = synth.se3_exp([1.0, 0.5, 0.0, 0.0, 0.0, 0.1])
+    r.global_map_append_frame(T)
+    r.global_map_size()
+    per = []
+    for _ in range(3):
+        t0 = time.perf_counter()
+        for _ in range(50):
+            r.global_map_append_frame(T)
+        r.global_map_size()
+        per.append(round(1e3 * (time.perf_counter() - t0) / 50, 3))
+    res["append_frame_ms"] = per
+    r.close()
+    cpu_map_frame(raw, T)
+    t0 = time.perf_counter()
+    for _ in range(5):
+        cpu_map_frame(raw, T)
+    res["cpu_numpy_ms_per_frame"] = round(1e3 * (time.perf_counter() - t0) / 5, 2)
+    print(json.dumps(res))
+
+
 def main():
-    reps = int(sys.argv[1]) if len(sys.argv) > 1 else 20
+    args = [a for a in sys.argv[1:] if not a.startswith("--")]
+    reps = int(args[0]) if args else 20
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    if "--mapping" in sys.argv:
+        return mapping_main(reps, card)
     raw = synth.raw_scan()
     reg = tloam_b200.LocalRegistration()
     s = reg.segment_raw_scan(raw)
@@ -74,12 +155,7 @@ def main():
     res["b_equals_c_up_to_voxel_order"] = bool(same)
 
     # (d) the per-frame loop over rigid motions of the scan, seeded from frame 0
-    xis = [np.array([0.3 * k, 0.02 * k, 0.0, 0.0, 0.0, 0.004 * k]) for k in range(reps + 1)]
-    scans = [raw]
-    for k in range(1, reps + 1):
-        Ti = np.linalg.inv(synth.se3_exp(xis[k]))
-        scans.append(np.ascontiguousarray(raw @ Ti[:3, :3].T + Ti[:3, 3]))
-    prev = synth.se3_exp(-xis[1])
+    scans, prev = moved_scans(raw, reps)
     for mode in ("device", "host_glue"):
         r = tloam_b200.LocalRegistration(fitness_thres=0.3)
         if mode == "device":

@@ -18,6 +18,7 @@ import numpy as np, tloam_b200
 from tloam_b200 import synth
 fe = dict(cvr_submap=0.005, cvr_scan=0.01)
 r = tloam_b200.LocalRegistration()
+r.enable_global_map()
 scan = synth.raw_scan(n_az=300)
 print("process_raw_scan", r.process_raw_scan(scan, ring_min_num=16, dcvc=dict(min_seg=20), feature=fe))
 r.submap_init_frame()
@@ -26,12 +27,15 @@ Ti = np.linalg.inv(T)
 print("process_raw_scan", r.process_raw_scan(np.ascontiguousarray(scan @ Ti[:3, :3].T + Ti[:3, 3]), ring_min_num=16, dcvc=dict(min_seg=20), feature=fe))
 r.scan_matching_predicted_async()
 r.submap_update_frame_chained()
+r.global_map_append_frame()
 print("pose", r.get_result()[:3, 3])
+r.global_map_append(np.vstack([scan, np.full((10, 3), np.nan)]), T)
+print("global map", r.global_map_size(), len(r.registered_scan()))
 r.close()
 PY
 for tool in memcheck racecheck; do
   echo "== $tool: tloam_b200_segment_scan + pageable staging (set_target of a 4.8 MB cloud)"
   timeout 600 compute-sanitizer --tool $tool --print-limit 5 python /tmp/seg_one.py 2>&1 | tail -4
-  echo "== $tool: tloam_b200_process_raw_scan -> submap_init_frame -> scan_match_predicted_async -> submap_update_frame_chained"
+  echo "== $tool: tloam_b200_process_raw_scan -> submap_init_frame -> scan_match_predicted_async -> submap_update_frame_chained -> global_map_append_frame_chained, global_map_append"
   timeout 600 compute-sanitizer --tool $tool --print-limit 5 python /tmp/process_one.py 2>&1 | tail -4
 done
