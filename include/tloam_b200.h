@@ -497,6 +497,30 @@ int tloam_b200_global_map_capacity(tloam_b200_handle* h, size_t* capacity_points
  * first append, INVALID_ARG if capacity_points < *n. */
 int tloam_b200_registered_scan_download(tloam_b200_handle* h, double* out, size_t capacity_points, size_t* n);
 
+/* ---- The map's intensity channel (the reference's map is XYZI): the same appends with the raw scan's intensity (n host
+ * FP64 values, one per raw row).  Each voxel's intensity is the reference's AccumulatedPoint::GetAverageIntensity
+ * (PointCloud2.cpp:253-286): a sequential FP64 sum of its rows' values in raw-row order from +0.0, divided by the count,
+ * bit for bit (NaN / Inf propagate).  The rows left out of the map (non-finite xyz) are left out of the sums too.
+ *   - The map has the channel under the rule of PointCloud2::operator+= (:99-100, :118-124): a frame that adds points keeps
+ *     it iff (map empty || map has it) && the frame has it.  A frame that adds nothing (empty, all non-finite, refused)
+ *     changes nothing; once points without intensity are in the map it has none until tloam_b200_global_map_reset.
+ *   - The xyz map, the frame table and the registered scan are the bits of the same appends without intensity.
+ *   - The kernels live in libtloam_b200_gmi.so, loaded from this library's directory on the first intensity call; if it is
+ *     missing these calls return ERR_CUDA (tloam_b200_last_error names the file) and nothing else is affected.
+ * intensity null: INVALID_ARG; mapping off: NOT_READY (and, for _frame, NOT_READY like tloam_b200_global_map_append_frame). */
+int tloam_b200_global_map_append_intensity(tloam_b200_handle* h, const double pose[16], const double* xyz, const double* intensity,
+                                           size_t n);
+int tloam_b200_global_map_append_intensity_chained(tloam_b200_handle* h, const double* xyz, const double* intensity, size_t n);
+/* the raw scan of the last tloam_b200_process_raw_scan with its intensity (as many values as that scan has rows) */
+int tloam_b200_global_map_append_frame_intensity(tloam_b200_handle* h, const double pose[16], const double* intensity);
+int tloam_b200_global_map_append_frame_intensity_chained(tloam_b200_handle* h, const double* intensity);
+/* *has = 1 if the map has an intensity channel (non-empty, every point with one; synchronises).  Reports the sticky flags
+ * as tloam_b200_global_map_size does. */
+int tloam_b200_global_map_has_intensity(tloam_b200_handle* h, int* has);
+/* intensities of map points [first, first + count) to out (synchronises).  NOT_READY when the map has no channel,
+ * INVALID_ARG past the end. */
+int tloam_b200_global_map_intensity_download(tloam_b200_handle* h, size_t first, size_t count, double* out);
+
 /* Pinned host memory helpers (optional; pinned inputs make set_* a direct DMA, no staging threads). */
 int tloam_b200_host_alloc(void** p, size_t bytes);
 int tloam_b200_host_free(void* p);

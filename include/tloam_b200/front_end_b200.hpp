@@ -11,7 +11,8 @@
 // submap selections and the submap itself stay on the GPU; the caller reads a source cloud back only to inspect it.
 // With mapping_flag (ref: front_end.cpp:57, :269-274) updateGlobalMap(raw, pose) after updateSubmap appends the frame's raw
 // scan, transformed and VoxelDownSample(1.0)'d on its own, to a global map kept on the GPU (globalMap / registeredScan read
-// it back); frame 0 has no append, as in the reference.
+// it back); frame 0 has no append, as in the reference.  A raw scan with intensity_ gives the map its intensity channel
+// (per-voxel averages, the reference's XYZI map); globalMap(points, intensity) reads it back.
 // Without the reference headers (this repository's tests) define TLOAM_B200_MOCK_HOST_TYPES and provide the host types
 // (tests/mock/mock_tloam.hpp).
 #ifndef TLOAM_B200_FRONT_END_B200_HPP
@@ -81,13 +82,20 @@ class FrontEndB200 {
   bool mappingFlag() const { return mapping_; }
   // global_map += raw.Transform(pose).VoxelDownSample(voxel) (ref: front_end.cpp:269-274): raw = the driver's scan, NaN rows
   // allowed (left out of the map).  No-ops returning true when mapping is off, like the reference.
+  // A raw cloud with intensity (PointCloud2::HasIntensity: the driver's /velodyne_points) gives each voxel the average of
+  // its rows' intensity_, as VoxelDownSample does; the map keeps the channel under operator+='s rule.
   bool updateGlobalMap(const CloudData& raw, const Eigen::Isometry3d& pose) {
     if (!mapping_) return true;
+    if (hasIntensity(raw))
+      return report(tloam_b200_global_map_append_intensity(h_, pose.matrix().data(), data(raw), intensity(raw), size(raw)),
+                    "updateGlobalMap");
     return report(tloam_b200_global_map_append(h_, pose.matrix().data(), data(raw), size(raw)), "updateGlobalMap");
   }
   // the same with the pose of the frame just enqueued on the handle (tloam_b200_scan_match_predicted_async)
   bool updateGlobalMapChained(const CloudData& raw) {
     if (!mapping_) return true;
+    if (hasIntensity(raw))
+      return report(tloam_b200_global_map_append_intensity_chained(h_, data(raw), intensity(raw), size(raw)), "updateGlobalMapChained");
     return report(tloam_b200_global_map_append_chained(h_, data(raw), size(raw)), "updateGlobalMapChained");
   }
   // the whole map (synchronises) and T.p of the last appended raw scan, raw order (the reference's /raw_cloud, :84-86)
@@ -96,6 +104,15 @@ class FrontEndB200 {
     if (!report(tloam_b200_global_map_size(h_, &n, &frames), "globalMap")) return false;
     out.resize(n);
     return report(tloam_b200_global_map_download(h_, 0, n, reinterpret_cast<double*>(out.data())), "globalMap");
+  }
+  // the map with its intensity channel: `intensity` is left empty when the map has none (the reference's intensity_.clear())
+  bool globalMap(std::vector<Eigen::Vector3d>& out, std::vector<double>& intensity) {
+    intensity.clear();
+    int has = 0;
+    if (!globalMap(out) || !report(tloam_b200_global_map_has_intensity(h_, &has), "globalMap")) return false;
+    if (!has) return true;
+    intensity.resize(out.size());
+    return report(tloam_b200_global_map_intensity_download(h_, 0, intensity.size(), intensity.data()), "globalMap");
   }
   bool registeredScan(std::vector<Eigen::Vector3d>& out) {
     size_t n = 0;
@@ -134,6 +151,10 @@ class FrontEndB200 {
     return c.cloud_ptr->points_.empty() ? nullptr : reinterpret_cast<const double*>(c.cloud_ptr->points_.data());
   }
   static size_t size(const CloudData& c) { return c.cloud_ptr->points_.size(); }
+  static bool hasIntensity(const CloudData& c) {                     // PointCloud2::HasIntensity (PointCloud2.hpp:108-110)
+    return !c.cloud_ptr->intensity_.empty() && c.cloud_ptr->intensity_.size() == c.cloud_ptr->points_.size();
+  }
+  static const double* intensity(const CloudData& c) { return c.cloud_ptr->intensity_.data(); }
   bool report(int rc, const char* where) {
     last_status_ = rc;
     if (rc != TLOAM_B200_OK)

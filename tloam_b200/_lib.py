@@ -131,6 +131,9 @@ EXPORTS = [
     "tloam_b200_global_map_append", "tloam_b200_global_map_append_chained", "tloam_b200_global_map_append_frame",
     "tloam_b200_global_map_append_frame_chained", "tloam_b200_global_map_size", "tloam_b200_global_map_download",
     "tloam_b200_global_map_frame_offsets", "tloam_b200_global_map_capacity", "tloam_b200_registered_scan_download",
+    "tloam_b200_global_map_append_intensity", "tloam_b200_global_map_append_intensity_chained",
+    "tloam_b200_global_map_append_frame_intensity", "tloam_b200_global_map_append_frame_intensity_chained",
+    "tloam_b200_global_map_has_intensity", "tloam_b200_global_map_intensity_download",
 ]
 
 _lib = None
@@ -267,5 +270,11 @@ def load():
     L.tloam_b200_global_map_frame_offsets.argtypes = [vp, szp, C.c_size_t]
     L.tloam_b200_global_map_capacity.argtypes = [vp, szp, szp]
     L.tloam_b200_registered_scan_download.argtypes = [vp, dp, C.c_size_t, szp]
+    L.tloam_b200_global_map_append_intensity.argtypes = [vp, dp, dp, dp, C.c_size_t]
+    L.tloam_b200_global_map_append_intensity_chained.argtypes = [vp, dp, dp, C.c_size_t]
+    L.tloam_b200_global_map_append_frame_intensity.argtypes = [vp, dp, dp]
+    L.tloam_b200_global_map_append_frame_intensity_chained.argtypes = [vp, dp]
+    L.tloam_b200_global_map_has_intensity.argtypes = [vp, C.POINTER(C.c_int)]
+    L.tloam_b200_global_map_intensity_download.argtypes = [vp, C.c_size_t, C.c_size_t, dp]
     _lib = L
     return L

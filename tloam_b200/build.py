@@ -1,8 +1,9 @@
-"""In-tree build of libtloam_b200.so (hand-written CUDA for sm_90a; no torch, no CPU fallback).
+"""In-tree build of libtloam_b200.so and libtloam_b200_gmi.so (hand-written CUDA for sm_90a; no torch, no CPU fallback).
 
     python -m tloam_b200.build [--force]
 
-nvcc cross-compiles without a GPU; the .so is git-ignored and built in the tree.
+nvcc cross-compiles without a GPU; the .so files are git-ignored and built in the tree.  libtloam_b200_gmi.so holds the
+global map's intensity kernels (csrc/gmap_intensity.cu); libtloam_b200.so loads it from its own directory when first needed.
 """
 import os
 import subprocess
@@ -12,6 +13,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libtloam_b200.so")
 SOURCES = [os.path.join(CSRC, "tloam_b200.cu")]
+GMI_LIB = os.path.join(HERE, "libtloam_b200_gmi.so")
+GMI_SOURCES = [os.path.join(CSRC, "gmap_intensity.cu")]
 import glob
 # every header the translation unit can include: editing any of them triggers a rebuild
 HEADERS = sorted(glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(CSRC, "*.h")) +
@@ -23,18 +26,16 @@ NVCC_FLAGS = [
 ]
 
 
-def needs_build():
-    if not os.path.exists(LIB):
+def needs_build(lib=LIB, sources=SOURCES):
+    if not os.path.exists(lib):
         return True
-    t = os.path.getmtime(LIB)
-    return any(os.path.getmtime(p) > t for p in SOURCES + HEADERS + [os.path.abspath(__file__)])
+    t = os.path.getmtime(lib)
+    return any(os.path.getmtime(p) > t for p in sources + HEADERS + [os.path.abspath(__file__)])
 
 
-def build(force=False, verbose=False, extra=()):
-    if not force and not needs_build():
-        return LIB
+def _nvcc(lib, sources, verbose, extra):
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    cmd = [nvcc] + NVCC_FLAGS + list(extra) + ["-o", LIB] + SOURCES
+    cmd = [nvcc] + NVCC_FLAGS + list(extra) + ["-o", lib] + sources
     if verbose:
         print(" ".join(cmd))
     res = subprocess.run(cmd, capture_output=True, text=True)
@@ -42,6 +43,13 @@ def build(force=False, verbose=False, extra=()):
         raise RuntimeError("nvcc failed:\n" + res.stdout + res.stderr)
     if verbose and (res.stdout or res.stderr):
         print(res.stdout + res.stderr)
+
+
+def build(force=False, verbose=False, extra=()):
+    """builds both libraries (each only when out of date); returns the path of libtloam_b200.so"""
+    for lib, sources in ((LIB, SOURCES), (GMI_LIB, GMI_SOURCES)):
+        if force or needs_build(lib, sources):
+            _nvcc(lib, sources, verbose, extra)
     return LIB
 
 

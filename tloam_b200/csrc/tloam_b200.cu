@@ -1,13 +1,16 @@
 // tloam_b200.cu -- kernels + C ABI of libtloam_b200.so (sm_90a). See include/tloam_b200.h for the boundary
 // and registration.cuh for the execution model.  No CPU fallback exists anywhere in this file.
 #include <cuda_runtime.h>
+#include <dlfcn.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
 #include <cmath>
 #include <functional>
+#include <mutex>
 #include <new>
+#include <string>
 #include <utility>
 #include <vector>
 
@@ -23,6 +26,7 @@
 #include "edge_extract.cuh"
 #include "object_segment.cuh"
 #include "host_stage.h"
+#include "gmap_intensity.h"
 
 
 
@@ -198,6 +202,13 @@ struct tloam_b200_handle {
   size_t gmap_growths = 0;
   struct GMapProbe { cudaEvent_t ev = nullptr; unsigned long long* h_count = nullptr; unsigned long long cum = 0; bool pending = false; };
   GMapProbe gmap_probes[4];                int gmap_probe_next = 0;
+  // ---- the map's intensity channel (tloam_b200_global_map_*intensity*, libtloam_b200_gmi.so): allocated on the first
+  //      intensity append; d_gmi_map has the capacity of d_gmap ----
+  bool gmi_used = false;                   // an intensity frame was appended since enable / reset
+  unsigned* d_gmi_st = nullptr;            // [0] the map has the channel, [1] a finite row found no voxel (sticky)
+  double* d_gmi_map = nullptr;
+  double* d_gmi_in = nullptr;              size_t cap_gmi_in = 0;                               // uploaded intensities
+  void* d_gmi_scratch = nullptr;           size_t cap_gmi_scratch = 0;
 };
 
 // launch bookkeeping: counts the kernel and, in profiling mode, brackets it with events
@@ -392,6 +403,7 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   cudaFree(h->d_vox1); cudaFree(h->d_acc_tmp1); cudaFree(h->d_up_planar); cudaFree(h->d_chain); cudaFree(h->d_frame);
   cudaFree(h->d_gmap_st); cudaFree(h->d_gmap_pose); cudaFree(h->d_gmap); cudaFree(h->d_gmap_off); cudaFree(h->d_gmap_reg);
   cudaFree(h->d_gmap_fin);
+  cudaFree(h->d_gmi_st); cudaFree(h->d_gmi_map); cudaFree(h->d_gmi_in); cudaFree(h->d_gmi_scratch);
   for (auto& pr : h->gmap_probes) { if (pr.ev) cudaEventDestroy(pr.ev); if (pr.h_count) cudaFreeHost(pr.h_count); }
   for (int i = 0; i < 2; ++i) if (h->ev_stage_free[i]) cudaEventDestroy(h->ev_stage_free[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_fit[i]) cudaEventDestroy(h->ev_fit[i]);
@@ -1837,7 +1849,7 @@ static int ensure_dev(tloam_b200_handle* h, double** p, size_t* cap, size_t need
 // device memory.
 // sorted (optional): the voxels are put in ascending key order instead of being emitted (the scan features of
 // tloam_b200_process_cloud, see submap.cuh); voxel_emit_sorted writes them once the count is known.
-struct VoxSorted { VoxArgs a; unsigned* slots = nullptr; };
+struct VoxSorted { VoxArgs a; unsigned* slots = nullptr; const unsigned long long* keys = nullptr; /* ~key, descending */ };
 static int voxel_pipeline(tloam_b200_handle* h, const double* d_in, size_t n_bound, const unsigned* n_dev, unsigned n_add,
                           const double* lo, const double* hi, const double* box_pose, double box_len, double voxel,
                           double* d_out, unsigned* out_count, cudaStream_t stream = nullptr, int scratch = 0,
@@ -1899,6 +1911,7 @@ static int voxel_pipeline(tloam_b200_handle* h, const double* d_in, size_t n_bou
   CU_TRY(cudaGetLastError());
   sorted->a = a;
   sorted->slots = slot_sorted;
+  sorted->keys = key_sorted;
   return TLOAM_B200_OK;
 }
 
@@ -3049,6 +3062,7 @@ static int gmap_clear(tloam_b200_handle* h) {
   h->gmap_cum = h->gmap_known_cum = h->gmap_known = h->gmap_calls = 0;
   for (auto& pr : h->gmap_probes) pr.pending = false;
   h->gmap_reg_valid = false; h->gmap_reg_n = 0;
+  h->gmi_used = false;                     // re-arms the intensity channel (the next intensity frame starts it afresh)
   return TLOAM_B200_OK;
 }
 
@@ -3067,6 +3081,7 @@ int tloam_b200_global_map_enable(tloam_b200_handle* h, const tloam_global_map_co
   const size_t cap = cfg->initial_capacity_points ? cfg->initial_capacity_points : 1;
   if (cap != h->cap_gmap) {
     cudaFree(h->d_gmap); h->d_gmap = nullptr; h->cap_gmap = 0;
+    cudaFree(h->d_gmi_map); h->d_gmi_map = nullptr;                       // reallocated by the next intensity append
     CU_TRY(cudaMalloc(&h->d_gmap, cap * 3 * sizeof(double)));
     h->cap_gmap = cap;
   }
@@ -3105,6 +3120,14 @@ static int gmap_grow(tloam_b200_handle* h, size_t n) {
     CU_TRY(cudaStreamSynchronize(h->stream));
     cudaFree(h->d_gmap);
     h->d_gmap = q; h->cap_gmap = ncap;
+    if (h->d_gmi_map) {                    // the intensity channel grows with the map
+      double* qi = nullptr;
+      CU_TRY(cudaMalloc(&qi, ncap * sizeof(double)));
+      if (st.count) CU_TRY(cudaMemcpyAsync(qi, h->d_gmi_map, st.count * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
+      CU_TRY(cudaStreamSynchronize(h->stream));
+      cudaFree(h->d_gmi_map);
+      h->d_gmi_map = qi;
+    }
   }
   if (h->gmap_calls + 2 > h->cap_gmap_off) {
     size_t ncap = h->cap_gmap_off + h->cap_gmap_off / 2;
@@ -3120,17 +3143,95 @@ static int gmap_grow(tloam_b200_handle* h, size_t n) {
   return TLOAM_B200_OK;
 }
 
+// ---- the intensity channel's kernels live in libtloam_b200_gmi.so (gmap_intensity.cu), next to this library: loaded on the
+//      first intensity call, so that the kernels of this library keep their SASS and a process that never asks for
+//      intensity never loads it ----
+struct GmiLib { tloam_gmi_scratch_bytes_fn scratch_bytes = nullptr; tloam_gmi_append_fn append = nullptr; tloam_gmi_plain_fn plain = nullptr; };
+static std::mutex g_gmi_mu;
+static GmiLib g_gmi;
+
+static int gmi_load(tloam_b200_handle* h, GmiLib* out) {
+  std::lock_guard<std::mutex> lk(g_gmi_mu);
+  if (!g_gmi.append) {
+    Dl_info info;
+    std::string path = "libtloam_b200_gmi.so";
+    if (dladdr(reinterpret_cast<void*>(&tloam_b200_global_map_has_intensity), &info) && info.dli_fname) {
+      const std::string self = info.dli_fname;
+      const size_t slash = self.rfind('/');
+      if (slash != std::string::npos) path = self.substr(0, slash + 1) + path;
+    }
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    GmiLib l;
+    if (so) {
+      l.scratch_bytes = reinterpret_cast<tloam_gmi_scratch_bytes_fn>(dlsym(so, "tloam_gmi_scratch_bytes"));
+      l.append = reinterpret_cast<tloam_gmi_append_fn>(dlsym(so, "tloam_gmi_append"));
+      l.plain = reinterpret_cast<tloam_gmi_plain_fn>(dlsym(so, "tloam_gmi_plain"));
+    }
+    if (!so || !l.scratch_bytes || !l.append || !l.plain) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "global map intensity: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_gmi = l;
+  }
+  *out = g_gmi;
+  return TLOAM_B200_OK;
+}
+
+static int gmi_status(tloam_b200_handle* h, int e, const char* where) {
+  if (e == cudaSuccess) return TLOAM_B200_OK;
+  snprintf(h->last_error, sizeof(h->last_error), "global map intensity: %s: %s", where, cudaGetErrorString((cudaError_t)e));
+  return TLOAM_B200_ERR_CUDA;
+}
+
+// device buffers of an intensity frame of n rows (after gmap_grow: d_gmi_map takes the map's current capacity)
+static int gmi_prepare(tloam_b200_handle* h, const GmiLib& lib, size_t n) {
+  if (!h->d_gmi_st) {
+    CU_TRY(cudaMalloc(&h->d_gmi_st, 2 * sizeof(unsigned)));
+    CU_TRY(cudaMemsetAsync(h->d_gmi_st, 0, 2 * sizeof(unsigned), h->stream));
+  }
+  if (!h->d_gmi_map) CU_TRY(cudaMalloc(&h->d_gmi_map, h->cap_gmap * sizeof(double)));
+  if (n > h->cap_gmi_in) {
+    const size_t ncap = n + n / 2 + 1024;
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_gmi_in); h->d_gmi_in = nullptr; h->cap_gmi_in = 0;
+    CU_TRY(cudaMalloc(&h->d_gmi_in, ncap * sizeof(double)));
+    h->cap_gmi_in = ncap;
+  }
+  const size_t bytes = lib.scratch_bytes((unsigned)n);
+  if (bytes > h->cap_gmi_scratch) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_gmi_scratch); h->d_gmi_scratch = nullptr; h->cap_gmi_scratch = 0;
+    CU_TRY(cudaMalloc(&h->d_gmi_scratch, bytes + bytes / 2));
+    h->cap_gmi_scratch = bytes + bytes / 2;
+  }
+  return TLOAM_B200_OK;
+}
+
 // global_map += (T . raw).VoxelDownSample(voxel).  d_raw: a device raw scan read in place, or nullptr: xyz_host is uploaded
 // into the registered-scan buffer and transformed there.  pose_host == nullptr: the device-side result of the frame just
-// enqueued (as submap_update_impl's chained form).
-static int gmap_append_impl(tloam_b200_handle* h, const double* pose_host, const double* xyz_host, const double* d_raw, size_t n) {
+// enqueued (as submap_update_impl's chained form).  int_host: the raw scan's intensity (n host values), or nullptr: the frame
+// has no intensity channel.
+static int gmap_append_impl(tloam_b200_handle* h, const double* pose_host, const double* xyz_host, const double* d_raw, size_t n,
+                            const double* int_host = nullptr) {
   if (n > ((size_t)1 << 30)) return TLOAM_B200_ERR_INVALID_ARG;
   CU_TRY(cudaSetDevice(h->device));
-  gmap_harvest(h);
   int rc;
+  GmiLib gmi;
+  const bool with_int = int_host && n;     // an empty frame adds nothing: the channel is left as it is
+  if ((with_int || h->gmi_used) && (rc = gmi_load(h, &gmi)) != TLOAM_B200_OK) return rc;
+  gmap_harvest(h);
   const unsigned long long bound = h->gmap_known + (h->gmap_cum - h->gmap_known_cum) + n;   // voxels <= finite rows <= rows
   if (bound > h->cap_gmap || h->gmap_calls + 2 > h->cap_gmap_off)
     if ((rc = gmap_grow(h, n)) != TLOAM_B200_OK) return rc;
+  if (with_int) {
+    if ((rc = gmi_prepare(h, gmi, n)) != TLOAM_B200_OK) return rc;
+    if (HostStage::pageable(int_host) && getenv("TLOAM_B200_NO_HOST_STAGE") == nullptr)
+      CU_TRY(h->hstage.upload(h->d_gmi_in, int_host, n * 8, h->stream));
+    else
+      CU_TRY(cudaMemcpyAsync(h->d_gmi_in, int_host, n * 8, cudaMemcpyHostToDevice, h->stream));
+  }
   if ((rc = ensure_dev(h, &h->d_gmap_reg, &h->cap_gmap_reg, n, false)) != TLOAM_B200_OK) return rc;
   if ((rc = ensure_dev(h, &h->d_gmap_fin, &h->cap_gmap_fin, n, false)) != TLOAM_B200_OK) return rc;
   const double* d_in = d_raw;
@@ -3158,6 +3259,24 @@ static int gmap_append_impl(tloam_b200_handle* h, const double* pose_host, const
   if ((rc = voxel_pipeline(h, h->d_gmap_fin, n, &st->n_fin, 0u, nullptr, nullptr, nullptr, 0.0, h->gmap_voxel, nullptr, &st->n_vox,
                            h->stream, 0, &vs)) != TLOAM_B200_OK) return rc;
   if (n) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_emit<<<gb, tb, 0, h->stream>>>(vs.a, vs.slots, h->d_gmap, st, h->cap_gmap)));
+  // the intensity channel, while st->count is still the frame's base (gmap_intensity.cu)
+  if (with_int) {
+    tloam_gmi_frame f;
+    f.reg = h->d_gmap_reg; f.intensity = h->d_gmi_in; f.n = (unsigned)n;
+    f.minenc = vs.a.minenc; f.voxel = h->gmap_voxel; f.keys_sorted = vs.keys; f.n_vox = &st->n_vox; f.refused = &st->refused;
+    f.count = &st->count; f.frames = &st->frames; f.cap = h->cap_gmap; f.frame_cap = h->cap_gmap_off;
+    f.map_intensity = h->d_gmi_map; f.state = h->d_gmi_st; f.fresh = h->gmi_used ? 0 : 1; f.scratch = h->d_gmi_scratch;
+    int launches = 0, e = 0;
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = gmi.append(&f, h->device, h->stream, &launches)));
+    h->launches += launches > 0 ? launches - 1 : 0;
+    if ((rc = gmi_status(h, e, "append")) != TLOAM_B200_OK) return rc;
+    h->gmi_used = true;
+  } else if (n && h->gmi_used) {
+    int e = 0;
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = gmi.plain(h->d_gmi_st, &st->n_vox, &st->refused, &st->count, &st->frames, h->cap_gmap,
+                                                  h->cap_gmap_off, h->device, h->stream)));
+    if ((rc = gmi_status(h, e, "plain")) != TLOAM_B200_OK) return rc;
+  }
   TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_commit<<<1, 32, 0, h->stream>>>(st, h->d_gmap_off, h->cap_gmap, h->cap_gmap_off)));
   CU_TRY(cudaGetLastError());
   h->gmap_cum += n;
@@ -3275,6 +3394,80 @@ int tloam_b200_registered_scan_download(tloam_b200_handle* h, double* out, size_
   if (h->gmap_reg_n) CU_TRY(cudaMemcpyAsync(out, h->d_gmap_reg, h->gmap_reg_n * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   CU_TRY(cudaStreamSynchronize(h->stream));
   return TLOAM_B200_OK;
+}
+
+// ---- the intensity channel (kernels in gmap_intensity.cu): the same appends with the raw scan's intensity ----
+int tloam_b200_global_map_append_intensity(tloam_b200_handle* h, const double pose[16], const double* xyz, const double* intensity,
+                                           size_t n) {
+  if (!h || !pose || (!xyz && n) || !intensity) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on) return TLOAM_B200_ERR_NOT_READY;
+  return gmap_append_impl(h, pose, xyz, nullptr, n, intensity);
+}
+
+int tloam_b200_global_map_append_intensity_chained(tloam_b200_handle* h, const double* xyz, const double* intensity, size_t n) {
+  if (!h || (!xyz && n) || !intensity) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on) return TLOAM_B200_ERR_NOT_READY;
+  return gmap_append_impl(h, nullptr, xyz, nullptr, n, intensity);
+}
+
+int tloam_b200_global_map_append_frame_intensity(tloam_b200_handle* h, const double pose[16], const double* intensity) {
+  if (!h || !pose || !intensity) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on || h->raw_gen != h->seg_gen) return TLOAM_B200_ERR_NOT_READY;
+  return gmap_append_impl(h, pose, nullptr, h->raw_scan, h->raw_n, intensity);
+}
+
+int tloam_b200_global_map_append_frame_intensity_chained(tloam_b200_handle* h, const double* intensity) {
+  if (!h || !intensity) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on || h->raw_gen != h->seg_gen) return TLOAM_B200_ERR_NOT_READY;
+  return gmap_append_impl(h, nullptr, nullptr, h->raw_scan, h->raw_n, intensity);
+}
+
+// synchronises (gmap_read: the sticky flags of the xyz map) and reads whether the map has the channel (PointCloud2::
+// HasIntensity: a non-empty map whose every point has an intensity)
+static int gmi_read(tloam_b200_handle* h, GMapState* st, int* flag_status, bool* has) {
+  int rc = gmap_read(h, st, flag_status);
+  if (rc != TLOAM_B200_OK) return rc;
+  *has = false;
+  if (!h->gmi_used) return TLOAM_B200_OK;
+  unsigned s[2];
+  CU_TRY(cudaMemcpyAsync(s, h->d_gmi_st, sizeof(s), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (s[1]) {                              // a finite row found no voxel of its frame: a bug, not an input error
+    CU_TRY(cudaMemsetAsync(h->d_gmi_st + 1, 0, sizeof(unsigned), h->stream));
+    snprintf(h->last_error, sizeof(h->last_error), "global map intensity: a finite row found no voxel of its frame");
+    *flag_status = TLOAM_B200_ERR_CUDA;
+  }
+  *has = s[0] != 0u && st->count > 0;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_global_map_has_intensity(tloam_b200_handle* h, int* has) {
+  if (!h || !has) return TLOAM_B200_ERR_INVALID_ARG;
+  *has = 0;
+  if (!h->gmap_on) return TLOAM_B200_ERR_NOT_READY;
+  GMapState st;
+  int flag = TLOAM_B200_OK;
+  bool b = false;
+  const int rc = gmi_read(h, &st, &flag, &b);
+  if (rc != TLOAM_B200_OK) return rc;
+  *has = b ? 1 : 0;
+  return flag;
+}
+
+int tloam_b200_global_map_intensity_download(tloam_b200_handle* h, size_t first, size_t count, double* out) {
+  if (!h || (!out && count)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on) return TLOAM_B200_ERR_NOT_READY;
+  GMapState st;
+  int flag = TLOAM_B200_OK;
+  bool has = false;
+  const int rc = gmi_read(h, &st, &flag, &has);
+  if (rc != TLOAM_B200_OK) return rc;
+  if (flag == TLOAM_B200_ERR_CUDA) return flag;
+  if (!has) return TLOAM_B200_ERR_NOT_READY;
+  if (first > st.count || count > st.count - first) return TLOAM_B200_ERR_INVALID_ARG;
+  if (count) CU_TRY(cudaMemcpyAsync(out, h->d_gmi_map + first, count * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return flag;
 }
 
 int tloam_b200_host_alloc(void** p, size_t bytes) {

@@ -503,6 +503,7 @@ class LocalRegistration:
                                                         float(ground_down_sample), float(edge_down_sample), _dp(a), a.shape[0], ns),
                     "process_raw_scan")
         self.n_source = [int(v) for v in ns]
+        self._raw_scan_rows = a.shape[0]       # global_map_append_frame(intensity=...) takes one value per row
         return list(self.n_source)
 
     def source_cloud(self, cloud):
@@ -534,25 +535,62 @@ class LocalRegistration:
     def reset_global_map(self):
         self._check(self._L.tloam_b200_global_map_reset(self._h), "global_map_reset")
 
-    def global_map_append(self, scan, pose=None):
+    @staticmethod
+    def _intensity(intensity, rows):
+        v = _f64(intensity).reshape(-1)
+        if v.shape[0] != rows:
+            raise ValueError(f"intensity has {v.shape[0]} values for {rows} rows")
+        return v
+
+    def global_map_append(self, scan, pose=None, intensity=None):
         """append a host raw scan (NaN / Inf rows allowed) with `pose` (4x4), or with the pose of the frame just enqueued on
-        this handle when pose is None (no host round trip)"""
+        this handle when pose is None (no host round trip).  intensity: one value per row (the reference's XYZI map: each
+        voxel gets the average of its rows'), or None for a frame without intensity"""
         a = _f64(scan).reshape(-1, 3)
-        if pose is None:
+        p = None if pose is None else _f64(np.asarray(pose).T).reshape(16)
+        if intensity is not None:
+            v = self._intensity(intensity, a.shape[0])
+            if p is None:
+                rc = self._L.tloam_b200_global_map_append_intensity_chained(self._h, _dp(a), _dp(v), a.shape[0])
+            else:
+                rc = self._L.tloam_b200_global_map_append_intensity(self._h, _dp(p), _dp(a), _dp(v), a.shape[0])
+        elif p is None:
             rc = self._L.tloam_b200_global_map_append_chained(self._h, _dp(a), a.shape[0])
         else:
-            p = _f64(np.asarray(pose).T).reshape(16)
             rc = self._L.tloam_b200_global_map_append(self._h, _dp(p), _dp(a), a.shape[0])
         self._check(rc, "global_map_append")
 
-    def global_map_append_frame(self, pose=None):
-        """append the raw scan the last process_raw_scan uploaded (read on the device); pose None = chained"""
-        if pose is None:
+    def global_map_append_frame(self, pose=None, intensity=None):
+        """append the raw scan the last process_raw_scan uploaded (read on the device); pose None = chained.  intensity: one
+        value per row of that scan, or None"""
+        p = None if pose is None else _f64(np.asarray(pose).T).reshape(16)
+        if intensity is not None:
+            v = self._intensity(intensity, getattr(self, "_raw_scan_rows", 0))
+            if p is None:
+                rc = self._L.tloam_b200_global_map_append_frame_intensity_chained(self._h, _dp(v))
+            else:
+                rc = self._L.tloam_b200_global_map_append_frame_intensity(self._h, _dp(p), _dp(v))
+        elif p is None:
             rc = self._L.tloam_b200_global_map_append_frame_chained(self._h)
         else:
-            p = _f64(np.asarray(pose).T).reshape(16)
             rc = self._L.tloam_b200_global_map_append_frame(self._h, _dp(p))
         self._check(rc, "global_map_append_frame")
+
+    def global_map_has_intensity(self):
+        """True if the map has an intensity channel (PointCloud2::HasIntensity); raises like global_map_size"""
+        has = C.c_int(0)
+        self._check(self._L.tloam_b200_global_map_has_intensity(self._h, C.byref(has)), "global_map_has_intensity")
+        return bool(has.value)
+
+    def global_map_intensity(self, first=0, count=None):
+        """intensities of map points [first, first + count) (all from `first` when count is None), float64; raises
+        RegistrationError(ERR_NOT_READY) when the map has no intensity channel"""
+        if count is None:
+            count = self.global_map_size()[0] - first
+        out = np.zeros(max(count, 0))
+        self._check(self._L.tloam_b200_global_map_intensity_download(self._h, int(first), int(count), _dp(out)),
+                    "global_map_intensity_download")
+        return out
 
     def global_map_size(self):
         """(points, frames) of the map; raises RegistrationError(ERR_VOXEL_RANGE) once after a refused frame"""

@@ -12,7 +12,10 @@ With --mapping it measures the global map instead: frames/s of the loop (d) with
 submap update against the same loop without it, three alternating runs each, the voxels appended per frame, and the time
 per frame of the same work on the CPU (numpy: transform, finite rows, VoxelDownSample(1.0) by np.unique and a group mean).
 
-    python tools/process_cloud_bench.py [reps] [--mapping]
+With --mapping --intensity it times one global_map_append_frame of the raw scan with and without its intensity channel
+(two handles, alternating rounds of back-to-back appends) and checks that the xyz map is the same.
+
+    python tools/process_cloud_bench.py [reps] [--mapping [--intensity]]
 """
 import json
 import os
@@ -130,10 +133,51 @@ def mapping_main(reps, card):
     print(json.dumps(res))
 
 
+def intensity_main(card, rounds=5, calls=50):
+    """one global_map_append_frame on the 116k-point raw scan with and without the intensity channel: two handles (one never
+    sees intensity), `calls` back-to-back appends each ending in a synchronise, `rounds` alternating rounds"""
+    raw = synth.raw_scan()
+    inten = np.random.default_rng(1).uniform(0.0, 255.0, len(raw))
+    T = synth.se3_exp([1.0, 0.5, 0.0, 0.0, 0.0, 0.1])
+    handles = {}
+    for mode in ("without_intensity", "with_intensity"):
+        r = tloam_b200.LocalRegistration()
+        r.enable_global_map()
+        r.process_raw_scan(raw, feature=FE)
+        handles[mode] = r
+    kw = {"without_intensity": {}, "with_intensity": {"intensity": inten}}
+    per = {m: [] for m in handles}
+    for _ in range(rounds):
+        for mode, r in handles.items():                                  # alternating: the shared card drifts
+            r.reset_global_map()
+            r.global_map_append_frame(T, **kw[mode])
+            r.global_map_size()
+            t0 = time.perf_counter()
+            for _ in range(calls):
+                r.global_map_append_frame(T, **kw[mode])
+            r.global_map_size()
+            per[mode].append(round(1e3 * (time.perf_counter() - t0) / calls, 4))
+    r = handles["with_intensity"]
+    n, f = r.global_map_size()
+    assert r.global_map_has_intensity() and len(r.global_map_intensity()) == n
+    a = handles["without_intensity"]
+    same = np.array_equal(a.global_map(), r.global_map())
+    res = {"gpu": card, "raw_points": int(len(raw)), "voxels_per_frame": n / f, "xyz_map_identical": bool(same),
+           "calls_per_round": calls}
+    for mode, v in per.items():
+        res[f"append_frame_{mode}_ms"] = v
+    res["added_ms"] = [round(w - wo, 4) for wo, w in zip(per["without_intensity"], per["with_intensity"])]
+    for h in handles.values():
+        h.close()
+    print(json.dumps(res))
+
+
 def main():
     args = [a for a in sys.argv[1:] if not a.startswith("--")]
     reps = int(args[0]) if args else 20
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    if "--mapping" in sys.argv and "--intensity" in sys.argv:
+        return intensity_main(card)
     if "--mapping" in sys.argv:
         return mapping_main(reps, card)
     raw = synth.raw_scan()

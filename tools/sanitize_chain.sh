@@ -31,11 +31,21 @@ r.global_map_append_frame()
 print("pose", r.get_result()[:3, 3])
 r.global_map_append(np.vstack([scan, np.full((10, 3), np.nan)]), T)
 print("global map", r.global_map_size(), len(r.registered_scan()))
+inten = np.random.default_rng(0).uniform(0, 255, len(scan) + 10)
+r.global_map_append(np.vstack([scan, np.full((10, 3), np.nan)]), T, intensity=inten)       # libtloam_b200_gmi.so
+r.reset_global_map()
+r.global_map_append(np.vstack([scan, np.full((10, 3), np.nan)]), T, intensity=inten)
+r.global_map_append(scan, T)                                                                # clears the channel
+r.global_map_append(np.vstack([scan, np.full((10, 3), np.nan)]), None, intensity=inten)
+print("global map intensity", r.global_map_size(), r.global_map_has_intensity())
+r.reset_global_map()
+r.global_map_append(scan, T, intensity=inten[:len(scan)])
+print("intensity", r.global_map_intensity()[:3])
 r.close()
 PY
 for tool in memcheck racecheck; do
   echo "== $tool: tloam_b200_segment_scan + pageable staging (set_target of a 4.8 MB cloud)"
   timeout 600 compute-sanitizer --tool $tool --print-limit 5 python /tmp/seg_one.py 2>&1 | tail -4
-  echo "== $tool: tloam_b200_process_raw_scan -> submap_init_frame -> scan_match_predicted_async -> submap_update_frame_chained -> global_map_append_frame_chained, global_map_append"
+  echo "== $tool: tloam_b200_process_raw_scan -> submap_init_frame -> scan_match_predicted_async -> submap_update_frame_chained -> global_map_append_frame_chained, global_map_append (with and without intensity)"
   timeout 600 compute-sanitizer --tool $tool --print-limit 5 python /tmp/process_one.py 2>&1 | tail -4
 done
