@@ -415,6 +415,29 @@ int tloam_b200_segment_raw_scan(tloam_b200_handle* h, const tloam_ground_config*
                                 size_t* n_edge, size_t* general_index, size_t* n_general, int* n_clusters, int* sizes, double* boxes,
                                 double* intensity);
 
+/* ---- Raw scans in the sensor's packed layout (the reference's RosToOpen3d, ref: src/open3d/open3d_to_ros.cpp:344-374, and
+ * readVelodyneToO3d, include/tloam/models/io/read_file.hpp:307-327, on the device): the records cross PCIe once, as the
+ * driver delivers them, and k_unpack_scan writes (double)float of every field on the GPU -- exact, so a packed call gives the
+ * bits of the FP64 call on the same values.  A sensor_msgs/PointCloud2 with FLOAT32 x / y / z (and intensity) fields, or a
+ * KITTI .bin scan (16-byte records: x, y, z, reflectance).  Anything this cannot express is the caller's to refuse:
+ * big-endian data, other field types, padding between rows (include/tloam_b200/packed_scan_b200.hpp does it for a
+ * PointCloud2).  The kernel lives in libtloam_b200_unpack.so, loaded from this library's directory on the first packed call;
+ * if it is missing these calls return ERR_CUDA (tloam_b200_last_error names the file) and nothing else is affected.
+ * INVALID_ARG: data null with n > 0, point_step < 12, a field not inside the record (offset < 0 or offset + 4 >
+ * point_step; intensity_offset may be -1), n > 2^26.  n == 0 is an empty scan. */
+typedef struct tloam_packed_scan {
+  const void* data;                   /* HOST, n records of point_step bytes, little-endian */
+  size_t n, point_step;
+  int x_offset, y_offset, z_offset;   /* FLOAT32 fields */
+  int intensity_offset;               /* FLOAT32 field, or -1: the scan has no intensity */
+} tloam_packed_scan;
+/* tloam_b200_segment_raw_scan on a packed scan (its intensity field, if any, is not read: the `intensity` output is the
+ * channel the segmentation computes, as there) */
+int tloam_b200_segment_raw_scan_packed(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg,
+                                       int ring_min_num, double near_dis, const tloam_packed_scan* scan, size_t* ground_index,
+                                       size_t* n_ground, size_t* edge_index, size_t* n_edge, size_t* general_index, size_t* n_general,
+                                       int* n_clusters, int* sizes, double* boxes, double* intensity);
+
 /* ---- FrontEnd::processCloud on the device (ref: src/front_end/front_end.cpp:181-199): the scan features become the
  * registration source without leaving the GPU.  VoxelDownSample(ground, ground_down_sample) and VoxelDownSample(edge,
  * edge_down_sample), extractPlanarSphere(general) with fcfg, SelectByIndex of the planar and sphere features, then
@@ -442,6 +465,11 @@ int tloam_b200_process_cloud(tloam_b200_handle* h, const tloam_feature_config* f
 int tloam_b200_process_raw_scan(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg, int ring_min_num,
                                 double near_dis, const tloam_feature_config* fcfg, double ground_down_sample, double edge_down_sample,
                                 const double* xyz, size_t n, size_t n_source[4]);
+/* tloam_b200_process_raw_scan on a packed scan (validation as tloam_b200_segment_raw_scan_packed).  With an intensity field,
+ * its values stay on the device with the raw scan, for tloam_b200_global_map_append_frame*. */
+int tloam_b200_process_raw_scan_packed(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg,
+                                       int ring_min_num, double near_dis, const tloam_feature_config* fcfg, double ground_down_sample,
+                                       double edge_down_sample, const tloam_packed_scan* scan, size_t n_source[4]);
 /* copies source cloud `cloud` (0 edge, 1 sphere, 2 planar, 3 ground; sensor frame, FP64 AoS) to the host (synchronises) */
 int tloam_b200_source_download(tloam_b200_handle* h, int cloud, double* out, size_t capacity_points);
 /* tloam_b200_submap_init from the last processed frame (front_end.cpp:285-305): edge = its raw edge cloud, ground =
@@ -482,7 +510,11 @@ int tloam_b200_global_map_reset(tloam_b200_handle* h);
 int tloam_b200_global_map_append(tloam_b200_handle* h, const double pose[16], const double* xyz, size_t n);
 int tloam_b200_global_map_append_chained(tloam_b200_handle* h, const double* xyz, size_t n);
 /* the same for the raw scan that the last tloam_b200_process_raw_scan uploaded (no upload).  NOT_READY when there is none,
- * or when any segmentation or process call has run since (its buffer may have been reused). */
+ * or when any segmentation or process call has run since (its buffer may have been reused).
+ * After tloam_b200_process_raw_scan_packed whose layout has an intensity field, the frame is appended WITH that intensity,
+ * read on the device (the reference's raw cloud carries its channel into global_map += ...); without one, or after the FP64
+ * tloam_b200_process_raw_scan, it is a frame without intensity.  tloam_b200_global_map_append_frame_intensity[_chained]
+ * with an explicit host array takes precedence over the packed intensity. */
 int tloam_b200_global_map_append_frame(tloam_b200_handle* h, const double pose[16]);
 int tloam_b200_global_map_append_frame_chained(tloam_b200_handle* h);
 /* exact points and frames in the map (synchronises); returns VOXEL_RANGE once after a refused frame */
@@ -520,6 +552,11 @@ int tloam_b200_global_map_has_intensity(tloam_b200_handle* h, int* has);
 /* intensities of map points [first, first + count) to out (synchronises).  NOT_READY when the map has no channel,
  * INVALID_ARG past the end. */
 int tloam_b200_global_map_intensity_download(tloam_b200_handle* h, size_t first, size_t count, double* out);
+/* tloam_b200_global_map_append[_chained] of a HOST packed scan (see tloam_packed_scan): one upload, unpacked on the device.
+ * With an intensity field the frame is an intensity frame (as tloam_b200_global_map_append_intensity), without one a plain
+ * frame.  scan null or an invalid layout: INVALID_ARG; mapping off: NOT_READY. */
+int tloam_b200_global_map_append_packed(tloam_b200_handle* h, const double pose[16], const tloam_packed_scan* scan);
+int tloam_b200_global_map_append_packed_chained(tloam_b200_handle* h, const tloam_packed_scan* scan);
 
 /* Pinned host memory helpers (optional; pinned inputs make set_* a direct DMA, no staging threads). */
 int tloam_b200_host_alloc(void** p, size_t bytes);

@@ -12,7 +12,9 @@
 // With mapping_flag (ref: front_end.cpp:57, :269-274) updateGlobalMap(raw, pose) after updateSubmap appends the frame's raw
 // scan, transformed and VoxelDownSample(1.0)'d on its own, to a global map kept on the GPU (globalMap / registeredScan read
 // it back); frame 0 has no append, as in the reference.  A raw scan with intensity_ gives the map its intensity channel
-// (per-voxel averages, the reference's XYZI map); globalMap(points, intensity) reads it back.
+// (per-voxel averages, the reference's XYZI map); globalMap(points, intensity) reads it back.  updateGlobalMap also takes
+// the driver's sensor_msgs/PointCloud2 as it arrived (packed_scan_b200.hpp): one upload, unpacked on the device, its
+// intensity field (if any) carried into the map.
 // Without the reference headers (this repository's tests) define TLOAM_B200_MOCK_HOST_TYPES and provide the host types
 // (tests/mock/mock_tloam.hpp).
 #ifndef TLOAM_B200_FRONT_END_B200_HPP
@@ -24,6 +26,7 @@
 
 #include "../tloam_b200.h"
 #include "local_registration_b200.hpp"
+#include "packed_scan_b200.hpp"
 
 #ifndef TLOAM_B200_MOCK_HOST_TYPES
 #include <yaml-cpp/yaml.h>
@@ -97,6 +100,25 @@ class FrontEndB200 {
     if (hasIntensity(raw))
       return report(tloam_b200_global_map_append_intensity_chained(h_, data(raw), intensity(raw), size(raw)), "updateGlobalMapChained");
     return report(tloam_b200_global_map_append_chained(h_, data(raw), size(raw)), "updateGlobalMapChained");
+  }
+  // the same from the driver's message (any sensor_msgs::PointCloud2-shaped type, see packedScanOf): no host conversion, the
+  // records cross PCIe once.  A message with a FLOAT32 intensity field gives an intensity frame.  A layout packedScanOf
+  // refuses returns false with lastStatus() INVALID_ARG.
+  template <class Msg>
+  bool updateGlobalMap(const Msg& raw, const Eigen::Isometry3d& pose) {
+    if (!mapping_) return true;
+    tloam_packed_scan scan;
+    const int rc = packedScanOf(raw, &scan);
+    if (rc != TLOAM_B200_OK) return report(rc, "updateGlobalMap");
+    return report(tloam_b200_global_map_append_packed(h_, pose.matrix().data(), &scan), "updateGlobalMap");
+  }
+  template <class Msg>
+  bool updateGlobalMapChained(const Msg& raw) {
+    if (!mapping_) return true;
+    tloam_packed_scan scan;
+    const int rc = packedScanOf(raw, &scan);
+    if (rc != TLOAM_B200_OK) return report(rc, "updateGlobalMapChained");
+    return report(tloam_b200_global_map_append_packed_chained(h_, &scan), "updateGlobalMapChained");
   }
   // the whole map (synchronises) and T.p of the last appended raw scan, raw order (the reference's /raw_cloud, :84-86)
   bool globalMap(std::vector<Eigen::Vector3d>& out) {

@@ -42,6 +42,13 @@ class GlobalMapConfig(C.Structure):
     _fields_ = [("voxel", C.c_double), ("initial_capacity_points", C.c_size_t)]
 
 
+class PackedScan(C.Structure):
+    """tloam_packed_scan (include/tloam_b200.h): n little-endian records of point_step bytes with FLOAT32 x / y / z (and
+    intensity, or intensity_offset -1) fields.  Build one with tloam_b200.packed_scan."""
+    _fields_ = [("data", C.c_void_p), ("n", C.c_size_t), ("point_step", C.c_size_t), ("x_offset", C.c_int), ("y_offset", C.c_int),
+                ("z_offset", C.c_int), ("intensity_offset", C.c_int)]
+
+
 class InnerTrace(C.Structure):
     _fields_ = [
         ("x_candidate", C.c_double * 6), ("candidate_cost", C.c_double), ("model_cost_change", C.c_double),
@@ -134,6 +141,8 @@ EXPORTS = [
     "tloam_b200_global_map_append_intensity", "tloam_b200_global_map_append_intensity_chained",
     "tloam_b200_global_map_append_frame_intensity", "tloam_b200_global_map_append_frame_intensity_chained",
     "tloam_b200_global_map_has_intensity", "tloam_b200_global_map_intensity_download",
+    "tloam_b200_segment_raw_scan_packed", "tloam_b200_process_raw_scan_packed", "tloam_b200_global_map_append_packed",
+    "tloam_b200_global_map_append_packed_chained",
 ]
 
 _lib = None
@@ -276,5 +285,12 @@ def load():
     L.tloam_b200_global_map_append_frame_intensity_chained.argtypes = [vp, dp]
     L.tloam_b200_global_map_has_intensity.argtypes = [vp, C.POINTER(C.c_int)]
     L.tloam_b200_global_map_intensity_download.argtypes = [vp, C.c_size_t, C.c_size_t, dp]
+    pk = C.POINTER(PackedScan)
+    L.tloam_b200_segment_raw_scan_packed.argtypes = [vp, C.POINTER(GroundConfig), C.POINTER(DcvcConfig), C.c_int, C.c_double, pk, szp,
+                                                     szp, szp, szp, szp, szp, ip, ip, dp, dp]
+    L.tloam_b200_process_raw_scan_packed.argtypes = [vp, C.POINTER(GroundConfig), C.POINTER(DcvcConfig), C.c_int, C.c_double,
+                                                     C.POINTER(FeatureConfig), C.c_double, C.c_double, pk, szp]
+    L.tloam_b200_global_map_append_packed.argtypes = [vp, dp, pk]
+    L.tloam_b200_global_map_append_packed_chained.argtypes = [vp, pk]
     _lib = L
     return L

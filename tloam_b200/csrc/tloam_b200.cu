@@ -27,6 +27,7 @@
 #include "object_segment.cuh"
 #include "host_stage.h"
 #include "gmap_intensity.h"
+#include "unpack_scan.h"
 
 
 
@@ -187,6 +188,8 @@ struct tloam_b200_handle {
   //      has run since, i.e. while seg_gen == raw_gen ----
   unsigned long long seg_gen = 0, raw_gen = ~0ull;
   const double* raw_scan = nullptr;        size_t raw_n = 0;
+  const double* raw_int = nullptr;         // its intensity (in d_chain) when it came packed with an intensity field
+  unsigned char* d_packed = nullptr;       size_t cap_packed = 0;                               // uploaded packed records
   // ---- global map (tloam_b200_global_map_*, submap.cuh): nothing is allocated or launched until it is enabled ----
   bool gmap_on = false;
   double gmap_voxel = 1.0;
@@ -403,7 +406,7 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   cudaFree(h->d_vox1); cudaFree(h->d_acc_tmp1); cudaFree(h->d_up_planar); cudaFree(h->d_chain); cudaFree(h->d_frame);
   cudaFree(h->d_gmap_st); cudaFree(h->d_gmap_pose); cudaFree(h->d_gmap); cudaFree(h->d_gmap_off); cudaFree(h->d_gmap_reg);
   cudaFree(h->d_gmap_fin);
-  cudaFree(h->d_gmi_st); cudaFree(h->d_gmi_map); cudaFree(h->d_gmi_in); cudaFree(h->d_gmi_scratch);
+  cudaFree(h->d_gmi_st); cudaFree(h->d_gmi_map); cudaFree(h->d_gmi_in); cudaFree(h->d_gmi_scratch); cudaFree(h->d_packed);
   for (auto& pr : h->gmap_probes) { if (pr.ev) cudaEventDestroy(pr.ev); if (pr.h_count) cudaFreeHost(pr.h_count); }
   for (int i = 0; i < 2; ++i) if (h->ev_stage_free[i]) cudaEventDestroy(h->ev_stage_free[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_fit[i]) cudaEventDestroy(h->ev_fit[i]);
@@ -2746,14 +2749,99 @@ __global__ void __launch_bounds__(256) k_chain_final(const unsigned* ground, uns
 }
 }  // namespace
 
-// The one implementation of the chained segmentation.  remove: run RemoveClosedNonFinitePoints(near_dis) on the device
-// first (tloam_b200_segment_raw_scan); tloam_b200_segment_scan runs without that step.  beam / intensity (optional, n
-// values): the channel of every point of the scan as int / FP64 (NaN for removed points).  keep (optional): the three final
-// lists stay on the device (tloam_b200_process_raw_scan) -- the index arrays are not written, *keep receives the uploaded scan
-// and the lists (valid until the handle's next segmentation call); the counts still land in *n_ground / *n_edge / *n_general.
-struct ChainKeep { const double* scan = nullptr; const unsigned long long *ground = nullptr, *edge = nullptr, *general = nullptr; };
+// a library that ships next to this one (libtloam_b200_gmi.so, libtloam_b200_unpack.so): its path in this library's directory
+static std::string sibling_path(const char* file) {
+  Dl_info info;
+  std::string path = file;
+  if (dladdr(reinterpret_cast<void*>(&tloam_b200_last_error), &info) && info.dli_fname) {
+    const std::string self = info.dli_fname;
+    const size_t slash = self.rfind('/');
+    if (slash != std::string::npos) path = self.substr(0, slash + 1) + path;
+  }
+  return path;
+}
+
+// host staging of a copy to the device: pageable memory through HostStage, pinned / registered memory by DMA
+static int upload_host(tloam_b200_handle* h, void* dst, const void* src, size_t bytes) {
+  if (HostStage::pageable(src) && getenv("TLOAM_B200_NO_HOST_STAGE") == nullptr) CU_TRY(h->hstage.upload(dst, src, bytes, h->stream));
+  else CU_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->stream));
+  return TLOAM_B200_OK;
+}
+
+// ---- packed raw scans (tloam_packed_scan): k_unpack_scan lives in libtloam_b200_unpack.so (unpack_scan.cu), loaded on the
+//      first packed call so that the kernels of this library keep their SASS ----
+static std::mutex g_unpack_mu;
+static tloam_unpack_scan_fn g_unpack = nullptr;
+
+static int unpack_load(tloam_b200_handle* h, tloam_unpack_scan_fn* out) {
+  std::lock_guard<std::mutex> lk(g_unpack_mu);
+  if (!g_unpack) {
+    const std::string path = sibling_path("libtloam_b200_unpack.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    tloam_unpack_scan_fn fn = so ? reinterpret_cast<tloam_unpack_scan_fn>(dlsym(so, "tloam_unpack_scan")) : nullptr;
+    if (!fn) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "packed scan: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_unpack = fn;
+  }
+  *out = g_unpack;
+  return TLOAM_B200_OK;
+}
+
+static bool packed_valid(const tloam_packed_scan* s) {
+  if (!s || (!s->data && s->n) || s->point_step < 12 || s->n > ((size_t)1 << 26)) return false;
+  if (s->n && s->point_step > SIZE_MAX / s->n) return false;                 // no such host buffer
+  const int off[4] = {s->x_offset, s->y_offset, s->z_offset, s->intensity_offset};
+  for (int k = 0; k < 4; ++k) {
+    if (k == 3 && off[k] == -1) continue;
+    if (off[k] < 0 || (size_t)off[k] + 4 > s->point_step) return false;
+  }
+  return true;
+}
+
+// one upload of the packed records, then (double)float of every field on the device: xyz (n x 3) and, when `intensity` is
+// not null and the layout has the field, the intensity (n).  The layout has been validated.
+static int unpack_packed(tloam_b200_handle* h, const tloam_packed_scan* s, double* xyz, double* intensity) {
+  if (!s->n) return TLOAM_B200_OK;
+  tloam_unpack_scan_fn unpack;
+  int rc = unpack_load(h, &unpack);
+  if (rc != TLOAM_B200_OK) return rc;
+  const size_t bytes = s->n * s->point_step, padded = round_up(bytes, 16);   // the kernel loads whole 16-byte chunks
+  if (padded > h->cap_packed) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_packed); h->d_packed = nullptr; h->cap_packed = 0;
+    CU_TRY(cudaMalloc(&h->d_packed, padded + padded / 4));
+    h->cap_packed = padded + padded / 4;
+  }
+  if ((rc = upload_host(h, h->d_packed, s->data, bytes)) != TLOAM_B200_OK) return rc;
+  const int off[4] = {s->x_offset, s->y_offset, s->z_offset, s->intensity_offset};
+  int e = 0;
+  TL_LAUNCH(TLOAM_B200_K_GROUND, (e = unpack(h->d_packed, s->n, s->point_step, off, xyz, intensity, h->device, h->stream)));
+  if (e != cudaSuccess) {
+    snprintf(h->last_error, sizeof(h->last_error), "packed scan: k_unpack_scan: %s", cudaGetErrorString((cudaError_t)e));
+    return TLOAM_B200_ERR_CUDA;
+  }
+  return TLOAM_B200_OK;
+}
+
+// the raw scan a chain call starts from: FP64 AoS rows (xyz), or a packed scan unpacked on the device
+struct RawScanIn { const double* xyz = nullptr; const tloam_packed_scan* packed = nullptr; size_t n = 0; };
+
+// The one implementation of the chained segmentation; only the way the scan reaches the device depends on its form (in).
+// remove: run RemoveClosedNonFinitePoints(near_dis) on the device first (tloam_b200_segment_raw_scan); tloam_b200_segment_scan
+// runs without that step.  beam / intensity (optional, n values): the channel of every point of the scan as int / FP64 (NaN
+// for removed points).  keep (optional): the three final lists stay on the device (tloam_b200_process_raw_scan) -- the index
+// arrays are not written, *keep receives the uploaded scan, the intensity of a packed scan with that field (else null) and
+// the lists (valid until the handle's next segmentation call); the counts still land in *n_ground / *n_edge / *n_general.
+struct ChainKeep {
+  const double* scan = nullptr; const double* intensity = nullptr;
+  const unsigned long long *ground = nullptr, *edge = nullptr, *general = nullptr;
+};
 static int segment_chain(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg, int ring_min_num, bool remove,
-                         double near_dis, const double* xyz, size_t n, size_t* ground_index, size_t* n_ground, size_t* edge_index,
+                         double near_dis, const RawScanIn& in, size_t* ground_index, size_t* n_ground, size_t* edge_index,
                          size_t* n_edge, size_t* general_index, size_t* n_general, int* n_clusters, int* sizes, double* boxes, int* beam,
                          double* intensity, ChainKeep* keep = nullptr) {
   if (!h || !gcfg || !dcfg || !ground_index || !n_ground || !edge_index || !n_edge || !general_index || !n_general || !n_clusters)
@@ -2761,8 +2849,10 @@ static int segment_chain(tloam_b200_handle* h, const tloam_ground_config* gcfg, 
   h->seg_gen++;                                           // d_chain (the raw scan of the last process_raw_scan) is rewritten
   *n_ground = *n_edge = *n_general = 0; *n_clusters = 0;
   if (remove && gcfg->sensor_model != 64 && gcfg->sensor_model != 16) return TLOAM_B200_ERR_INVALID_ARG;
+  if (in.packed && !packed_valid(in.packed)) return TLOAM_B200_ERR_INVALID_ARG;
+  const size_t n = in.n;
   if (n == 0) return TLOAM_B200_OK;
-  if (!xyz || n > ((size_t)1 << 26)) return TLOAM_B200_ERR_INVALID_ARG;
+  if ((!in.packed && !in.xyz) || n > ((size_t)1 << 26)) return TLOAM_B200_ERR_INVALID_ARG;
   CU_TRY(cudaSetDevice(h->device));
   // chain buffer: what must outlive a stage's arena
   const unsigned nchunk = (unsigned)((n + kGeChunk - 1) / kGeChunk);
@@ -2772,6 +2862,8 @@ static int segment_chain(tloam_b200_handle* h, const tloam_ground_config* gcfg, 
                o_spts = take(n * 24), o_sbeam = take(n * 8), o_sorig = take(n * 4), o_fg = take(n * 8), o_fe = take(n * 8), o_fn = take(n * 8),
                o_beam = take(n * 4), o_kept = remove ? take(n * 24) : 0, o_map = remove ? take(n * 4) : 0,
                o_rmc = remove ? take(nchunk * 4 + 64) : 0, o_int = intensity ? take(n * 8) : 0, o_fi = intensity ? take(n * 8) : 0;
+  const bool keep_int = keep && in.packed && in.packed->intensity_offset >= 0;
+  const size_t o_pint = keep_int ? take(n * 8) : 0;
   if (off > h->cap_chain) {
     CU_TRY(cudaStreamSynchronize(h->stream));
     cudaFree(h->d_chain); h->d_chain = nullptr; h->cap_chain = 0;
@@ -2785,8 +2877,9 @@ static int segment_chain(tloam_b200_handle* h, const tloam_ground_config* gcfg, 
   double* d_spts = (double*)(c + o_spts); double* d_sbeam = (double*)(c + o_sbeam); unsigned* d_sorig = (unsigned*)(c + o_sorig);
   unsigned long long* d_fg = (unsigned long long*)(c + o_fg); unsigned long long* d_fe = (unsigned long long*)(c + o_fe);
   unsigned long long* d_fn = (unsigned long long*)(c + o_fn);
-  if (HostStage::pageable(xyz) && getenv("TLOAM_B200_NO_HOST_STAGE") == nullptr) CU_TRY(h->hstage.upload(d_scan, xyz, n * 24, h->stream));
-  else CU_TRY(cudaMemcpyAsync(d_scan, xyz, n * 24, cudaMemcpyHostToDevice, h->stream));
+  double* d_pint = keep_int ? (double*)(c + o_pint) : nullptr;
+  int rc = in.packed ? unpack_packed(h, in.packed, d_scan, d_pint) : upload_host(h, d_scan, in.xyz, n * 24);
+  if (rc != TLOAM_B200_OK) return rc;
   struct Reset { tloam_b200_handle* h; ~Reset() { h->seg = tloam_b200_handle::SegChain(); } } reset{h};
   // ---- 0. RemoveClosedNonFinitePoints (:48, :472-499): kept points + kept -> raw map ----
   const double* pts = d_scan;
@@ -2813,8 +2906,8 @@ static int segment_chain(tloam_b200_handle* h, const tloam_ground_config* gcfg, 
     h->seg.active = true;
     // ---- 1. groundRemove ----
     h->seg.dev_xyz = pts;
-    int rc = ground_run(h, gcfg, xyz, nk, ground_index, &ng, general_index /*scratch: not written when chained*/, &no, nullptr, nullptr,
-                        nullptr, nullptr, nullptr);
+    rc = ground_run(h, gcfg, pts /*placeholder: read on the device*/, nk, ground_index, &ng, general_index /*scratch: not written when
+                    chained*/, &no, nullptr, nullptr, nullptr, nullptr, nullptr);
     if (rc != TLOAM_B200_OK) return rc;
     if (ng) CU_TRY(cudaMemcpyAsync(d_gnd, h->seg.ground, ng * 4, cudaMemcpyDeviceToDevice, h->stream));
     if (beam) CU_TRY(cudaMemcpyAsync(c + o_beam, h->seg.beam, nk * 4, cudaMemcpyDeviceToDevice, h->stream));
@@ -2853,7 +2946,7 @@ static int segment_chain(tloam_b200_handle* h, const tloam_ground_config* gcfg, 
     if (ne && !keep) CU_TRY(cudaMemcpyAsync(edge_index, d_fe, ne * 8, cudaMemcpyDeviceToHost, h->stream));
     if (nn && !keep) CU_TRY(cudaMemcpyAsync(general_index, d_fn, nn * 8, cudaMemcpyDeviceToHost, h->stream));
   }
-  if (keep) { keep->scan = d_scan; keep->ground = d_fg; keep->edge = d_fe; keep->general = d_fn; }
+  if (keep) { keep->scan = d_scan; keep->intensity = d_pint; keep->ground = d_fg; keep->edge = d_fe; keep->general = d_fn; }
   if (beam) CU_TRY(cudaMemcpyAsync(beam, c + o_beam, n * 4, cudaMemcpyDeviceToHost, h->stream));
   if (intensity) CU_TRY(cudaMemcpyAsync(intensity, c + o_fi, n * 8, cudaMemcpyDeviceToHost, h->stream));
   CU_TRY(cudaStreamSynchronize(h->stream));
@@ -2864,7 +2957,9 @@ static int segment_chain(tloam_b200_handle* h, const tloam_ground_config* gcfg, 
 int tloam_b200_segment_scan(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg, int ring_min_num,
                             const double* xyz, size_t n, size_t* ground_index, size_t* n_ground, size_t* edge_index, size_t* n_edge,
                             size_t* general_index, size_t* n_general, int* n_clusters, int* sizes, double* boxes, int* beam) {
-  return segment_chain(h, gcfg, dcfg, ring_min_num, false, 0.0, xyz, n, ground_index, n_ground, edge_index, n_edge, general_index, n_general,
+  RawScanIn in;
+  in.xyz = xyz; in.n = n;
+  return segment_chain(h, gcfg, dcfg, ring_min_num, false, 0.0, in, ground_index, n_ground, edge_index, n_edge, general_index, n_general,
                        n_clusters, sizes, boxes, beam, nullptr);
 }
 
@@ -2872,7 +2967,20 @@ int tloam_b200_segment_raw_scan(tloam_b200_handle* h, const tloam_ground_config*
                                 double near_dis, const double* xyz, size_t n, size_t* ground_index, size_t* n_ground, size_t* edge_index,
                                 size_t* n_edge, size_t* general_index, size_t* n_general, int* n_clusters, int* sizes, double* boxes,
                                 double* intensity) {
-  return segment_chain(h, gcfg, dcfg, ring_min_num, true, near_dis, xyz, n, ground_index, n_ground, edge_index, n_edge, general_index, n_general,
+  RawScanIn in;
+  in.xyz = xyz; in.n = n;
+  return segment_chain(h, gcfg, dcfg, ring_min_num, true, near_dis, in, ground_index, n_ground, edge_index, n_edge, general_index, n_general,
+                       n_clusters, sizes, boxes, nullptr, intensity);
+}
+
+int tloam_b200_segment_raw_scan_packed(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg,
+                                       int ring_min_num, double near_dis, const tloam_packed_scan* scan, size_t* ground_index,
+                                       size_t* n_ground, size_t* edge_index, size_t* n_edge, size_t* general_index, size_t* n_general,
+                                       int* n_clusters, int* sizes, double* boxes, double* intensity) {
+  if (!scan) return TLOAM_B200_ERR_INVALID_ARG;
+  RawScanIn in;
+  in.packed = scan; in.n = scan->n;
+  return segment_chain(h, gcfg, dcfg, ring_min_num, true, near_dis, in, ground_index, n_ground, edge_index, n_edge, general_index, n_general,
                        n_clusters, sizes, boxes, nullptr, intensity);
 }
 
@@ -2974,10 +3082,10 @@ int tloam_b200_process_cloud(tloam_b200_handle* h, const tloam_feature_config* f
   return process_frame(h, fcfg, ground_down_sample, edge_down_sample, ng, ne, nn, n_source);
 }
 
-int tloam_b200_process_raw_scan(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg, int ring_min_num,
-                                double near_dis, const tloam_feature_config* fcfg, double ground_down_sample, double edge_down_sample,
-                                const double* xyz, size_t n, size_t n_source[4]) {
-  if (!h || !gcfg || !dcfg || !fcfg || !n_source || (!xyz && n)) return TLOAM_B200_ERR_INVALID_ARG;
+static int process_raw(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg, int ring_min_num,
+                       double near_dis, const tloam_feature_config* fcfg, double ground_down_sample, double edge_down_sample,
+                       const RawScanIn& in, size_t n_source[4]) {
+  if (!h || !gcfg || !dcfg || !fcfg || !n_source || (!in.packed && !in.xyz && in.n)) return TLOAM_B200_ERR_INVALID_ARG;
   for (int k = 0; k < 4; ++k) n_source[k] = 0;
   if (!(ground_down_sample > 0.0) || !(edge_down_sample > 0.0)) return TLOAM_B200_ERR_INVALID_ARG;
   CU_TRY(cudaSetDevice(h->device));
@@ -2986,7 +3094,7 @@ int tloam_b200_process_raw_scan(tloam_b200_handle* h, const tloam_ground_config*
   size_t ng = 0, ne = 0, nn = 0;
   int n_clusters = 0;
   ChainKeep keep;
-  int rc = segment_chain(h, gcfg, dcfg, ring_min_num, true, near_dis, xyz, n, unused, &ng, unused, &ne, unused, &nn, &n_clusters, nullptr,
+  int rc = segment_chain(h, gcfg, dcfg, ring_min_num, true, near_dis, in, unused, &ng, unused, &ne, unused, &nn, &n_clusters, nullptr,
                          nullptr, nullptr, nullptr, &keep);
   if (rc != TLOAM_B200_OK) return rc;
   if ((rc = reserve_frame(h, ng, ne, nn)) != TLOAM_B200_OK) return rc;
@@ -3000,8 +3108,25 @@ int tloam_b200_process_raw_scan(tloam_b200_handle* h, const tloam_ground_config*
   }
   CU_TRY(cudaGetLastError());
   if ((rc = process_frame(h, fcfg, ground_down_sample, edge_down_sample, ng, ne, nn, n_source)) != TLOAM_B200_OK) return rc;
-  h->raw_scan = keep.scan; h->raw_n = n; h->raw_gen = h->seg_gen;   // for tloam_b200_global_map_append_frame*
+  h->raw_scan = keep.scan; h->raw_int = keep.intensity; h->raw_n = in.n; h->raw_gen = h->seg_gen;   // for global_map_append_frame*
   return TLOAM_B200_OK;
+}
+
+int tloam_b200_process_raw_scan(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg, int ring_min_num,
+                                double near_dis, const tloam_feature_config* fcfg, double ground_down_sample, double edge_down_sample,
+                                const double* xyz, size_t n, size_t n_source[4]) {
+  RawScanIn in;
+  in.xyz = xyz; in.n = n;
+  return process_raw(h, gcfg, dcfg, ring_min_num, near_dis, fcfg, ground_down_sample, edge_down_sample, in, n_source);
+}
+
+int tloam_b200_process_raw_scan_packed(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg,
+                                       int ring_min_num, double near_dis, const tloam_feature_config* fcfg, double ground_down_sample,
+                                       double edge_down_sample, const tloam_packed_scan* scan, size_t n_source[4]) {
+  if (!scan) return TLOAM_B200_ERR_INVALID_ARG;
+  RawScanIn in;
+  in.packed = scan; in.n = scan->n;
+  return process_raw(h, gcfg, dcfg, ring_min_num, near_dis, fcfg, ground_down_sample, edge_down_sample, in, n_source);
 }
 
 int tloam_b200_source_download(tloam_b200_handle* h, int cloud, double* out, size_t capacity_points) {
@@ -3153,13 +3278,7 @@ static GmiLib g_gmi;
 static int gmi_load(tloam_b200_handle* h, GmiLib* out) {
   std::lock_guard<std::mutex> lk(g_gmi_mu);
   if (!g_gmi.append) {
-    Dl_info info;
-    std::string path = "libtloam_b200_gmi.so";
-    if (dladdr(reinterpret_cast<void*>(&tloam_b200_global_map_has_intensity), &info) && info.dli_fname) {
-      const std::string self = info.dli_fname;
-      const size_t slash = self.rfind('/');
-      if (slash != std::string::npos) path = self.substr(0, slash + 1) + path;
-    }
+    const std::string path = sibling_path("libtloam_b200_gmi.so");
     void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
     GmiLib l;
     if (so) {
@@ -3192,13 +3311,6 @@ static int gmi_prepare(tloam_b200_handle* h, const GmiLib& lib, size_t n) {
     CU_TRY(cudaMemsetAsync(h->d_gmi_st, 0, 2 * sizeof(unsigned), h->stream));
   }
   if (!h->d_gmi_map) CU_TRY(cudaMalloc(&h->d_gmi_map, h->cap_gmap * sizeof(double)));
-  if (n > h->cap_gmi_in) {
-    const size_t ncap = n + n / 2 + 1024;
-    CU_TRY(cudaStreamSynchronize(h->stream));
-    cudaFree(h->d_gmi_in); h->d_gmi_in = nullptr; h->cap_gmi_in = 0;
-    CU_TRY(cudaMalloc(&h->d_gmi_in, ncap * sizeof(double)));
-    h->cap_gmi_in = ncap;
-  }
   const size_t bytes = lib.scratch_bytes((unsigned)n);
   if (bytes > h->cap_gmi_scratch) {
     CU_TRY(cudaStreamSynchronize(h->stream));
@@ -3209,39 +3321,34 @@ static int gmi_prepare(tloam_b200_handle* h, const GmiLib& lib, size_t n) {
   return TLOAM_B200_OK;
 }
 
-// global_map += (T . raw).VoxelDownSample(voxel).  d_raw: a device raw scan read in place, or nullptr: xyz_host is uploaded
-// into the registered-scan buffer and transformed there.  pose_host == nullptr: the device-side result of the frame just
-// enqueued (as submap_update_impl's chained form).  int_host: the raw scan's intensity (n host values), or nullptr: the frame
-// has no intensity channel.
-static int gmap_append_impl(tloam_b200_handle* h, const double* pose_host, const double* xyz_host, const double* d_raw, size_t n,
-                            const double* int_host = nullptr) {
-  if (n > ((size_t)1 << 30)) return TLOAM_B200_ERR_INVALID_ARG;
+// d_gmi_in holds the intensity of a host frame of n rows (uploaded or unpacked there)
+static int gmi_reserve_in(tloam_b200_handle* h, size_t n) {
+  if (n <= h->cap_gmi_in) return TLOAM_B200_OK;
+  const size_t ncap = n + n / 2 + 1024;
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  cudaFree(h->d_gmi_in); h->d_gmi_in = nullptr; h->cap_gmi_in = 0;
+  CU_TRY(cudaMalloc(&h->d_gmi_in, ncap * sizeof(double)));
+  h->cap_gmi_in = ncap;
+  return TLOAM_B200_OK;
+}
+
+// global_map += (T . raw).VoxelDownSample(voxel).  d_in: the raw scan on the device -- read in place, or the registered-scan
+// buffer the host frame was staged into (transformed there).  pose_host == nullptr: the device-side result of the frame just
+// enqueued (as submap_update_impl's chained form).  d_int: the raw scan's intensity on the device (n values), or nullptr: the
+// frame has no intensity channel.
+static int gmap_append_impl(tloam_b200_handle* h, const double* pose_host, const double* d_in, size_t n, const double* d_int) {
   CU_TRY(cudaSetDevice(h->device));
   int rc;
   GmiLib gmi;
-  const bool with_int = int_host && n;     // an empty frame adds nothing: the channel is left as it is
+  const bool with_int = d_int && n;        // an empty frame adds nothing: the channel is left as it is
   if ((with_int || h->gmi_used) && (rc = gmi_load(h, &gmi)) != TLOAM_B200_OK) return rc;
   gmap_harvest(h);
   const unsigned long long bound = h->gmap_known + (h->gmap_cum - h->gmap_known_cum) + n;   // voxels <= finite rows <= rows
   if (bound > h->cap_gmap || h->gmap_calls + 2 > h->cap_gmap_off)
     if ((rc = gmap_grow(h, n)) != TLOAM_B200_OK) return rc;
-  if (with_int) {
-    if ((rc = gmi_prepare(h, gmi, n)) != TLOAM_B200_OK) return rc;
-    if (HostStage::pageable(int_host) && getenv("TLOAM_B200_NO_HOST_STAGE") == nullptr)
-      CU_TRY(h->hstage.upload(h->d_gmi_in, int_host, n * 8, h->stream));
-    else
-      CU_TRY(cudaMemcpyAsync(h->d_gmi_in, int_host, n * 8, cudaMemcpyHostToDevice, h->stream));
-  }
+  if (with_int && (rc = gmi_prepare(h, gmi, n)) != TLOAM_B200_OK) return rc;
   if ((rc = ensure_dev(h, &h->d_gmap_reg, &h->cap_gmap_reg, n, false)) != TLOAM_B200_OK) return rc;
   if ((rc = ensure_dev(h, &h->d_gmap_fin, &h->cap_gmap_fin, n, false)) != TLOAM_B200_OK) return rc;
-  const double* d_in = d_raw;
-  if (!d_raw && n) {                       // the only point data that crosses PCIe
-    if (HostStage::pageable(xyz_host) && getenv("TLOAM_B200_NO_HOST_STAGE") == nullptr)
-      CU_TRY(h->hstage.upload(h->d_gmap_reg, xyz_host, n * 24, h->stream));
-    else
-      CU_TRY(cudaMemcpyAsync(h->d_gmap_reg, xyz_host, n * 24, cudaMemcpyHostToDevice, h->stream));
-    d_in = h->d_gmap_reg;
-  }
   const double* d_pose = h->d_gmap_pose;
   if (pose_host) {
     double tmp[16];
@@ -3262,7 +3369,7 @@ static int gmap_append_impl(tloam_b200_handle* h, const double* pose_host, const
   // the intensity channel, while st->count is still the frame's base (gmap_intensity.cu)
   if (with_int) {
     tloam_gmi_frame f;
-    f.reg = h->d_gmap_reg; f.intensity = h->d_gmi_in; f.n = (unsigned)n;
+    f.reg = h->d_gmap_reg; f.intensity = d_int; f.n = (unsigned)n;
     f.minenc = vs.a.minenc; f.voxel = h->gmap_voxel; f.keys_sorted = vs.keys; f.n_vox = &st->n_vox; f.refused = &st->refused;
     f.count = &st->count; f.frames = &st->frames; f.cap = h->cap_gmap; f.frame_cap = h->cap_gmap_off;
     f.map_intensity = h->d_gmi_map; f.state = h->d_gmi_st; f.fresh = h->gmi_used ? 0 : 1; f.scratch = h->d_gmi_scratch;
@@ -3293,23 +3400,52 @@ static int gmap_append_impl(tloam_b200_handle* h, const double* pose_host, const
   return TLOAM_B200_OK;
 }
 
+// a host frame: its rows are staged in the registered-scan buffer (transformed there) and its intensity, if any, in
+// d_gmi_in -- uploaded as FP64 (xyz, inten), or uploaded packed and unpacked on the device (packed, n == packed->n).  The
+// only point data that crosses PCIe.
+static int gmap_append_host(tloam_b200_handle* h, const double* pose_host, const double* xyz, const double* inten,
+                            const tloam_packed_scan* packed, size_t n) {
+  if (n > ((size_t)1 << 30)) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  const bool with_int = packed ? packed->intensity_offset >= 0 : inten != nullptr;
+  int rc;
+  if ((rc = ensure_dev(h, &h->d_gmap_reg, &h->cap_gmap_reg, n, false)) != TLOAM_B200_OK) return rc;
+  if (with_int && (rc = gmi_reserve_in(h, n)) != TLOAM_B200_OK) return rc;
+  if (packed) {
+    if ((rc = unpack_packed(h, packed, h->d_gmap_reg, with_int ? h->d_gmi_in : nullptr)) != TLOAM_B200_OK) return rc;
+  } else if (n) {
+    if ((rc = upload_host(h, h->d_gmap_reg, xyz, n * 24)) != TLOAM_B200_OK) return rc;
+    if (with_int && (rc = upload_host(h, h->d_gmi_in, inten, n * 8)) != TLOAM_B200_OK) return rc;
+  }
+  return gmap_append_impl(h, pose_host, h->d_gmap_reg, n, with_int ? h->d_gmi_in : nullptr);
+}
+
 int tloam_b200_global_map_append(tloam_b200_handle* h, const double pose[16], const double* xyz, size_t n) {
   if (!h || !pose || (!xyz && n)) return TLOAM_B200_ERR_INVALID_ARG;
   if (!h->gmap_on) return TLOAM_B200_ERR_NOT_READY;
-  return gmap_append_impl(h, pose, xyz, nullptr, n);
+  return gmap_append_host(h, pose, xyz, nullptr, nullptr, n);
 }
 
 int tloam_b200_global_map_append_chained(tloam_b200_handle* h, const double* xyz, size_t n) {
   if (!h || (!xyz && n)) return TLOAM_B200_ERR_INVALID_ARG;
   if (!h->gmap_on) return TLOAM_B200_ERR_NOT_READY;
-  return gmap_append_impl(h, nullptr, xyz, nullptr, n);
+  return gmap_append_host(h, nullptr, xyz, nullptr, nullptr, n);
 }
 
 // the raw scan is read where process_raw_scan uploaded it (d_chain); any segmentation / process call since may have
-// reused that buffer, so the generation must still match
-static int gmap_append_frame(tloam_b200_handle* h, const double* pose) {
+// reused that buffer, so the generation must still match.  inten: an explicit host intensity (n values, uploaded), else the
+// intensity a packed process_raw_scan left beside the raw scan (read in place), if any.
+static int gmap_append_frame(tloam_b200_handle* h, const double* pose, const double* inten = nullptr) {
   if (!h->gmap_on || h->raw_gen != h->seg_gen) return TLOAM_B200_ERR_NOT_READY;
-  return gmap_append_impl(h, pose, nullptr, h->raw_scan, h->raw_n);
+  const double* d_int = h->raw_int;
+  if (inten) {
+    CU_TRY(cudaSetDevice(h->device));
+    int rc;
+    if ((rc = gmi_reserve_in(h, h->raw_n)) != TLOAM_B200_OK) return rc;
+    if (h->raw_n && (rc = upload_host(h, h->d_gmi_in, inten, h->raw_n * 8)) != TLOAM_B200_OK) return rc;
+    d_int = h->d_gmi_in;
+  }
+  return gmap_append_impl(h, pose, h->raw_scan, h->raw_n, d_int);
 }
 
 int tloam_b200_global_map_append_frame(tloam_b200_handle* h, const double pose[16]) {
@@ -3401,25 +3537,35 @@ int tloam_b200_global_map_append_intensity(tloam_b200_handle* h, const double po
                                            size_t n) {
   if (!h || !pose || (!xyz && n) || !intensity) return TLOAM_B200_ERR_INVALID_ARG;
   if (!h->gmap_on) return TLOAM_B200_ERR_NOT_READY;
-  return gmap_append_impl(h, pose, xyz, nullptr, n, intensity);
+  return gmap_append_host(h, pose, xyz, intensity, nullptr, n);
 }
 
 int tloam_b200_global_map_append_intensity_chained(tloam_b200_handle* h, const double* xyz, const double* intensity, size_t n) {
   if (!h || (!xyz && n) || !intensity) return TLOAM_B200_ERR_INVALID_ARG;
   if (!h->gmap_on) return TLOAM_B200_ERR_NOT_READY;
-  return gmap_append_impl(h, nullptr, xyz, nullptr, n, intensity);
+  return gmap_append_host(h, nullptr, xyz, intensity, nullptr, n);
 }
 
 int tloam_b200_global_map_append_frame_intensity(tloam_b200_handle* h, const double pose[16], const double* intensity) {
   if (!h || !pose || !intensity) return TLOAM_B200_ERR_INVALID_ARG;
-  if (!h->gmap_on || h->raw_gen != h->seg_gen) return TLOAM_B200_ERR_NOT_READY;
-  return gmap_append_impl(h, pose, nullptr, h->raw_scan, h->raw_n, intensity);
+  return gmap_append_frame(h, pose, intensity);
 }
 
 int tloam_b200_global_map_append_frame_intensity_chained(tloam_b200_handle* h, const double* intensity) {
   if (!h || !intensity) return TLOAM_B200_ERR_INVALID_ARG;
-  if (!h->gmap_on || h->raw_gen != h->seg_gen) return TLOAM_B200_ERR_NOT_READY;
-  return gmap_append_impl(h, nullptr, nullptr, h->raw_scan, h->raw_n, intensity);
+  return gmap_append_frame(h, nullptr, intensity);
+}
+
+int tloam_b200_global_map_append_packed(tloam_b200_handle* h, const double pose[16], const tloam_packed_scan* scan) {
+  if (!h || !pose || !packed_valid(scan)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on) return TLOAM_B200_ERR_NOT_READY;
+  return gmap_append_host(h, pose, nullptr, nullptr, scan, scan->n);
+}
+
+int tloam_b200_global_map_append_packed_chained(tloam_b200_handle* h, const tloam_packed_scan* scan) {
+  if (!h || !packed_valid(scan)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on) return TLOAM_B200_ERR_NOT_READY;
+  return gmap_append_host(h, nullptr, nullptr, nullptr, scan, scan->n);
 }
 
 // synchronises (gmap_read: the sticky flags of the xyz map) and reads whether the map has the channel (PointCloud2::

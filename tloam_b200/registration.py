@@ -45,6 +45,45 @@ def _f64(a):
     return np.ascontiguousarray(a, dtype=np.float64)
 
 
+_F32 = np.dtype("<f4")
+
+
+def packed_scan(arr):
+    """The tloam_packed_scan descriptor of a raw scan in the sensor's own float32 layout, for the *_packed calls (one upload,
+    unpacked on the device).  arr is one of
+      - a numpy structured array (a PointCloud2's records: np.frombuffer(msg.data, dtype)) with little-endian float32 fields
+        x, y, z and optionally intensity, any itemsize and offsets;
+      - a float32 (n, 4) array (a KITTI .bin scan: np.fromfile(path, "<f4").reshape(-1, 4)), intensity in column 3;
+      - a float32 (n, 3) array, no intensity.
+    It must be C-contiguous; anything else raises ValueError.  The descriptor keeps a reference to arr."""
+    if not isinstance(arr, np.ndarray) or not arr.flags.c_contiguous:
+        raise ValueError("packed_scan: a C-contiguous numpy array is required")
+    fields = arr.dtype.fields
+    if fields is not None:
+        off = {}
+        for name in ("x", "y", "z", "intensity"):
+            if name not in fields:
+                if name == "intensity":
+                    continue
+                raise ValueError(f"packed_scan: the records have no field {name!r}")
+            dt, o = fields[name][:2]
+            if dt != _F32:
+                raise ValueError(f"packed_scan: field {name!r} is {dt.str}, not little-endian float32")
+            off[name] = o
+        d = _lib.PackedScan(arr.ctypes.data, arr.size, arr.dtype.itemsize, off["x"], off["y"], off["z"], off.get("intensity", -1))
+    elif arr.dtype == _F32 and arr.ndim == 2 and arr.shape[1] in (3, 4):
+        d = _lib.PackedScan(arr.ctypes.data, arr.shape[0], 4 * arr.shape[1], 0, 4, 8, 12 if arr.shape[1] == 4 else -1)
+    else:
+        raise ValueError(f"packed_scan: {arr.dtype.str} array of shape {arr.shape} is neither structured records nor float32 "
+                         "(n, 3) / (n, 4)")
+    d._keep = arr
+    return d
+
+
+def _packed(scan):
+    return scan if isinstance(scan, _lib.PackedScan) else packed_scan(scan)
+
+
 class Frame:
     """Mirror of tloam::Frame (ref: registration_interface.hpp:19-38): the four feature clouds, (n,3) float64.
     scan_cloud is accepted and ignored, as in the reference (registration.cpp:232-239)."""
@@ -434,13 +473,7 @@ class LocalRegistration:
         return dict(ground=g[:ng.value].copy(), edge=e[:ne.value].copy(), general=o[:no.value].copy(), sizes=sizes[:k].copy(),
                     boxes=boxes[:k].copy(), beam=beam[:n].copy())
 
-    def segment_raw_scan(self, scan, near_dis=3.0, ring_min_num=131, ground=None, dcvc=None):
-        """RemoveClosedNonFinitePoints(near_dis) -> groundRemove -> objectSegmentation -> extractEdgePoint on the device, the
-        raw scan as the driver delivers it (NaN / Inf rows allowed; a point is kept iff its norm is >= near_dis**2, as in the
-        reference).  Returns dict(ground, edge, general, sizes, boxes, intensity): index lists into the RAW scan, the cluster
-        table, the FP64 channel per raw point (NaN where removed).  ground / dcvc: dicts of configuration overrides."""
-        a = _f64(scan).reshape(-1, 3)
-        n = a.shape[0]
+    def _segmentation_configs(self, ground, dcvc):
         gc, dc = _lib.GroundConfig(), _lib.DcvcConfig()
         self._L.tloam_b200_ground_default_config(C.byref(gc))
         self._L.tloam_b200_dcvc_default_config(C.byref(dc))
@@ -448,6 +481,24 @@ class LocalRegistration:
             setattr(gc, k, v)
         for k, v in (dcvc or {}).items():
             setattr(dc, k, v)
+        return gc, dc
+
+    def segment_raw_scan(self, scan, near_dis=3.0, ring_min_num=131, ground=None, dcvc=None):
+        """RemoveClosedNonFinitePoints(near_dis) -> groundRemove -> objectSegmentation -> extractEdgePoint on the device, the
+        raw scan as the driver delivers it (NaN / Inf rows allowed; a point is kept iff its norm is >= near_dis**2, as in the
+        reference).  Returns dict(ground, edge, general, sizes, boxes, intensity): index lists into the RAW scan, the cluster
+        table, the FP64 channel per raw point (NaN where removed).  ground / dcvc: dicts of configuration overrides."""
+        a = _f64(scan).reshape(-1, 3)
+        return self._segment_raw("segment_raw_scan", (_dp(a), a.shape[0]), a.shape[0], near_dis, ring_min_num, ground, dcvc)
+
+    def segment_raw_scan_packed(self, scan, near_dis=3.0, ring_min_num=131, ground=None, dcvc=None):
+        """segment_raw_scan of a raw scan in the sensor's float32 layout (a packed_scan descriptor, or an array packed_scan
+        accepts): one upload, unpacked on the device.  Its intensity field is not read; the result is segment_raw_scan's."""
+        d = _packed(scan)
+        return self._segment_raw("segment_raw_scan_packed", (C.byref(d),), d.n, near_dis, ring_min_num, ground, dcvc)
+
+    def _segment_raw(self, fn, scan_args, n, near_dis, ring_min_num, ground, dcvc):
+        gc, dc = self._segmentation_configs(ground, dcvc)
         m = max(n, 1)
         g, e, o = (np.zeros(m, dtype=np.uintp) for _ in range(3))
         ng, ne, no = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
@@ -456,10 +507,10 @@ class LocalRegistration:
         inten = np.zeros(m)
         boxes = np.zeros((m, 6))
         szp, ip = C.POINTER(C.c_size_t), C.POINTER(C.c_int)
-        self._check(self._L.tloam_b200_segment_raw_scan(self._h, C.byref(gc), C.byref(dc), ring_min_num, float(near_dis), _dp(a), n,
-                                                        g.ctypes.data_as(szp), C.byref(ng), e.ctypes.data_as(szp), C.byref(ne),
-                                                        o.ctypes.data_as(szp), C.byref(no), C.byref(ncl), sizes.ctypes.data_as(ip),
-                                                        _dp(boxes), _dp(inten)), "segment_raw_scan")
+        self._check(getattr(self._L, "tloam_b200_" + fn)(self._h, C.byref(gc), C.byref(dc), ring_min_num, float(near_dis), *scan_args,
+                                                         g.ctypes.data_as(szp), C.byref(ng), e.ctypes.data_as(szp), C.byref(ne),
+                                                         o.ctypes.data_as(szp), C.byref(no), C.byref(ncl), sizes.ctypes.data_as(ip),
+                                                         _dp(boxes), _dp(inten)), fn)
         k = ncl.value
         return dict(ground=g[:ng.value].copy(), edge=e[:ne.value].copy(), general=o[:no.value].copy(), sizes=sizes[:k].copy(),
                     boxes=boxes[:k].copy(), intensity=inten[:n].copy())
@@ -490,20 +541,26 @@ class LocalRegistration:
         """segment_raw_scan -> process_cloud on the device with one upload of the raw scan and no index list going home.
         ground / dcvc / feature: dicts of configuration overrides.  Returns the four source sizes."""
         a = _f64(scan).reshape(-1, 3)
-        gc, dc = _lib.GroundConfig(), _lib.DcvcConfig()
-        self._L.tloam_b200_ground_default_config(C.byref(gc))
-        self._L.tloam_b200_dcvc_default_config(C.byref(dc))
-        for k, v in (ground or {}).items():
-            setattr(gc, k, v)
-        for k, v in (dcvc or {}).items():
-            setattr(dc, k, v)
+        return self._process_raw("process_raw_scan", (_dp(a), a.shape[0]), a.shape[0], near_dis, ring_min_num, ground, dcvc, feature,
+                                 ground_down_sample, edge_down_sample)
+
+    def process_raw_scan_packed(self, scan, near_dis=3.0, ring_min_num=131, ground=None, dcvc=None, feature=None, ground_down_sample=0.3,
+                                edge_down_sample=0.1):
+        """process_raw_scan of a raw scan in the sensor's float32 layout (a packed_scan descriptor, or an array packed_scan
+        accepts): one upload, unpacked on the device.  With an intensity field, global_map_append_frame() appends the frame
+        with that intensity, read on the device."""
+        d = _packed(scan)
+        return self._process_raw("process_raw_scan_packed", (C.byref(d),), d.n, near_dis, ring_min_num, ground, dcvc, feature,
+                                 ground_down_sample, edge_down_sample)
+
+    def _process_raw(self, fn, scan_args, n, near_dis, ring_min_num, ground, dcvc, feature, ground_down_sample, edge_down_sample):
+        gc, dc = self._segmentation_configs(ground, dcvc)
         fc = self._feature_config(feature or {})
         ns = (C.c_size_t * 4)()
-        self._check(self._L.tloam_b200_process_raw_scan(self._h, C.byref(gc), C.byref(dc), ring_min_num, float(near_dis), C.byref(fc),
-                                                        float(ground_down_sample), float(edge_down_sample), _dp(a), a.shape[0], ns),
-                    "process_raw_scan")
+        self._check(getattr(self._L, "tloam_b200_" + fn)(self._h, C.byref(gc), C.byref(dc), ring_min_num, float(near_dis), C.byref(fc),
+                                                         float(ground_down_sample), float(edge_down_sample), *scan_args, ns), fn)
         self.n_source = [int(v) for v in ns]
-        self._raw_scan_rows = a.shape[0]       # global_map_append_frame(intensity=...) takes one value per row
+        self._raw_scan_rows = n                # global_map_append_frame(intensity=...) takes one value per row
         return list(self.n_source)
 
     def source_cloud(self, cloud):
@@ -560,9 +617,20 @@ class LocalRegistration:
             rc = self._L.tloam_b200_global_map_append(self._h, _dp(p), _dp(a), a.shape[0])
         self._check(rc, "global_map_append")
 
+    def global_map_append_packed(self, scan, pose=None):
+        """global_map_append of a host raw scan in the sensor's float32 layout (a packed_scan descriptor, or an array
+        packed_scan accepts): one upload, unpacked on the device.  With an intensity field it is an intensity frame."""
+        d = _packed(scan)
+        if pose is None:
+            rc = self._L.tloam_b200_global_map_append_packed_chained(self._h, C.byref(d))
+        else:
+            p = _f64(np.asarray(pose).T).reshape(16)
+            rc = self._L.tloam_b200_global_map_append_packed(self._h, _dp(p), C.byref(d))
+        self._check(rc, "global_map_append_packed")
+
     def global_map_append_frame(self, pose=None, intensity=None):
         """append the raw scan the last process_raw_scan uploaded (read on the device); pose None = chained.  intensity: one
-        value per row of that scan, or None"""
+        value per row of that scan, or None (after process_raw_scan_packed with an intensity field: that intensity)"""
         p = None if pose is None else _f64(np.asarray(pose).T).reshape(16)
         if intensity is not None:
             v = self._intensity(intensity, getattr(self, "_raw_scan_rows", 0))

@@ -41,11 +41,22 @@ print("global map intensity", r.global_map_size(), r.global_map_has_intensity())
 r.reset_global_map()
 r.global_map_append(scan, T, intensity=inten[:len(scan)])
 print("intensity", r.global_map_intensity()[:3])
+# packed scans (libtloam_b200_unpack.so): a 22-byte velodyne XYZIRT message and a KITTI (n, 4) scan
+dt = np.dtype(dict(names=["x", "y", "z", "intensity", "ring", "time"], formats=["<f4"] * 4 + ["<u2", "<f4"], offsets=[0, 4, 8, 12, 16, 18], itemsize=22))
+msg = np.zeros(len(scan) + 10, dt)
+f = np.vstack([scan, np.full((10, 3), np.nan)]).astype(np.float32)
+msg["x"], msg["y"], msg["z"], msg["intensity"] = f[:, 0], f[:, 1], f[:, 2], inten.astype(np.float32)
+print("segment_raw_scan_packed", {k: len(v) for k, v in r.segment_raw_scan_packed(msg, ring_min_num=16, dcvc=dict(min_seg=20)).items()})
+print("process_raw_scan_packed", r.process_raw_scan_packed(msg, ring_min_num=16, dcvc=dict(min_seg=20), feature=fe))
+r.global_map_append_frame(T)                                                                # the packed intensity, on the device
+r.global_map_append_packed(np.ascontiguousarray(np.column_stack([f, inten.astype(np.float32)])), T)
+r.global_map_append_packed(np.ascontiguousarray(f[:333]), None)
+print("packed", r.global_map_size(), r.global_map_has_intensity())
 r.close()
 PY
 for tool in memcheck racecheck; do
   echo "== $tool: tloam_b200_segment_scan + pageable staging (set_target of a 4.8 MB cloud)"
   timeout 600 compute-sanitizer --tool $tool --print-limit 5 python /tmp/seg_one.py 2>&1 | tail -4
-  echo "== $tool: tloam_b200_process_raw_scan -> submap_init_frame -> scan_match_predicted_async -> submap_update_frame_chained -> global_map_append_frame_chained, global_map_append (with and without intensity)"
+  echo "== $tool: tloam_b200_process_raw_scan -> submap_init_frame -> scan_match_predicted_async -> submap_update_frame_chained -> global_map_append_frame_chained, global_map_append (with and without intensity), the packed-scan calls"
   timeout 600 compute-sanitizer --tool $tool --print-limit 5 python /tmp/process_one.py 2>&1 | tail -4
 done
