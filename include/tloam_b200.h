@@ -470,6 +470,40 @@ int tloam_b200_process_raw_scan(tloam_b200_handle* h, const tloam_ground_config*
 int tloam_b200_process_raw_scan_packed(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg,
                                        int ring_min_num, double near_dis, const tloam_feature_config* fcfg, double ground_down_sample,
                                        double edge_down_sample, const tloam_packed_scan* scan, size_t n_source[4]);
+
+/* ---- Deskewing (motion correction of a raw scan; the reference reads scanPeriod and never uses it).  Opt-in: the timed
+ * forms below take per-point times; every other call behaves as before.  With t_end the largest finite time, P =
+ * frame_period (the unit of the times, e.g. 0.1 s at 10 Hz) and xi = log(last^-1 . curr) (se3 log of the pose history's
+ * constant-velocity increment -- the one tloam_b200_scan_match_predicted_async predicts with -- read on the device when the
+ * call runs, after the previous frame's solver), every row becomes
+ *     p'_i = exp(s_i . xi) . p_i,   s_i = (t_i - t_end) / P,
+ * the point in the sensor frame at the end of the sweep: the pose the loop returns is the pose at t_end.  A non-finite t_i,
+ * or a scan without a finite time, gives s_i = 0 (the row is copied bit for bit); non-finite rows stay non-finite.  A fresh
+ * handle's history is identity, so frames 0 and 1 are not corrected unless tloam_b200_set_pose_history seeded it.
+ *   - Segmentation reads the RAW scan (its ring / range-image topology is the sensor's).  The corrected scan replaces it
+ *     where the ground / edge / general clouds are gathered (so the source, the submap selections and the frame are
+ *     corrected) and as the raw scan tloam_b200_global_map_append_frame* and tloam_b200_registered_scan_download read.
+ *   - The kernels live in libtloam_b200_deskew.so, loaded from this library's directory on the first timed call; if it is
+ *     missing these calls return ERR_CUDA (tloam_b200_last_error names the file).
+ *   - INVALID_ARG, besides the untimed call's: time null with n > 0, frame_period not finite or not > 0, and for a packed
+ *     time field: offset < 0 or offset + size > point_step, a datatype other than 6 / 7 / 8, unit not finite or not > 0. */
+/* a time field of a tloam_packed_scan record: a record's time is the field's value times unit */
+typedef struct tloam_packed_time {
+  int offset;                         /* bytes into the record */
+  int datatype;                       /* sensor_msgs/PointField: 6 UINT32, 7 FLOAT32, 8 FLOAT64 (little-endian) */
+  double unit;                        /* e.g. 1 for seconds, 1e-9 for Ouster's nanoseconds */
+} tloam_packed_time;
+/* tloam_b200_process_raw_scan with time (HOST, n FP64 values, in the unit of frame_period) */
+int tloam_b200_process_raw_scan_timed(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg,
+                                      int ring_min_num, double near_dis, const tloam_feature_config* fcfg, double ground_down_sample,
+                                      double edge_down_sample, const double* xyz, const double* time, size_t n, double frame_period,
+                                      size_t n_source[4]);
+/* tloam_b200_process_raw_scan_packed with the time field `time` of the same records (read where they were uploaded) */
+int tloam_b200_process_raw_scan_packed_timed(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg,
+                                             int ring_min_num, double near_dis, const tloam_feature_config* fcfg,
+                                             double ground_down_sample, double edge_down_sample, const tloam_packed_scan* scan,
+                                             const tloam_packed_time* time, double frame_period, size_t n_source[4]);
+
 /* copies source cloud `cloud` (0 edge, 1 sphere, 2 planar, 3 ground; sensor frame, FP64 AoS) to the host (synchronises) */
 int tloam_b200_source_download(tloam_b200_handle* h, int cloud, double* out, size_t capacity_points);
 /* tloam_b200_submap_init from the last processed frame (front_end.cpp:285-305): edge = its raw edge cloud, ground =
@@ -514,7 +548,8 @@ int tloam_b200_global_map_append_chained(tloam_b200_handle* h, const double* xyz
  * After tloam_b200_process_raw_scan_packed whose layout has an intensity field, the frame is appended WITH that intensity,
  * read on the device (the reference's raw cloud carries its channel into global_map += ...); without one, or after the FP64
  * tloam_b200_process_raw_scan, it is a frame without intensity.  tloam_b200_global_map_append_frame_intensity[_chained]
- * with an explicit host array takes precedence over the packed intensity. */
+ * with an explicit host array takes precedence over the packed intensity.
+ * After a timed process_raw_scan (see Deskewing) the frame appended is the corrected scan; after an untimed one, the raw scan. */
 int tloam_b200_global_map_append_frame(tloam_b200_handle* h, const double pose[16]);
 int tloam_b200_global_map_append_frame_chained(tloam_b200_handle* h);
 /* exact points and frames in the map (synchronises); returns VOXEL_RANGE once after a refused frame */

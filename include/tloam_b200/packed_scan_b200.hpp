@@ -6,7 +6,8 @@
 //
 // Deliberately stricter than RosToOpen3d, which reads any field named "intensity" as a float whatever its datatype: x, y, z
 // and intensity must be FLOAT32 (datatype 7) with count 1.  Big-endian data and rows with padding (row_step != width *
-// point_step) are refused too.  A message without an intensity field is a scan without intensity.
+// point_step) are refused too.  A message without an intensity field is a scan without intensity.  packedTimeOf describes
+// the message's per-point time field for the timed (deskewing) call.
 #ifndef TLOAM_B200_PACKED_SCAN_B200_HPP
 #define TLOAM_B200_PACKED_SCAN_B200_HPP
 
@@ -41,6 +42,29 @@ int packedScanOf(const Msg& msg, tloam_packed_scan* out) {
   out->point_step = msg.point_step;
   out->x_offset = off[0]; out->y_offset = off[1]; out->z_offset = off[2]; out->intensity_offset = off[3];
   return TLOAM_B200_OK;
+}
+
+// fills *out with the per-point time field of msg, for tloam_b200_process_raw_scan_packed_timed: the first of "time"
+// (FLOAT32, seconds: velodyne_pointcloud), "t" (UINT32, nanoseconds: Ouster) and "timestamp" (FLOAT64, seconds: Hesai) the
+// message has, which must have that datatype with count 1.  Returns TLOAM_B200_OK, or TLOAM_B200_ERR_INVALID_ARG for a
+// big-endian message, a message without any of the three fields, or one of another type (tloam_b200.packed_time's rules).
+template <class Msg>
+int packedTimeOf(const Msg& msg, tloam_packed_time* out) {
+  if (!out || msg.is_bigendian) return TLOAM_B200_ERR_INVALID_ARG;
+  static const char* const kNames[3] = {"time", "t", "timestamp"};
+  static const int kTypes[3] = {7, 6, 8};                 // FLOAT32, UINT32, FLOAT64
+  static const double kUnits[3] = {1.0, 1e-9, 1.0};
+  for (int k = 0; k < 3; ++k) {
+    for (const auto& f : msg.fields) {
+      if (f.name != kNames[k]) continue;
+      if (f.datatype != kTypes[k] || f.count != 1 || f.offset > static_cast<unsigned>(INT_MAX)) return TLOAM_B200_ERR_INVALID_ARG;
+      out->offset = static_cast<int>(f.offset);
+      out->datatype = kTypes[k];
+      out->unit = kUnits[k];
+      return TLOAM_B200_OK;
+    }
+  }
+  return TLOAM_B200_ERR_INVALID_ARG;
 }
 
 }  // namespace tloam

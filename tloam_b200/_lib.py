@@ -49,6 +49,12 @@ class PackedScan(C.Structure):
                 ("z_offset", C.c_int), ("intensity_offset", C.c_int)]
 
 
+class PackedTime(C.Structure):
+    """tloam_packed_time (include/tloam_b200.h): the time field of a tloam_packed_scan record (PointField datatype 6 UINT32,
+    7 FLOAT32 or 8 FLOAT64, times unit).  Build one with tloam_b200.packed_time."""
+    _fields_ = [("offset", C.c_int), ("datatype", C.c_int), ("unit", C.c_double)]
+
+
 class InnerTrace(C.Structure):
     _fields_ = [
         ("x_candidate", C.c_double * 6), ("candidate_cost", C.c_double), ("model_cost_change", C.c_double),
@@ -143,6 +149,7 @@ EXPORTS = [
     "tloam_b200_global_map_has_intensity", "tloam_b200_global_map_intensity_download",
     "tloam_b200_segment_raw_scan_packed", "tloam_b200_process_raw_scan_packed", "tloam_b200_global_map_append_packed",
     "tloam_b200_global_map_append_packed_chained",
+    "tloam_b200_process_raw_scan_timed", "tloam_b200_process_raw_scan_packed_timed",
 ]
 
 _lib = None
@@ -292,5 +299,11 @@ def load():
                                                      C.POINTER(FeatureConfig), C.c_double, C.c_double, pk, szp]
     L.tloam_b200_global_map_append_packed.argtypes = [vp, dp, pk]
     L.tloam_b200_global_map_append_packed_chained.argtypes = [vp, pk]
+    L.tloam_b200_process_raw_scan_timed.argtypes = [vp, C.POINTER(GroundConfig), C.POINTER(DcvcConfig), C.c_int, C.c_double,
+                                                    C.POINTER(FeatureConfig), C.c_double, C.c_double, dp, dp, C.c_size_t, C.c_double,
+                                                    szp]
+    L.tloam_b200_process_raw_scan_packed_timed.argtypes = [vp, C.POINTER(GroundConfig), C.POINTER(DcvcConfig), C.c_int, C.c_double,
+                                                           C.POINTER(FeatureConfig), C.c_double, C.c_double, pk,
+                                                           C.POINTER(PackedTime), C.c_double, szp]
     _lib = L
     return L

@@ -28,6 +28,7 @@
 #include "host_stage.h"
 #include "gmap_intensity.h"
 #include "unpack_scan.h"
+#include "deskew.h"
 
 
 
@@ -2827,17 +2828,85 @@ static int unpack_packed(tloam_b200_handle* h, const tloam_packed_scan* s, doubl
   return TLOAM_B200_OK;
 }
 
-// the raw scan a chain call starts from: FP64 AoS rows (xyz), or a packed scan unpacked on the device
-struct RawScanIn { const double* xyz = nullptr; const tloam_packed_scan* packed = nullptr; size_t n = 0; };
+// ---- deskewing (the *_timed calls): the kernels live in libtloam_b200_deskew.so (deskew.cu), loaded on the first timed call
+//      so that the kernels of this library keep their SASS ----
+static std::mutex g_deskew_mu;
+struct DeskewLib { tloam_deskew_fn motion = nullptr, tend = nullptr, apply = nullptr; };
+static DeskewLib g_deskew;
+
+static int deskew_load(tloam_b200_handle* h, DeskewLib* out) {
+  std::lock_guard<std::mutex> lk(g_deskew_mu);
+  if (!g_deskew.apply) {
+    const std::string path = sibling_path("libtloam_b200_deskew.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    DeskewLib l;
+    if (so) {
+      l.motion = reinterpret_cast<tloam_deskew_fn>(dlsym(so, "tloam_deskew_motion"));
+      l.tend = reinterpret_cast<tloam_deskew_fn>(dlsym(so, "tloam_deskew_tend"));
+      l.apply = reinterpret_cast<tloam_deskew_fn>(dlsym(so, "tloam_deskew_apply"));
+    }
+    if (!l.motion || !l.tend || !l.apply) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "deskew: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_deskew = l;
+  }
+  *out = g_deskew;
+  return TLOAM_B200_OK;
+}
+
+static bool packed_time_valid(const tloam_packed_time* t, size_t point_step) {
+  const int bytes = t->datatype == 8 ? 8 : (t->datatype == 6 || t->datatype == 7) ? 4 : 0;
+  return bytes && t->offset >= 0 && (size_t)t->offset + bytes <= point_step && std::isfinite(t->unit) && t->unit > 0.0;
+}
+
+// the raw scan a chain call starts from: FP64 AoS rows (xyz), or a packed scan unpacked on the device.  timed: deskew it
+// (process_raw only) with the FP64 times `time` or, for a packed scan, its field `ptime`, over the frame period `period`.
+struct RawScanIn {
+  const double* xyz = nullptr; const tloam_packed_scan* packed = nullptr; size_t n = 0;
+  bool timed = false; const double* time = nullptr; const tloam_packed_time* ptime = nullptr; double period = 0.0;
+};
+
+// k_deskew_motion -> k_deskew_tend -> k_deskew on the handle's stream: scan (n x 3, on the device) corrected into out.  The
+// times are d_time (uploaded) or the packed records where unpack_packed uploaded them.  scratch: TLOAM_DESKEW_SCRATCH_DOUBLES.
+static int deskew_scan(tloam_b200_handle* h, const RawScanIn& in, const double* scan, const double* d_time, double* scratch,
+                       double* out) {
+  DeskewLib lib;
+  int rc = deskew_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  tloam_deskew_args a;
+  a.last_pose = reinterpret_cast<const double*>(reinterpret_cast<const char*>(h->d_state) + offsetof(FrameState, last_pose));
+  a.curr_pose = reinterpret_cast<const double*>(reinterpret_cast<const char*>(h->d_state) + offsetof(FrameState, curr_pose));
+  a.time = d_time; a.records = nullptr; a.point_step = 0; a.offset = 0; a.datatype = 0; a.unit = 1.0;
+  if (!d_time) {
+    a.records = h->d_packed; a.point_step = in.packed->point_step;
+    a.offset = in.ptime->offset; a.datatype = in.ptime->datatype; a.unit = in.ptime->unit;
+  }
+  a.n = in.n; a.period = in.period; a.xyz = scan; a.out = out; a.scratch = scratch; a.device = h->device; a.stream = h->stream;
+  const tloam_deskew_fn step[3] = {lib.motion, lib.tend, lib.apply};
+  static const char* const names[3] = {"k_deskew_motion", "k_deskew_tend", "k_deskew"};
+  for (int k = 0; k < 3; ++k) {
+    int e = 0;
+    TL_LAUNCH(TLOAM_B200_K_FEATURE, (e = step[k](&a)));
+    if (e != cudaSuccess) {
+      snprintf(h->last_error, sizeof(h->last_error), "deskew: %s: %s", names[k], cudaGetErrorString((cudaError_t)e));
+      return TLOAM_B200_ERR_CUDA;
+    }
+  }
+  return TLOAM_B200_OK;
+}
 
 // The one implementation of the chained segmentation; only the way the scan reaches the device depends on its form (in).
 // remove: run RemoveClosedNonFinitePoints(near_dis) on the device first (tloam_b200_segment_raw_scan); tloam_b200_segment_scan
 // runs without that step.  beam / intensity (optional, n values): the channel of every point of the scan as int / FP64 (NaN
 // for removed points).  keep (optional): the three final lists stay on the device (tloam_b200_process_raw_scan) -- the index
-// arrays are not written, *keep receives the uploaded scan, the intensity of a packed scan with that field (else null) and
-// the lists (valid until the handle's next segmentation call); the counts still land in *n_ground / *n_edge / *n_general.
+// arrays are not written, *keep receives the uploaded scan, the intensity of a packed scan with that field (else null), the
+// deskewed scan of a timed call (else null) and the lists (valid until the handle's next segmentation call); the counts
+// still land in *n_ground / *n_edge / *n_general.  The segmentation itself always reads the uploaded (raw) scan.
 struct ChainKeep {
-  const double* scan = nullptr; const double* intensity = nullptr;
+  const double* scan = nullptr; const double* intensity = nullptr; const double* deskewed = nullptr;
   const unsigned long long *ground = nullptr, *edge = nullptr, *general = nullptr;
 };
 static int segment_chain(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg, int ring_min_num, bool remove,
@@ -2864,6 +2933,9 @@ static int segment_chain(tloam_b200_handle* h, const tloam_ground_config* gcfg, 
                o_rmc = remove ? take(nchunk * 4 + 64) : 0, o_int = intensity ? take(n * 8) : 0, o_fi = intensity ? take(n * 8) : 0;
   const bool keep_int = keep && in.packed && in.packed->intensity_offset >= 0;
   const size_t o_pint = keep_int ? take(n * 8) : 0;
+  const bool timed = keep && in.timed;
+  const size_t o_dsk = timed ? take(n * 24) : 0, o_time = timed && !in.packed ? take(n * 8) : 0,
+               o_dscr = timed ? take(TLOAM_DESKEW_SCRATCH_DOUBLES * 8) : 0;
   if (off > h->cap_chain) {
     CU_TRY(cudaStreamSynchronize(h->stream));
     cudaFree(h->d_chain); h->d_chain = nullptr; h->cap_chain = 0;
@@ -2880,6 +2952,12 @@ static int segment_chain(tloam_b200_handle* h, const tloam_ground_config* gcfg, 
   double* d_pint = keep_int ? (double*)(c + o_pint) : nullptr;
   int rc = in.packed ? unpack_packed(h, in.packed, d_scan, d_pint) : upload_host(h, d_scan, in.xyz, n * 24);
   if (rc != TLOAM_B200_OK) return rc;
+  double* d_dsk = timed ? (double*)(c + o_dsk) : nullptr;
+  if (timed) {
+    double* d_time = in.packed ? nullptr : (double*)(c + o_time);
+    if (d_time && (rc = upload_host(h, d_time, in.time, n * 8)) != TLOAM_B200_OK) return rc;
+    if ((rc = deskew_scan(h, in, d_scan, d_time, (double*)(c + o_dscr), d_dsk)) != TLOAM_B200_OK) return rc;
+  }
   struct Reset { tloam_b200_handle* h; ~Reset() { h->seg = tloam_b200_handle::SegChain(); } } reset{h};
   // ---- 0. RemoveClosedNonFinitePoints (:48, :472-499): kept points + kept -> raw map ----
   const double* pts = d_scan;
@@ -2946,7 +3024,10 @@ static int segment_chain(tloam_b200_handle* h, const tloam_ground_config* gcfg, 
     if (ne && !keep) CU_TRY(cudaMemcpyAsync(edge_index, d_fe, ne * 8, cudaMemcpyDeviceToHost, h->stream));
     if (nn && !keep) CU_TRY(cudaMemcpyAsync(general_index, d_fn, nn * 8, cudaMemcpyDeviceToHost, h->stream));
   }
-  if (keep) { keep->scan = d_scan; keep->intensity = d_pint; keep->ground = d_fg; keep->edge = d_fe; keep->general = d_fn; }
+  if (keep) {
+    keep->scan = d_scan; keep->intensity = d_pint; keep->deskewed = d_dsk;
+    keep->ground = d_fg; keep->edge = d_fe; keep->general = d_fn;
+  }
   if (beam) CU_TRY(cudaMemcpyAsync(beam, c + o_beam, n * 4, cudaMemcpyDeviceToHost, h->stream));
   if (intensity) CU_TRY(cudaMemcpyAsync(intensity, c + o_fi, n * 8, cudaMemcpyDeviceToHost, h->stream));
   CU_TRY(cudaStreamSynchronize(h->stream));
@@ -3088,6 +3169,11 @@ static int process_raw(tloam_b200_handle* h, const tloam_ground_config* gcfg, co
   if (!h || !gcfg || !dcfg || !fcfg || !n_source || (!in.packed && !in.xyz && in.n)) return TLOAM_B200_ERR_INVALID_ARG;
   for (int k = 0; k < 4; ++k) n_source[k] = 0;
   if (!(ground_down_sample > 0.0) || !(edge_down_sample > 0.0)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (in.timed) {
+    if (!std::isfinite(in.period) || !(in.period > 0.0)) return TLOAM_B200_ERR_INVALID_ARG;
+    if (in.packed ? (in.ptime ? !packed_time_valid(in.ptime, in.packed->point_step) : in.n > 0) : (!in.time && in.n))
+      return TLOAM_B200_ERR_INVALID_ARG;
+  }
   CU_TRY(cudaSetDevice(h->device));
   h->have_frame = false;
   size_t unused[1];                                       // the index lists stay on the device (ChainKeep)
@@ -3101,14 +3187,15 @@ static int process_raw(tloam_b200_handle* h, const tloam_ground_config* gcfg, co
   const unsigned long long* lists[3] = {keep.ground, keep.edge, keep.general};
   const size_t cnt[3] = {ng, ne, nn};
   size_t off = 0;
+  const double* rows = keep.deskewed ? keep.deskewed : keep.scan;   // the corrected scan of a timed call
   for (int c = 0; c < 3; ++c) {                           // ground / edge / general clouds gathered from the uploaded raw scan
     if (cnt[c]) TL_LAUNCH(TLOAM_B200_K_FEATURE, (k_select_by_index<unsigned long long><<<(unsigned)((cnt[c] + 255) / 256), 256, 0, h->stream>>>(
-                                                    keep.scan, lists[c], (unsigned)cnt[c], h->d_frame + 3 * off)));
+                                                    rows, lists[c], (unsigned)cnt[c], h->d_frame + 3 * off)));
     off += cnt[c];
   }
   CU_TRY(cudaGetLastError());
   if ((rc = process_frame(h, fcfg, ground_down_sample, edge_down_sample, ng, ne, nn, n_source)) != TLOAM_B200_OK) return rc;
-  h->raw_scan = keep.scan; h->raw_int = keep.intensity; h->raw_n = in.n; h->raw_gen = h->seg_gen;   // for global_map_append_frame*
+  h->raw_scan = rows; h->raw_int = keep.intensity; h->raw_n = in.n; h->raw_gen = h->seg_gen;   // for global_map_append_frame*
   return TLOAM_B200_OK;
 }
 
@@ -3126,6 +3213,25 @@ int tloam_b200_process_raw_scan_packed(tloam_b200_handle* h, const tloam_ground_
   if (!scan) return TLOAM_B200_ERR_INVALID_ARG;
   RawScanIn in;
   in.packed = scan; in.n = scan->n;
+  return process_raw(h, gcfg, dcfg, ring_min_num, near_dis, fcfg, ground_down_sample, edge_down_sample, in, n_source);
+}
+
+int tloam_b200_process_raw_scan_timed(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg,
+                                      int ring_min_num, double near_dis, const tloam_feature_config* fcfg, double ground_down_sample,
+                                      double edge_down_sample, const double* xyz, const double* time, size_t n, double frame_period,
+                                      size_t n_source[4]) {
+  RawScanIn in;
+  in.xyz = xyz; in.n = n; in.timed = true; in.time = time; in.period = frame_period;
+  return process_raw(h, gcfg, dcfg, ring_min_num, near_dis, fcfg, ground_down_sample, edge_down_sample, in, n_source);
+}
+
+int tloam_b200_process_raw_scan_packed_timed(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg,
+                                             int ring_min_num, double near_dis, const tloam_feature_config* fcfg,
+                                             double ground_down_sample, double edge_down_sample, const tloam_packed_scan* scan,
+                                             const tloam_packed_time* time, double frame_period, size_t n_source[4]) {
+  if (!scan) return TLOAM_B200_ERR_INVALID_ARG;
+  RawScanIn in;
+  in.packed = scan; in.n = scan->n; in.timed = true; in.ptime = time; in.period = frame_period;
   return process_raw(h, gcfg, dcfg, ring_min_num, near_dis, fcfg, ground_down_sample, edge_down_sample, in, n_source);
 }
 

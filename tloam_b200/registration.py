@@ -84,6 +84,29 @@ def _packed(scan):
     return scan if isinstance(scan, _lib.PackedScan) else packed_scan(scan)
 
 
+# the per-point time fields drivers publish: name -> (PointField datatype, numpy dtype, unit to seconds)
+_TIME_FIELDS = (("time", 7, np.dtype("<f4"), 1.0),          # velodyne_pointcloud XYZIRT: float32 s from the sweep's start
+                ("t", 6, np.dtype("<u4"), 1e-9),            # Ouster: uint32 ns
+                ("timestamp", 8, np.dtype("<f8"), 1.0))     # Hesai: float64 s
+
+
+def packed_time(arr):
+    """The tloam_packed_time descriptor of the per-point time field of a structured array (the records packed_scan
+    describes), for the timed packed calls: the first of `time` (little-endian float32, s), `t` (little-endian uint32, ns)
+    and `timestamp` (little-endian float64, s) the records have, which must have that type.  Anything else raises
+    ValueError."""
+    fields = getattr(getattr(arr, "dtype", None), "fields", None)
+    if not isinstance(arr, np.ndarray) or fields is None:
+        raise ValueError("packed_time: a numpy structured array is required")
+    for name, datatype, dt, unit in _TIME_FIELDS:
+        if name in fields:
+            fdt, off = fields[name][:2]
+            if fdt != dt:
+                raise ValueError(f"packed_time: field {name!r} is {fdt.str}, not {dt.str}")
+            return _lib.PackedTime(off, datatype, unit)
+    raise ValueError("packed_time: the records have no field 'time', 't' or 'timestamp'")
+
+
 class Frame:
     """Mirror of tloam::Frame (ref: registration_interface.hpp:19-38): the four feature clouds, (n,3) float64.
     scan_cloud is accepted and ignored, as in the reference (registration.cpp:232-239)."""
@@ -537,21 +560,34 @@ class LocalRegistration:
         return list(self.n_source)
 
     def process_raw_scan(self, scan, near_dis=3.0, ring_min_num=131, ground=None, dcvc=None, feature=None, ground_down_sample=0.3,
-                         edge_down_sample=0.1):
+                         edge_down_sample=0.1, time=None, frame_period=0.1):
         """segment_raw_scan -> process_cloud on the device with one upload of the raw scan and no index list going home.
-        ground / dcvc / feature: dicts of configuration overrides.  Returns the four source sizes."""
+        ground / dcvc / feature: dicts of configuration overrides.  Returns the four source sizes.
+        time: one value per row (in the unit of frame_period) to deskew the scan with the pose history's constant-velocity
+        increment (include/tloam_b200.h, Deskewing); None: the scan is taken as it is."""
         a = _f64(scan).reshape(-1, 3)
-        return self._process_raw("process_raw_scan", (_dp(a), a.shape[0]), a.shape[0], near_dis, ring_min_num, ground, dcvc, feature,
-                                 ground_down_sample, edge_down_sample)
+        if time is None:
+            return self._process_raw("process_raw_scan", (_dp(a), a.shape[0]), a.shape[0], near_dis, ring_min_num, ground, dcvc,
+                                     feature, ground_down_sample, edge_down_sample)
+        t = _f64(time).reshape(-1)
+        if t.shape[0] != a.shape[0]:
+            raise ValueError(f"process_raw_scan: {t.shape[0]} times for {a.shape[0]} rows")
+        return self._process_raw("process_raw_scan_timed", (_dp(a), _dp(t), a.shape[0], float(frame_period)), a.shape[0], near_dis,
+                                 ring_min_num, ground, dcvc, feature, ground_down_sample, edge_down_sample)
 
     def process_raw_scan_packed(self, scan, near_dis=3.0, ring_min_num=131, ground=None, dcvc=None, feature=None, ground_down_sample=0.3,
-                                edge_down_sample=0.1):
+                                edge_down_sample=0.1, deskew=False, frame_period=0.1):
         """process_raw_scan of a raw scan in the sensor's float32 layout (a packed_scan descriptor, or an array packed_scan
         accepts): one upload, unpacked on the device.  With an intensity field, global_map_append_frame() appends the frame
-        with that intensity, read on the device."""
+        with that intensity, read on the device.  deskew: correct the scan with the records' time field (packed_time) over
+        frame_period seconds, read where the records were uploaded."""
         d = _packed(scan)
-        return self._process_raw("process_raw_scan_packed", (C.byref(d),), d.n, near_dis, ring_min_num, ground, dcvc, feature,
-                                 ground_down_sample, edge_down_sample)
+        if not deskew:
+            return self._process_raw("process_raw_scan_packed", (C.byref(d),), d.n, near_dis, ring_min_num, ground, dcvc, feature,
+                                     ground_down_sample, edge_down_sample)
+        t = packed_time(getattr(d, "_keep", None))
+        return self._process_raw("process_raw_scan_packed_timed", (C.byref(d), C.byref(t), float(frame_period)), d.n, near_dis,
+                                 ring_min_num, ground, dcvc, feature, ground_down_sample, edge_down_sample)
 
     def _process_raw(self, fn, scan_args, n, near_dis, ring_min_num, ground, dcvc, feature, ground_down_sample, edge_down_sample):
         gc, dc = self._segmentation_configs(ground, dcvc)
