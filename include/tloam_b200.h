@@ -593,6 +593,67 @@ int tloam_b200_global_map_intensity_download(tloam_b200_handle* h, size_t first,
 int tloam_b200_global_map_append_packed(tloam_b200_handle* h, const double pose[16], const tloam_packed_scan* scan);
 int tloam_b200_global_map_append_packed_chained(tloam_b200_handle* h, const tloam_packed_scan* scan);
 
+/* ---- Loop closure (place recognition; the reference is pure odometry).  Every added frame gets a Scan Context descriptor
+ * (Kim & Kim, IROS 2018) kept in a database on the device, and is compared with EVERY earlier frame at EVERY column shift.
+ *   - Descriptor.  Every finite row (x, y, z) of the scan, sensor frame: r = sqrt(x*x + y*y) (separately rounded, no FMA);
+ *     a row with r > max_radius is left out.  ring = clamp(ceil(r / max_radius * n_ring), 1, n_ring) - 1.  sector = the
+ *     number of sector boundaries k = 1 .. n_sector - 1 the row lies strictly counter-clockwise of, where boundary k is the
+ *     direction (cos, sin)(2 pi k / n_sector) computed by the C library's cos / sin on the host, a row of the upper
+ *     half-plane (y > 0, or y == 0 and x >= 0) is compared with the boundaries k < n_sector / 2 and lies below the others,
+ *     a row of the lower half-plane lies above those and is compared with the rest, and "counter-clockwise of (c, s)" is
+ *     c*y - s*x > 0 (separately rounded): Scan Context's ceil-and-clamp sector of the azimuth in [0, 360), without atan2.
+ *     Bin (ring, sector) = max of z + lidar_height over its rows; an empty bin is 0, a negative maximum stays.
+ *   - Next to the n_ring x n_sector bins (row-major): the ring key (each ring's sum in sector order / n_sector) and the
+ *     column norms (sqrt of the sum of squares in ring order).  Sums start from +0.0.
+ *   - Distance of query A and candidate B at shift s: B_s[:, c] = B[:, (c - s) mod n_sector] (np.roll(B, s, axis=1)).  A
+ *     column c counts when the norms of A[:, c] and B_s[:, c] are both non-zero; cos_c = (a . b, summed in ring order) /
+ *     (|a| * |b|); distance = 1 - (sum of cos_c in ascending c) / count, or 1.0 when no column counts (Scan Context divides
+ *     by zero there).  Every value is rounded as written, so the device's distances are bit-reproducible on the host.
+ *   - Search.  Frame i (the i-th add since enable / reset, from 0) is compared with every frame j <= i - exclude_recent at
+ *     every shift; the result is the minimum by (distance, j, s), lexicographic.  is_loop = distance < dist_threshold.
+ *     yaw = -s * 2 pi / n_sector wrapped to (-pi, pi] (computed as k * (2 pi / n_sector), k = -s, or n_sector - s when
+ *     2 s >= n_sector): p_candidate ~ Rz(yaw) . p_query, a coarse alignment.  No eligible frame: candidate -1, shift 0,
+ *     yaw 0, distance +inf, is_loop 0.
+ *   - Adds are enqueued on the handle's stream with no host round trip (the host synchronises only to grow the database,
+ *     x1.5); tloam_b200_loop_result waits for the newest add only.  Nothing here touches the odometry's buffers.
+ *   - The kernels live in libtloam_b200_loop.so, loaded from this library's directory on the first loop call; if it is
+ *     missing these calls return ERR_CUDA (tloam_b200_last_error names the file).  Off until tloam_b200_loop_enable:
+ *     every other loop call returns NOT_READY, and nothing is allocated or launched. */
+typedef struct tloam_loop_config {
+  double lidar_height;                 /* added to z (Scan Context's LIDAR_HEIGHT) */
+  int n_ring, n_sector;                /* n_ring * n_sector <= 4096 */
+  double max_radius;                   /* m */
+  int exclude_recent;                  /* the newest frames a query skips: frame i sees j <= i - exclude_recent */
+  double dist_threshold;               /* is_loop below this distance */
+  size_t initial_capacity_frames;      /* database slots before the first growth */
+} tloam_loop_config;
+typedef struct tloam_loop_result {
+  long long query, candidate;          /* frame indices since enable / reset; candidate -1: no eligible frame */
+  int shift, is_loop;
+  double yaw, distance;                /* rad; see above */
+} tloam_loop_result;
+/* lidar_height 2.0, n_ring 20, n_sector 60, max_radius 80 m, exclude_recent 50, dist_threshold 0.13 (Scan Context's),
+ * initial_capacity_frames 1024 */
+void tloam_b200_loop_default_config(tloam_loop_config* c);
+/* (re)starts an empty database with this configuration.  INVALID_ARG: cfg null, n_ring or n_sector < 1, n_ring * n_sector
+ * > 4096, max_radius <= 0 or not finite, exclude_recent < 0, lidar_height or dist_threshold not finite. */
+int tloam_b200_loop_enable(tloam_b200_handle* h, const tloam_loop_config* cfg);
+/* empties the database (the configuration and the buffers stay).  NOT_READY if not enabled. */
+int tloam_b200_loop_reset(tloam_b200_handle* h);
+/* adds the raw scan the last tloam_b200_process_raw_scan* uploaded (the corrected scan after a timed call) and enqueues
+ * its query.  NOT_READY under tloam_b200_global_map_append_frame's rule (no such scan, or a segmentation / process call
+ * since). */
+int tloam_b200_loop_add_frame(tloam_b200_handle* h);
+/* the same for a HOST cloud (n x 3 FP64 AoS, NaN / Inf rows allowed), uploaded */
+int tloam_b200_loop_add(tloam_b200_handle* h, const double* xyz, size_t n);
+/* the newest add's result (waits for that add).  NOT_READY before the first add since enable / reset. */
+int tloam_b200_loop_result(tloam_b200_handle* h, tloam_loop_result* out);
+/* frames in the database */
+int tloam_b200_loop_size(tloam_b200_handle* h, size_t* n_frames);
+/* frame's descriptor to out: n_ring * n_sector bins (row-major), n_ring ring key values, n_sector column norms
+ * (synchronises).  INVALID_ARG past the last frame. */
+int tloam_b200_loop_descriptor_download(tloam_b200_handle* h, size_t frame, double* out);
+
 /* Pinned host memory helpers (optional; pinned inputs make set_* a direct DMA, no staging threads). */
 int tloam_b200_host_alloc(void** p, size_t bytes);
 int tloam_b200_host_free(void* p);

@@ -14,7 +14,8 @@
 // it back); frame 0 has no append, as in the reference.  A raw scan with intensity_ gives the map its intensity channel
 // (per-voxel averages, the reference's XYZI map); globalMap(points, intensity) reads it back.  updateGlobalMap also takes
 // the driver's sensor_msgs/PointCloud2 as it arrived (packed_scan_b200.hpp): one upload, unpacked on the device, its
-// intensity field (if any) carried into the map.
+// intensity field (if any) carried into the map.  enableLoopDetection / addLoopFrame / loopResult add loop closure: a Scan
+// Context descriptor per frame and an exact search over every earlier frame, on the GPU.
 // Without the reference headers (this repository's tests) define TLOAM_B200_MOCK_HOST_TYPES and provide the host types
 // (tests/mock/mock_tloam.hpp).
 #ifndef TLOAM_B200_FRONT_END_B200_HPP
@@ -144,6 +145,27 @@ class FrontEndB200 {
     return report(tloam_b200_registered_scan_download(h_, reinterpret_cast<double*>(out.data()), out.size(), &n), "registeredScan");
   }
 
+  // loop closure (include/tloam_b200.h "Loop closure"; the reference is pure odometry): every added frame gets a Scan
+  // Context descriptor on the GPU and is compared with every frame at least cfg.exclude_recent frames older.  The library
+  // reports the best candidate; verifying it and correcting the poses belong to the caller's back end.
+  bool enableLoopDetection(const tloam_loop_config& cfg) {
+    loop_ = report(tloam_b200_loop_enable(h_, &cfg), "enableLoopDetection");
+    return loop_;
+  }
+  bool enableLoopDetection() {
+    tloam_loop_config c;
+    tloam_b200_loop_default_config(&c);
+    return enableLoopDetection(c);
+  }
+  bool loopDetection() const { return loop_; }
+  // adds the raw scan the last tloam_b200_process_raw_scan* on this handle uploaded (deskewed when timed), read on the GPU,
+  // and enqueues its query; no synchronisation
+  bool addLoopFrame() { return report(tloam_b200_loop_add_frame(h_), "addLoopFrame"); }
+  // the same for a host raw scan (the driver's cloud, NaN rows allowed), uploaded
+  bool addLoopFrame(const CloudData& raw) { return report(tloam_b200_loop_add(h_, data(raw), size(raw)), "addLoopFrame"); }
+  // the newest added frame's best earlier frame (waits for that add only); out.is_loop below cfg.dist_threshold
+  bool loopResult(tloam_loop_result& out) { return report(tloam_b200_loop_result(h_, &out), "loopResult"); }
+
   // processCloud + setInputSource (ref: front_end.cpp:181-199, :313): the three clouds the segmentation nodelet publishes
   bool processCloud(CloudData& ground, CloudData& edge, CloudData& general) {
     return report(tloam_b200_process_cloud(h_, &fcfg_, ground_down_sample_, edge_down_sample_, data(ground), size(ground), data(edge),
@@ -189,6 +211,7 @@ class FrontEndB200 {
   double ground_down_sample_ = 0.3, edge_down_sample_ = 0.1;
   size_t n_source_[4] = {0, 0, 0, 0};
   bool mapping_ = false;
+  bool loop_ = false;
   int last_status_ = TLOAM_B200_OK;
 };
 

@@ -55,6 +55,18 @@ class PackedTime(C.Structure):
     _fields_ = [("offset", C.c_int), ("datatype", C.c_int), ("unit", C.c_double)]
 
 
+class LoopConfig(C.Structure):
+    """tloam_loop_config (include/tloam_b200.h "Loop closure"): Scan Context's parameters and the database's first capacity."""
+    _fields_ = [("lidar_height", C.c_double), ("n_ring", C.c_int), ("n_sector", C.c_int), ("max_radius", C.c_double),
+                ("exclude_recent", C.c_int), ("dist_threshold", C.c_double), ("initial_capacity_frames", C.c_size_t)]
+
+
+class LoopResult(C.Structure):
+    """tloam_loop_result: the newest add's best earlier frame (candidate -1: none eligible)."""
+    _fields_ = [("query", C.c_longlong), ("candidate", C.c_longlong), ("shift", C.c_int), ("is_loop", C.c_int),
+                ("yaw", C.c_double), ("distance", C.c_double)]
+
+
 class InnerTrace(C.Structure):
     _fields_ = [
         ("x_candidate", C.c_double * 6), ("candidate_cost", C.c_double), ("model_cost_change", C.c_double),
@@ -150,6 +162,8 @@ EXPORTS = [
     "tloam_b200_segment_raw_scan_packed", "tloam_b200_process_raw_scan_packed", "tloam_b200_global_map_append_packed",
     "tloam_b200_global_map_append_packed_chained",
     "tloam_b200_process_raw_scan_timed", "tloam_b200_process_raw_scan_packed_timed",
+    "tloam_b200_loop_default_config", "tloam_b200_loop_enable", "tloam_b200_loop_reset", "tloam_b200_loop_add_frame",
+    "tloam_b200_loop_add", "tloam_b200_loop_result", "tloam_b200_loop_size", "tloam_b200_loop_descriptor_download",
 ]
 
 _lib = None
@@ -305,5 +319,14 @@ def load():
     L.tloam_b200_process_raw_scan_packed_timed.argtypes = [vp, C.POINTER(GroundConfig), C.POINTER(DcvcConfig), C.c_int, C.c_double,
                                                            C.POINTER(FeatureConfig), C.c_double, C.c_double, pk,
                                                            C.POINTER(PackedTime), C.c_double, szp]
+    L.tloam_b200_loop_default_config.argtypes = [C.POINTER(LoopConfig)]
+    L.tloam_b200_loop_default_config.restype = None
+    L.tloam_b200_loop_enable.argtypes = [vp, C.POINTER(LoopConfig)]
+    L.tloam_b200_loop_reset.argtypes = [vp]
+    L.tloam_b200_loop_add_frame.argtypes = [vp]
+    L.tloam_b200_loop_add.argtypes = [vp, dp, C.c_size_t]
+    L.tloam_b200_loop_result.argtypes = [vp, C.POINTER(LoopResult)]
+    L.tloam_b200_loop_size.argtypes = [vp, szp]
+    L.tloam_b200_loop_descriptor_download.argtypes = [vp, C.c_size_t, dp]
     _lib = L
     return L

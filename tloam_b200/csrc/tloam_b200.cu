@@ -29,6 +29,7 @@
 #include "gmap_intensity.h"
 #include "unpack_scan.h"
 #include "deskew.h"
+#include "scan_context.h"
 
 
 
@@ -213,6 +214,17 @@ struct tloam_b200_handle {
   double* d_gmi_map = nullptr;
   double* d_gmi_in = nullptr;              size_t cap_gmi_in = 0;                               // uploaded intensities
   void* d_gmi_scratch = nullptr;           size_t cap_gmi_scratch = 0;
+  // ---- loop closure (tloam_b200_loop_*, libtloam_b200_loop.so): nothing is allocated or launched until it is enabled.
+  //      loop_frames is exact (every add is one frame); the database grows x1.5 when full ----
+  bool loop_on = false;
+  tloam_loop_config loop_cfg;
+  double* d_loop_db = nullptr;             size_t loop_cap = 0, loop_frames = 0, loop_growths = 0;   // descriptor slots
+  double* d_loop_dirs = nullptr;           // sector boundary directions
+  double* d_loop_in = nullptr;             size_t cap_loop_in = 0;                                   // host clouds (loop_add)
+  tloam_sc_best* d_loop_best = nullptr;    // TLOAM_SC_MAX_BLOCKS block minima, then the result
+  tloam_sc_best* h_loop_best = nullptr;    // pinned: the newest add's result, landed when ev_loop has
+  cudaEvent_t ev_loop = nullptr;
+  bool loop_has_result = false;            long long loop_query = -1;
 };
 
 // launch bookkeeping: counts the kernel and, in profiling mode, brackets it with events
@@ -409,6 +421,9 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   cudaFree(h->d_gmap_fin);
   cudaFree(h->d_gmi_st); cudaFree(h->d_gmi_map); cudaFree(h->d_gmi_in); cudaFree(h->d_gmi_scratch); cudaFree(h->d_packed);
   for (auto& pr : h->gmap_probes) { if (pr.ev) cudaEventDestroy(pr.ev); if (pr.h_count) cudaFreeHost(pr.h_count); }
+  cudaFree(h->d_loop_db); cudaFree(h->d_loop_dirs); cudaFree(h->d_loop_in); cudaFree(h->d_loop_best);
+  if (h->h_loop_best) cudaFreeHost(h->h_loop_best);
+  if (h->ev_loop) cudaEventDestroy(h->ev_loop);
   for (int i = 0; i < 2; ++i) if (h->ev_stage_free[i]) cudaEventDestroy(h->ev_stage_free[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_fit[i]) cudaEventDestroy(h->ev_fit[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_res[i]) cudaEventDestroy(h->ev_res[i]);
@@ -3720,6 +3735,187 @@ int tloam_b200_global_map_intensity_download(tloam_b200_handle* h, size_t first,
   if (count) CU_TRY(cudaMemcpyAsync(out, h->d_gmi_map + first, count * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   CU_TRY(cudaStreamSynchronize(h->stream));
   return flag;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Loop closure (Scan Context descriptors and an exact search; kernels in scan_context.cu, loaded from libtloam_b200_loop.so
+// on the first loop call so that the kernels of this library keep their SASS).  Every add is enqueued on the handle's
+// stream; the host keeps the frame count and synchronises only to grow the database.
+// ---------------------------------------------------------------------------------------------
+struct LoopLib { tloam_sc_fn bin = nullptr, finish = nullptr, search = nullptr; };
+static std::mutex g_loop_mu;
+static LoopLib g_loop;
+
+static int loop_load(tloam_b200_handle* h, LoopLib* out) {
+  std::lock_guard<std::mutex> lk(g_loop_mu);
+  if (!g_loop.search) {
+    const std::string path = sibling_path("libtloam_b200_loop.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    LoopLib l;
+    if (so) {
+      l.bin = reinterpret_cast<tloam_sc_fn>(dlsym(so, "tloam_sc_bin"));
+      l.finish = reinterpret_cast<tloam_sc_fn>(dlsym(so, "tloam_sc_finish"));
+      l.search = reinterpret_cast<tloam_sc_fn>(dlsym(so, "tloam_sc_search"));
+    }
+    if (!l.bin || !l.finish || !l.search) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "loop closure: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_loop = l;
+  }
+  *out = g_loop;
+  return TLOAM_B200_OK;
+}
+
+void tloam_b200_loop_default_config(tloam_loop_config* c) {   // Scan Context's published parameters
+  c->lidar_height = 2.0; c->n_ring = 20; c->n_sector = 60; c->max_radius = 80.0;
+  c->exclude_recent = 50; c->dist_threshold = 0.13;
+  c->initial_capacity_frames = 1024;
+}
+
+int tloam_b200_loop_enable(tloam_b200_handle* h, const tloam_loop_config* cfg) {
+  if (!h || !cfg || cfg->n_ring < 1 || cfg->n_sector < 1 || (long long)cfg->n_ring * cfg->n_sector > 4096 ||
+      !std::isfinite(cfg->max_radius) || !(cfg->max_radius > 0.0) || cfg->exclude_recent < 0 || !std::isfinite(cfg->lidar_height) ||
+      !std::isfinite(cfg->dist_threshold))
+    return TLOAM_B200_ERR_INVALID_ARG;
+  LoopLib lib;
+  int rc = loop_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (!h->d_loop_best) {
+    CU_TRY(cudaMalloc(&h->d_loop_best, (TLOAM_SC_MAX_BLOCKS + 1) * sizeof(tloam_sc_best)));
+    CU_TRY(cudaMallocHost(&h->h_loop_best, sizeof(tloam_sc_best)));
+    CU_TRY(cudaEventCreateWithFlags(&h->ev_loop, cudaEventDisableTiming));
+  }
+  cudaFree(h->d_loop_db); h->d_loop_db = nullptr; h->loop_cap = 0;
+  cudaFree(h->d_loop_dirs); h->d_loop_dirs = nullptr;
+  const size_t cap = cfg->initial_capacity_frames ? cfg->initial_capacity_frames : 1;
+  CU_TRY(cudaMalloc(&h->d_loop_db, cap * TLOAM_SC_SLOT_DOUBLES(cfg->n_ring, cfg->n_sector) * sizeof(double)));
+  h->loop_cap = cap;
+  // the sector boundaries: (cos, sin) of 2 pi k / n_sector, k = 1 .. n_sector - 1, by the C library (the oracle calls the same)
+  std::vector<double> dirs(2 * (size_t)cfg->n_sector);
+  for (int k = 1; k < cfg->n_sector; ++k) {
+    const double t = 2.0 * M_PI * k / cfg->n_sector;
+    dirs[2 * (k - 1)] = std::cos(t);
+    dirs[2 * (k - 1) + 1] = std::sin(t);
+  }
+  CU_TRY(cudaMalloc(&h->d_loop_dirs, dirs.size() * sizeof(double)));
+  CU_TRY(cudaMemcpy(h->d_loop_dirs, dirs.data(), dirs.size() * sizeof(double), cudaMemcpyHostToDevice));
+  h->loop_cfg = *cfg;
+  h->loop_frames = 0; h->loop_growths = 0; h->loop_has_result = false; h->loop_query = -1;
+  h->loop_on = true;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_loop_reset(tloam_b200_handle* h) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loop_on) return TLOAM_B200_ERR_NOT_READY;
+  h->loop_frames = 0; h->loop_has_result = false; h->loop_query = -1;
+  return TLOAM_B200_OK;
+}
+
+// the one place an add synchronises: the database is full.  It grows to 1.5 x its capacity; the slots keep their bits.
+static int loop_grow(tloam_b200_handle* h) {
+  const size_t slot = TLOAM_SC_SLOT_DOUBLES(h->loop_cfg.n_ring, h->loop_cfg.n_sector);
+  size_t ncap = h->loop_cap + h->loop_cap / 2;
+  if (ncap < h->loop_cap + 1) ncap = h->loop_cap + 1;
+  double* q = nullptr;
+  CU_TRY(cudaMalloc(&q, ncap * slot * sizeof(double)));
+  if (h->loop_frames)
+    CU_TRY(cudaMemcpyAsync(q, h->d_loop_db, h->loop_frames * slot * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  cudaFree(h->d_loop_db);
+  h->d_loop_db = q; h->loop_cap = ncap;
+  h->loop_growths++;
+  return TLOAM_B200_OK;
+}
+
+// the descriptor of the n rows at d_xyz (device) into the next slot, then its query over every slot <= frame - exclude_recent;
+// the result lands in the pinned slot, ev_loop marks it
+static int loop_add_impl(tloam_b200_handle* h, const double* d_xyz, size_t n) {
+  LoopLib lib;
+  int rc = loop_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  if (h->loop_frames == h->loop_cap && (rc = loop_grow(h)) != TLOAM_B200_OK) return rc;
+  const tloam_loop_config& c = h->loop_cfg;
+  tloam_sc_args a;
+  a.n_ring = c.n_ring; a.n_sector = c.n_sector; a.lidar_height = c.lidar_height; a.max_radius = c.max_radius;
+  a.dirs = h->d_loop_dirs; a.xyz = d_xyz; a.n = n; a.db = h->d_loop_db; a.frame = h->loop_frames;
+  const size_t E = (size_t)c.exclude_recent;
+  a.n_candidates = h->loop_frames >= E ? h->loop_frames - E + 1 : 0;
+  a.partial = h->d_loop_best; a.best = h->d_loop_best + TLOAM_SC_MAX_BLOCKS;
+  a.device = h->device; a.stream = h->stream;
+  const tloam_sc_fn step[3] = {lib.bin, lib.finish, lib.search};
+  static const char* const names[3] = {"k_sc_bin", "k_sc_finish", "k_sc_search"};
+  for (int k = 0; k < 3; ++k) {
+    int e = 0;
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = step[k](&a)));
+    if (e != cudaSuccess) {
+      snprintf(h->last_error, sizeof(h->last_error), "loop closure: %s: %s", names[k], cudaGetErrorString((cudaError_t)e));
+      return TLOAM_B200_ERR_CUDA;
+    }
+  }
+  CU_TRY(cudaMemcpyAsync(h->h_loop_best, a.best, sizeof(tloam_sc_best), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaEventRecord(h->ev_loop, h->stream));
+  h->loop_query = (long long)h->loop_frames;
+  h->loop_frames++;
+  h->loop_has_result = true;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_loop_add_frame(tloam_b200_handle* h) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loop_on || h->raw_gen != h->seg_gen) return TLOAM_B200_ERR_NOT_READY;
+  return loop_add_impl(h, h->raw_scan, h->raw_n);
+}
+
+int tloam_b200_loop_add(tloam_b200_handle* h, const double* xyz, size_t n) {
+  if (!h || (!xyz && n) || n > ((size_t)1 << 30)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loop_on) return TLOAM_B200_ERR_NOT_READY;
+  CU_TRY(cudaSetDevice(h->device));
+  int rc;
+  if ((rc = ensure_dev(h, &h->d_loop_in, &h->cap_loop_in, n, false)) != TLOAM_B200_OK) return rc;
+  if (n && (rc = upload_host(h, h->d_loop_in, xyz, n * 24)) != TLOAM_B200_OK) return rc;
+  return loop_add_impl(h, h->d_loop_in, n);
+}
+
+int tloam_b200_loop_result(tloam_b200_handle* h, tloam_loop_result* out) {
+  if (!h || !out) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loop_on || !h->loop_has_result) return TLOAM_B200_ERR_NOT_READY;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaEventSynchronize(h->ev_loop));
+  const tloam_sc_best b = *h->h_loop_best;
+  const int S = h->loop_cfg.n_sector;
+  out->query = h->loop_query;
+  out->candidate = b.candidate;
+  out->shift = (int)b.shift;
+  const int k = 2 * out->shift >= S ? S - out->shift : -out->shift;      // yaw = -shift sectors, wrapped to (-pi, pi]
+  out->yaw = b.candidate >= 0 ? (double)k * (2.0 * M_PI / S) : 0.0;
+  out->distance = b.distance;
+  out->is_loop = b.candidate >= 0 && b.distance < h->loop_cfg.dist_threshold ? 1 : 0;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_loop_size(tloam_b200_handle* h, size_t* n_frames) {
+  if (!h || !n_frames) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loop_on) return TLOAM_B200_ERR_NOT_READY;
+  *n_frames = h->loop_frames;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_loop_descriptor_download(tloam_b200_handle* h, size_t frame, double* out) {
+  if (!h || !out) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loop_on) return TLOAM_B200_ERR_NOT_READY;
+  if (frame >= h->loop_frames) return TLOAM_B200_ERR_INVALID_ARG;
+  const size_t slot = TLOAM_SC_SLOT_DOUBLES(h->loop_cfg.n_ring, h->loop_cfg.n_sector);
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaMemcpyAsync(out, h->d_loop_db + frame * slot, slot * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
 }
 
 int tloam_b200_host_alloc(void** p, size_t bytes) {

@@ -7,6 +7,7 @@
 all arithmetic happens in libtloam_b200.so on the GPU.  There is no CPU path.
 """
 import ctypes as C
+import dataclasses
 
 import numpy as np
 
@@ -105,6 +106,18 @@ def packed_time(arr):
                 raise ValueError(f"packed_time: field {name!r} is {fdt.str}, not {dt.str}")
             return _lib.PackedTime(off, datatype, unit)
     raise ValueError("packed_time: the records have no field 'time', 't' or 'timestamp'")
+
+
+@dataclasses.dataclass(frozen=True)
+class LoopResult:
+    """tloam_loop_result: query = the newest added frame; candidate = its best earlier frame (-1: none eligible), found at
+    column shift `shift` with Scan Context distance `distance`; yaw (rad): p_candidate ~ Rz(yaw) . p_query."""
+    query: int
+    candidate: int
+    shift: int
+    yaw: float
+    distance: float
+    is_loop: bool
 
 
 class Frame:
@@ -733,6 +746,50 @@ class LocalRegistration:
         out = np.zeros((n.value, 3))
         self._check(self._L.tloam_b200_registered_scan_download(self._h, _dp(out), n.value, C.byref(n)), "registered_scan_download")
         return out
+
+    # ---- loop closure (Scan Context descriptors, exact search; include/tloam_b200.h "Loop closure") ----
+    def loop_enable(self, **overrides):
+        """start an empty descriptor database; overrides: fields of tloam_loop_config (lidar_height, n_ring, n_sector,
+        max_radius, exclude_recent, dist_threshold, initial_capacity_frames)"""
+        cfg = _lib.LoopConfig()
+        self._L.tloam_b200_loop_default_config(C.byref(cfg))
+        for k, v in overrides.items():
+            if not hasattr(cfg, k):
+                raise KeyError(k)
+            setattr(cfg, k, v)
+        self._check(self._L.tloam_b200_loop_enable(self._h, C.byref(cfg)), "loop_enable")
+        self._loop_shape = (cfg.n_ring, cfg.n_sector)
+
+    def loop_reset(self):
+        self._check(self._L.tloam_b200_loop_reset(self._h), "loop_reset")
+
+    def loop_add_frame(self):
+        """add the raw scan the last process_raw_scan* uploaded (corrected when timed), read on the device, and enqueue its
+        query; the result is read by loop_result"""
+        self._check(self._L.tloam_b200_loop_add_frame(self._h), "loop_add_frame")
+
+    def loop_add(self, scan):
+        """the same for a host cloud (n x 3, NaN / Inf rows allowed)"""
+        a = _f64(scan).reshape(-1, 3)
+        self._check(self._L.tloam_b200_loop_add(self._h, _dp(a), a.shape[0]), "loop_add")
+
+    def loop_result(self):
+        """the newest add's LoopResult (waits for that add only)"""
+        r = _lib.LoopResult()
+        self._check(self._L.tloam_b200_loop_result(self._h, C.byref(r)), "loop_result")
+        return LoopResult(r.query, r.candidate, r.shift, r.yaw, r.distance, bool(r.is_loop))
+
+    def loop_size(self):
+        n = C.c_size_t(0)
+        self._check(self._L.tloam_b200_loop_size(self._h, C.byref(n)), "loop_size")
+        return n.value
+
+    def loop_descriptor(self, frame):
+        """frame's (bins (n_ring, n_sector), ring key (n_ring,), column norms (n_sector,))"""
+        R, S = self._loop_shape
+        out = np.zeros(R * S + R + S)
+        self._check(self._L.tloam_b200_loop_descriptor_download(self._h, int(frame), _dp(out)), "loop_descriptor_download")
+        return out[:R * S].reshape(R, S), out[R * S:R * S + R], out[R * S + R:]
 
     # ---- shared map (multi-GPU) ----
     def map_blob_size(self):
