@@ -654,6 +654,83 @@ int tloam_b200_loop_size(tloam_b200_handle* h, size_t* n_frames);
  * (synchronises).  INVALID_ARG past the last frame. */
 int tloam_b200_loop_descriptor_download(tloam_b200_handle* h, size_t frame, double* out);
 
+/* ---- Loop verification (opt-in, on top of loop closure): a geometric check of a candidate that also gives the relative
+ * pose a pose-graph edge needs.  Scan Context's yaw is one sector coarse and it gives no translation; a descriptor match
+ * alone is no evidence of a loop.
+ *   - Keyframes.  After tloam_b200_loop_verify_enable, every tloam_b200_loop_add_frame / tloam_b200_loop_add also stores
+ *     that frame's keyframe: VoxelDownSample(voxel) of the scan's finite rows (the scan the descriptor reads), in the
+ *     sensor frame, by the global map's ordered path (each voxel the fixed-point average of its rows, voxels in ascending
+ *     (ix, iy, iz)).  Every add owns exactly one keyframe slot: an empty or all-non-finite scan, or one whose extent
+ *     reaches 2^21 voxels on an axis (the global map's key-range refusal), gets an empty keyframe, so keyframe i is always
+ *     loop frame i.  The store lives on the device; it is sized from an upper bound tightened by asynchronous read-backs
+ *     and grows x1.5 with one synchronisation, so an add does not synchronise.  The global map's buffers are not used.
+ *   - Verification of keyframe `query` (Q) against keyframe `candidate` (M) from the initial T = guess: T_cand_query with
+ *     p_cand ~ T . p_query (tloam_loop_result's yaw convention).  Per pass, for every q in Q: p = R q + t, each component
+ *     ((R[r][0] * qx + R[r][1] * qy) + R[r][2] * qz) + t[r], every operation separately rounded; its match is the nearest
+ *     m in M by d2 = ((px - mx)^2 + (py - my)^2) + (pz - mz)^2 (separately rounded), the lowest index on a tie: an exact
+ *     search over all of M, no grid, no radius.  The pair is an inlier iff d2 <= r * r.
+ *   - Step.  Gauss-Newton on SE(3), left perturbation: e = p - m, J = [I3, -[p]x]; H = sum J^T J, g = sum J^T e over the
+ *     inliers (a fixed reduction order: a run is bit-deterministic); delta = (upsilon, omega) = -H^-1 g by LDL^T; T <-
+ *     exp(delta) . T with Sophus' exp.  Fewer than 6 inliers, or a pivot that is not positive and finite, stops the run.
+ *   - Radius.  r starts at corr_dist_coarse.  After a step with |upsilon| < eps_translation and |omega| < eps_rotation: if
+ *     r == corr_dist_fine the run has converged, else r <- max(r / 2, corr_dist_fine).  At most max_iterations steps.
+ *   - Result, at the final T with one more pass at r = corr_dist_fine: inliers, rmse = sqrt(sum of their d2 / inliers) (0
+ *     without inliers), fitness = the mean nearest-neighbour d2 over ALL of Q (PCL's getFitnessScore(); the ground plane
+ *     matches almost anywhere, so an inlier ratio alone does not separate unrelated places), accepted = converged &&
+ *     fitness <= max_fitness.  An empty keyframe: no pass, T = guess, fitness +inf, not accepted.
+ *   - The kernels live in libtloam_b200_loopv.so, loaded from this library's directory on the first verification call; if
+ *     it is missing these calls return ERR_CUDA (tloam_b200_last_error names the file).  Off until enabled: nothing is
+ *     allocated or launched, and the loop calls give the bits and launch counts they give without it. */
+typedef struct tloam_loop_verify_config {
+  double voxel;                        /* keyframe down-sample, m */
+  double corr_dist_coarse;             /* first correspondence radius, m */
+  double corr_dist_fine;               /* last correspondence radius, m (<= corr_dist_coarse) */
+  int max_iterations;                  /* Gauss-Newton steps, 1 .. 200 */
+  double eps_translation;              /* m */
+  double eps_rotation;                 /* rad */
+  double max_fitness;                  /* m^2 */
+  size_t initial_capacity_points;      /* keyframe store points before the first growth */
+} tloam_loop_verify_config;
+enum {
+  TLOAM_LOOP_VERIFY_CONVERGED = 0,
+  TLOAM_LOOP_VERIFY_ITERATION_LIMIT = 1,
+  TLOAM_LOOP_VERIFY_FEW_INLIERS = 2,   /* fewer than 6 inliers in a pass */
+  TLOAM_LOOP_VERIFY_SINGULAR = 3,      /* an LDL^T pivot not positive and finite */
+  TLOAM_LOOP_VERIFY_EMPTY = 4          /* a keyframe without points */
+};
+typedef struct tloam_loop_verify_result {
+  long long query, candidate;
+  double T[16];                        /* T_cand_query, column-major: p_cand ~ T . p_query */
+  double fitness;                      /* m^2, mean nearest-neighbour d2 over every query keyframe point */
+  double rmse;                         /* m, over the inliers at corr_dist_fine */
+  long long inliers;
+  long long n_query_points, n_candidate_points;   /* keyframe sizes */
+  int iterations;                      /* Gauss-Newton steps taken */
+  int termination;                     /* TLOAM_LOOP_VERIFY_* */
+  int accepted;
+} tloam_loop_verify_result;
+/* voxel 0.5 m, corr_dist_coarse 4 m, corr_dist_fine 1 m, max_iterations 40, eps_translation 1e-4 m, eps_rotation 1e-5 rad,
+ * max_fitness 1.0 m^2, initial_capacity_points 2^21 (DESIGN.md section 4c has how they were chosen) */
+void tloam_b200_loop_verify_default_config(tloam_loop_verify_config* c);
+/* stores a keyframe with every later add.  Only while the loop database is empty (right after tloam_b200_loop_enable or
+ * tloam_b200_loop_reset), else NOT_READY.  tloam_b200_loop_reset empties the keyframes and keeps verification on;
+ * tloam_b200_loop_enable turns it off.  INVALID_ARG: cfg null; a value not finite or not > 0; corr_dist_fine >
+ * corr_dist_coarse; max_iterations outside [1, 200]. */
+int tloam_b200_loop_verify_enable(tloam_b200_handle* h, const tloam_loop_verify_config* cfg);
+/* frame's keyframe (n x 3 FP64) to out (synchronises); *n = its size.  INVALID_ARG past the last frame or when
+ * capacity_points < *n; NOT_READY when verification is off.  For tests and viewers. */
+int tloam_b200_loop_keyframe_download(tloam_b200_handle* h, size_t frame, double* out, size_t capacity_points, size_t* n);
+/* aligns keyframe query to keyframe candidate from guess (column-major 4 x 4; null: identity), enqueued behind every earlier
+ * add, and returns once the result is home.  BAD_POSE: guess not rigid; INVALID_ARG: an index out of range; NOT_READY:
+ * verification off. */
+int tloam_b200_loop_verify(tloam_b200_handle* h, long long query, long long candidate, const double guess[16],
+                           tloam_loop_verify_result* out);
+/* the last tloam_b200_loop_verify's matches at pass k, the pass at the k-th iterate of T (0: the guess; k = iterations:
+ * the final pass): per query keyframe point the candidate keyframe row (index) and its d2 (synchronises; *n = query
+ * keyframe size; either output may be null).  INVALID_ARG: k outside [0, iterations], capacity < *n, or a run that made
+ * no pass (an empty keyframe); NOT_READY: no verification since enable. */
+int tloam_b200_loop_verify_matches(tloam_b200_handle* h, int pass, int* index, double* d2, size_t capacity, size_t* n);
+
 /* Pinned host memory helpers (optional; pinned inputs make set_* a direct DMA, no staging threads). */
 int tloam_b200_host_alloc(void** p, size_t bytes);
 int tloam_b200_host_free(void* p);

@@ -15,12 +15,14 @@
 // (per-voxel averages, the reference's XYZI map); globalMap(points, intensity) reads it back.  updateGlobalMap also takes
 // the driver's sensor_msgs/PointCloud2 as it arrived (packed_scan_b200.hpp): one upload, unpacked on the device, its
 // intensity field (if any) carried into the map.  enableLoopDetection / addLoopFrame / loopResult add loop closure: a Scan
-// Context descriptor per frame and an exact search over every earlier frame, on the GPU.
+// Context descriptor per frame and an exact search over every earlier frame, on the GPU; enableLoopVerification / verifyLoop
+// check a candidate by a scan-to-scan ICP of down-sampled keyframes kept on the GPU and give the relative pose.
 // Without the reference headers (this repository's tests) define TLOAM_B200_MOCK_HOST_TYPES and provide the host types
 // (tests/mock/mock_tloam.hpp).
 #ifndef TLOAM_B200_FRONT_END_B200_HPP
 #define TLOAM_B200_FRONT_END_B200_HPP
 
+#include <cmath>
 #include <cstdio>
 #include <string>
 #include <vector>
@@ -147,7 +149,7 @@ class FrontEndB200 {
 
   // loop closure (include/tloam_b200.h "Loop closure"; the reference is pure odometry): every added frame gets a Scan
   // Context descriptor on the GPU and is compared with every frame at least cfg.exclude_recent frames older.  The library
-  // reports the best candidate; verifying it and correcting the poses belong to the caller's back end.
+  // reports the best candidate (verifyLoop checks it); correcting the poses belongs to the caller's back end.
   bool enableLoopDetection(const tloam_loop_config& cfg) {
     loop_ = report(tloam_b200_loop_enable(h_, &cfg), "enableLoopDetection");
     return loop_;
@@ -165,6 +167,24 @@ class FrontEndB200 {
   bool addLoopFrame(const CloudData& raw) { return report(tloam_b200_loop_add(h_, data(raw), size(raw)), "addLoopFrame"); }
   // the newest added frame's best earlier frame (waits for that add only); out.is_loop below cfg.dist_threshold
   bool loopResult(tloam_loop_result& out) { return report(tloam_b200_loop_result(h_, &out), "loopResult"); }
+
+  // loop verification (include/tloam_b200.h "Loop verification"): from now on every added loop frame also keeps a
+  // down-sampled keyframe on the GPU.  Call right after enableLoopDetection (an empty database).
+  bool enableLoopVerification(const tloam_loop_verify_config& cfg) {
+    return report(tloam_b200_loop_verify_enable(h_, &cfg), "enableLoopVerification");
+  }
+  bool enableLoopVerification() {
+    tloam_loop_verify_config c;
+    tloam_b200_loop_verify_default_config(&c);
+    return enableLoopVerification(c);
+  }
+  // aligns the loop result's query keyframe to its candidate's from Rz(lr.yaw) by a scan-to-scan ICP on the GPU; out.T is
+  // T_cand_query (column-major), to be handed to the back end when out.accepted
+  bool verifyLoop(const tloam_loop_result& lr, tloam_loop_verify_result& out) {
+    const double c = std::cos(lr.yaw), s = std::sin(lr.yaw);
+    const double guess[16] = {c, s, 0, 0, -s, c, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+    return report(tloam_b200_loop_verify(h_, lr.query, lr.candidate, guess, &out), "verifyLoop");
+  }
 
   // processCloud + setInputSource (ref: front_end.cpp:181-199, :313): the three clouds the segmentation nodelet publishes
   bool processCloud(CloudData& ground, CloudData& edge, CloudData& general) {

@@ -4,5 +4,5 @@ The product is the C-ABI CUDA library `libtloam_b200.so` (sources in tloam_b200/
 include/tloam_b200.h).  This package is only the Python host-side mirror of the reference interface plus the
 synthetic-scene generator used by tests and bench.py.  Importing it never touches oracle/.
 """
-from .registration import (BatchRegistration, Frame, LocalRegistration, LoopResult, RegistrationError, default_config,  # noqa: F401
-                           packed_scan, packed_time)
+from .registration import (BatchRegistration, Frame, LocalRegistration, LoopResult, LoopVerifyResult,  # noqa: F401
+                           RegistrationError, default_config, packed_scan, packed_time)

@@ -67,6 +67,20 @@ class LoopResult(C.Structure):
                 ("yaw", C.c_double), ("distance", C.c_double)]
 
 
+class LoopVerifyConfig(C.Structure):
+    """tloam_loop_verify_config (include/tloam_b200.h "Loop verification"): the keyframe voxel and the ICP's schedule."""
+    _fields_ = [("voxel", C.c_double), ("corr_dist_coarse", C.c_double), ("corr_dist_fine", C.c_double),
+                ("max_iterations", C.c_int), ("eps_translation", C.c_double), ("eps_rotation", C.c_double),
+                ("max_fitness", C.c_double), ("initial_capacity_points", C.c_size_t)]
+
+
+class LoopVerifyResult(C.Structure):
+    """tloam_loop_verify_result: T_cand_query (column-major) and the ICP's verdict."""
+    _fields_ = [("query", C.c_longlong), ("candidate", C.c_longlong), ("T", C.c_double * 16), ("fitness", C.c_double),
+                ("rmse", C.c_double), ("inliers", C.c_longlong), ("n_query_points", C.c_longlong),
+                ("n_candidate_points", C.c_longlong), ("iterations", C.c_int), ("termination", C.c_int), ("accepted", C.c_int)]
+
+
 class InnerTrace(C.Structure):
     _fields_ = [
         ("x_candidate", C.c_double * 6), ("candidate_cost", C.c_double), ("model_cost_change", C.c_double),
@@ -164,6 +178,8 @@ EXPORTS = [
     "tloam_b200_process_raw_scan_timed", "tloam_b200_process_raw_scan_packed_timed",
     "tloam_b200_loop_default_config", "tloam_b200_loop_enable", "tloam_b200_loop_reset", "tloam_b200_loop_add_frame",
     "tloam_b200_loop_add", "tloam_b200_loop_result", "tloam_b200_loop_size", "tloam_b200_loop_descriptor_download",
+    "tloam_b200_loop_verify_default_config", "tloam_b200_loop_verify_enable", "tloam_b200_loop_keyframe_download",
+    "tloam_b200_loop_verify", "tloam_b200_loop_verify_matches",
 ]
 
 _lib = None
@@ -328,5 +344,11 @@ def load():
     L.tloam_b200_loop_result.argtypes = [vp, C.POINTER(LoopResult)]
     L.tloam_b200_loop_size.argtypes = [vp, szp]
     L.tloam_b200_loop_descriptor_download.argtypes = [vp, C.c_size_t, dp]
+    L.tloam_b200_loop_verify_default_config.argtypes = [C.POINTER(LoopVerifyConfig)]
+    L.tloam_b200_loop_verify_default_config.restype = None
+    L.tloam_b200_loop_verify_enable.argtypes = [vp, C.POINTER(LoopVerifyConfig)]
+    L.tloam_b200_loop_keyframe_download.argtypes = [vp, C.c_size_t, dp, C.c_size_t, szp]
+    L.tloam_b200_loop_verify.argtypes = [vp, C.c_longlong, C.c_longlong, dp, C.POINTER(LoopVerifyResult)]
+    L.tloam_b200_loop_verify_matches.argtypes = [vp, C.c_int, C.POINTER(C.c_int), dp, C.c_size_t, szp]
     _lib = L
     return L

@@ -27,6 +27,7 @@
 #include "../../include/tloam_b200.h"
 #include "map_grid.cuh"
 #include "se3.cuh"
+#include "ldlt6.cuh"
 
 namespace tloam {
 
@@ -268,8 +269,5 @@ __device__ __forceinline__ void functor_line(const double c[3], const double a[3
     for (int j = 0; j < 6; ++j)
       J[i * 6 + j] = (S[i * 3 + 0] * M[0 * 6 + j] + S[i * 3 + 1] * M[1 * 6 + j] + S[i * 3 + 2] * M[2 * 6 + j]) * inv;
 }
-
-// upper-triangle index of (i,j), i <= j, row-major packed (21 entries)
-__host__ __device__ __forceinline__ int tri(int i, int j) { return i * 6 - (i * (i - 1)) / 2 + (j - i); }
 
 }  // namespace tloam

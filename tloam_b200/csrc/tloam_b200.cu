@@ -30,6 +30,7 @@
 #include "unpack_scan.h"
 #include "deskew.h"
 #include "scan_context.h"
+#include "loop_verify.h"
 
 
 
@@ -225,6 +226,24 @@ struct tloam_b200_handle {
   tloam_sc_best* h_loop_best = nullptr;    // pinned: the newest add's result, landed when ev_loop has
   cudaEvent_t ev_loop = nullptr;
   bool loop_has_result = false;            long long loop_query = -1;
+  // ---- loop verification (tloam_b200_loop_verify*, libtloam_b200_loopv.so): a keyframe per loop frame, kept by the
+  //      global map's ordered path in buffers of its own; nothing is allocated or launched until it is enabled.  The
+  //      host's bound of the store size = lv_known (exact, read asynchronously) + the rows added since ----
+  bool lv_on = false;
+  tloam_loop_verify_config lv_cfg;
+  GMapState* d_lv_st = nullptr;            // count = store points, frames = keyframes
+  double* d_lv_pose = nullptr;             // identity
+  double* d_lv_pts = nullptr;              size_t cap_lv = 0;                                   // keyframe points
+  unsigned long long* d_lv_off = nullptr;  size_t cap_lv_off = 0;                               // keyframe f: [off[f], off[f + 1])
+  double* d_lv_reg = nullptr;              size_t cap_lv_reg = 0;
+  double* d_lv_fin = nullptr;              size_t cap_lv_fin = 0;
+  unsigned long long lv_cum = 0, lv_known_cum = 0, lv_known = 0;
+  size_t lv_growths = 0;
+  GMapProbe lv_probes[4];                  int lv_probe_next = 0;
+  tloam_lv_state* d_lv_state = nullptr;
+  unsigned char* d_lv_scratch = nullptr;   size_t cap_lv_scratch = 0;                           // the verification's scratch
+  bool lv_ran = false;                     int lv_passes = 0;   unsigned long long lv_nq = 0;   // the last verification
+  const int* lv_match_index = nullptr;    const double* lv_match_d2 = nullptr;                 // its matches, pass-major
 };
 
 // launch bookkeeping: counts the kernel and, in profiling mode, brackets it with events
@@ -424,6 +443,9 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   cudaFree(h->d_loop_db); cudaFree(h->d_loop_dirs); cudaFree(h->d_loop_in); cudaFree(h->d_loop_best);
   if (h->h_loop_best) cudaFreeHost(h->h_loop_best);
   if (h->ev_loop) cudaEventDestroy(h->ev_loop);
+  cudaFree(h->d_lv_st); cudaFree(h->d_lv_pose); cudaFree(h->d_lv_pts); cudaFree(h->d_lv_off); cudaFree(h->d_lv_reg);
+  cudaFree(h->d_lv_fin); cudaFree(h->d_lv_state); cudaFree(h->d_lv_scratch);
+  for (auto& pr : h->lv_probes) { if (pr.ev) cudaEventDestroy(pr.ev); if (pr.h_count) cudaFreeHost(pr.h_count); }
   for (int i = 0; i < 2; ++i) if (h->ev_stage_free[i]) cudaEventDestroy(h->ev_stage_free[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_fit[i]) cudaEventDestroy(h->ev_fit[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_res[i]) cudaEventDestroy(h->ev_res[i]);
@@ -3807,13 +3829,20 @@ int tloam_b200_loop_enable(tloam_b200_handle* h, const tloam_loop_config* cfg) {
   h->loop_cfg = *cfg;
   h->loop_frames = 0; h->loop_growths = 0; h->loop_has_result = false; h->loop_query = -1;
   h->loop_on = true;
+  h->lv_on = false;                        // verification is enabled anew on the empty database
   return TLOAM_B200_OK;
 }
+
+static int lv_clear(tloam_b200_handle* h);
 
 int tloam_b200_loop_reset(tloam_b200_handle* h) {
   if (!h) return TLOAM_B200_ERR_INVALID_ARG;
   if (!h->loop_on) return TLOAM_B200_ERR_NOT_READY;
   h->loop_frames = 0; h->loop_has_result = false; h->loop_query = -1;
+  if (h->lv_on) {
+    CU_TRY(cudaSetDevice(h->device));
+    return lv_clear(h);
+  }
   return TLOAM_B200_OK;
 }
 
@@ -3833,6 +3862,8 @@ static int loop_grow(tloam_b200_handle* h) {
   return TLOAM_B200_OK;
 }
 
+static int lv_append(tloam_b200_handle* h, const double* d_in, size_t n);
+
 // the descriptor of the n rows at d_xyz (device) into the next slot, then its query over every slot <= frame - exclude_recent;
 // the result lands in the pinned slot, ev_loop marks it
 static int loop_add_impl(tloam_b200_handle* h, const double* d_xyz, size_t n) {
@@ -3841,6 +3872,7 @@ static int loop_add_impl(tloam_b200_handle* h, const double* d_xyz, size_t n) {
   if (rc != TLOAM_B200_OK) return rc;
   CU_TRY(cudaSetDevice(h->device));
   if (h->loop_frames == h->loop_cap && (rc = loop_grow(h)) != TLOAM_B200_OK) return rc;
+  if (h->lv_on && (rc = lv_append(h, d_xyz, n)) != TLOAM_B200_OK) return rc;
   const tloam_loop_config& c = h->loop_cfg;
   tloam_sc_args a;
   a.n_ring = c.n_ring; a.n_sector = c.n_sector; a.lidar_height = c.lidar_height; a.max_radius = c.max_radius;
@@ -3914,6 +3946,307 @@ int tloam_b200_loop_descriptor_download(tloam_b200_handle* h, size_t frame, doub
   const size_t slot = TLOAM_SC_SLOT_DOUBLES(h->loop_cfg.n_ring, h->loop_cfg.n_sector);
   CU_TRY(cudaSetDevice(h->device));
   CU_TRY(cudaMemcpyAsync(out, h->d_loop_db + frame * slot, slot * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Loop verification (a keyframe per loop frame, by the global map's ordered path into buffers of its own; the commit and
+// the ICP kernels in loop_verify.cu, loaded from libtloam_b200_loopv.so on the first verification call).
+// ---------------------------------------------------------------------------------------------
+struct LoopvLib { tloam_lv_verify_fn verify = nullptr; tloam_lv_commit_fn commit = nullptr; };
+static std::mutex g_loopv_mu;
+static LoopvLib g_loopv;
+
+static int loopv_load(tloam_b200_handle* h, LoopvLib* out) {
+  std::lock_guard<std::mutex> lk(g_loopv_mu);
+  if (!g_loopv.verify) {
+    const std::string path = sibling_path("libtloam_b200_loopv.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    LoopvLib l;
+    if (so) {
+      l.verify = reinterpret_cast<tloam_lv_verify_fn>(dlsym(so, "tloam_lv_verify"));
+      l.commit = reinterpret_cast<tloam_lv_commit_fn>(dlsym(so, "tloam_lv_commit"));
+    }
+    if (!l.verify || !l.commit) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "loop verification: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_loopv = l;
+  }
+  *out = g_loopv;
+  return TLOAM_B200_OK;
+}
+
+static int lv_status(tloam_b200_handle* h, int e, const char* where) {
+  if (e == cudaSuccess) return TLOAM_B200_OK;
+  snprintf(h->last_error, sizeof(h->last_error), "loop verification: %s: %s", where, cudaGetErrorString((cudaError_t)e));
+  return TLOAM_B200_ERR_CUDA;
+}
+
+void tloam_b200_loop_verify_default_config(tloam_loop_verify_config* c) {
+  c->voxel = 0.5;
+  c->corr_dist_coarse = 4.0; c->corr_dist_fine = 1.0;
+  c->max_iterations = 40;
+  c->eps_translation = 1e-4; c->eps_rotation = 1e-5;
+  c->max_fitness = 1.0;
+  c->initial_capacity_points = (size_t)1 << 21;
+}
+
+// an empty store (keyframe table offsets[0] = 0)
+static int lv_clear(tloam_b200_handle* h) {
+  CU_TRY(cudaMemsetAsync(h->d_lv_st, 0, sizeof(GMapState), h->stream));
+  CU_TRY(cudaMemsetAsync(h->d_lv_off, 0, sizeof(unsigned long long), h->stream));
+  h->lv_cum = h->lv_known_cum = h->lv_known = 0;
+  for (auto& pr : h->lv_probes) pr.pending = false;
+  h->lv_ran = false; h->lv_passes = 0; h->lv_nq = 0;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_loop_verify_enable(tloam_b200_handle* h, const tloam_loop_verify_config* c) {
+  if (!h || !c) return TLOAM_B200_ERR_INVALID_ARG;
+  const double v[6] = {c->voxel, c->corr_dist_coarse, c->corr_dist_fine, c->eps_translation, c->eps_rotation, c->max_fitness};
+  for (double x : v)
+    if (!std::isfinite(x) || !(x > 0.0)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (c->corr_dist_fine > c->corr_dist_coarse || c->max_iterations < 1 || c->max_iterations > 200) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loop_on || h->loop_frames != 0) return TLOAM_B200_ERR_NOT_READY;
+  LoopvLib lib;
+  int rc = loopv_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (!h->d_lv_st) {
+    CU_TRY(cudaMalloc(&h->d_lv_st, sizeof(GMapState)));
+    CU_TRY(cudaMalloc(&h->d_lv_pose, 16 * sizeof(double)));
+    const double eye[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+    CU_TRY(cudaMemcpy(h->d_lv_pose, eye, sizeof(eye), cudaMemcpyHostToDevice));
+    CU_TRY(cudaMalloc(&h->d_lv_state, sizeof(tloam_lv_state)));
+    for (auto& pr : h->lv_probes) {
+      CU_TRY(cudaEventCreateWithFlags(&pr.ev, cudaEventDisableTiming));
+      CU_TRY(cudaMallocHost(&pr.h_count, sizeof(unsigned long long)));
+    }
+  }
+  const size_t cap = c->initial_capacity_points ? c->initial_capacity_points : 1;
+  if (cap != h->cap_lv) {
+    cudaFree(h->d_lv_pts); h->d_lv_pts = nullptr; h->cap_lv = 0;
+    CU_TRY(cudaMalloc(&h->d_lv_pts, cap * 3 * sizeof(double)));
+    h->cap_lv = cap;
+  }
+  const size_t cap_off = h->loop_cap + 2;    // the descriptor database's capacity, plus the closing entry
+  if (cap_off > h->cap_lv_off) {
+    cudaFree(h->d_lv_off); h->d_lv_off = nullptr; h->cap_lv_off = 0;
+    CU_TRY(cudaMalloc(&h->d_lv_off, cap_off * sizeof(unsigned long long)));
+    h->cap_lv_off = cap_off;
+  }
+  h->lv_cfg = *c;
+  h->lv_growths = 0;
+  h->lv_on = true;
+  return lv_clear(h);
+}
+
+static void lv_harvest(tloam_b200_handle* h) {
+  for (auto& pr : h->lv_probes) {
+    if (!pr.pending) continue;
+    if (cudaEventQuery(pr.ev) != cudaSuccess) { cudaGetLastError(); continue; }
+    pr.pending = false;
+    if (pr.cum >= h->lv_known_cum) { h->lv_known_cum = pr.cum; h->lv_known = *pr.h_count; }
+  }
+}
+
+// the one place a keyframe add synchronises: the store (or its table) may not hold the next keyframe.  The exact size is
+// read, and the store grows to max(1.5 x capacity, exact size + n rows); the table x1.5.
+static int lv_grow(tloam_b200_handle* h, size_t n) {
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  GMapState st;
+  CU_TRY(cudaMemcpyAsync(&st, h->d_lv_st, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  h->lv_known = st.count; h->lv_known_cum = h->lv_cum;
+  for (auto& pr : h->lv_probes) pr.pending = false;
+  if (st.count + n > h->cap_lv) {
+    size_t ncap = h->cap_lv + h->cap_lv / 2;
+    if (ncap < st.count + n) ncap = st.count + n;
+    double* q = nullptr;
+    CU_TRY(cudaMalloc(&q, ncap * 3 * sizeof(double)));
+    if (st.count) CU_TRY(cudaMemcpyAsync(q, h->d_lv_pts, st.count * 3 * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_lv_pts);
+    h->d_lv_pts = q; h->cap_lv = ncap;
+  }
+  if (h->loop_frames + 2 > h->cap_lv_off) {
+    size_t ncap = h->cap_lv_off + h->cap_lv_off / 2;
+    if (ncap < h->loop_frames + 2) ncap = h->loop_frames + 2;
+    unsigned long long* q = nullptr;
+    CU_TRY(cudaMalloc(&q, ncap * sizeof(unsigned long long)));
+    CU_TRY(cudaMemcpyAsync(q, h->d_lv_off, (h->loop_frames + 1) * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_lv_off);
+    h->d_lv_off = q; h->cap_lv_off = ncap;
+  }
+  h->lv_growths++;
+  return TLOAM_B200_OK;
+}
+
+// keyframe loop_frames = VoxelDownSample(voxel) of the finite rows of the n rows at d_in: gmap_append_impl's transform ->
+// guard -> voxel_pipeline(sorted) -> emit at pose I, then a commit that closes the slot whatever the frame held
+static int lv_append(tloam_b200_handle* h, const double* d_in, size_t n) {
+  LoopvLib lib;
+  int rc = loopv_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  lv_harvest(h);
+  const unsigned long long bound = h->lv_known + (h->lv_cum - h->lv_known_cum) + n;   // voxels <= finite rows <= rows
+  if (bound > h->cap_lv || h->loop_frames + 2 > h->cap_lv_off)
+    if ((rc = lv_grow(h, n)) != TLOAM_B200_OK) return rc;
+  if ((rc = ensure_dev(h, &h->d_lv_reg, &h->cap_lv_reg, n, false)) != TLOAM_B200_OK) return rc;
+  if ((rc = ensure_dev(h, &h->d_lv_fin, &h->cap_lv_fin, n, false)) != TLOAM_B200_OK) return rc;
+  GMapState* st = h->d_lv_st;
+  const double voxel = h->lv_cfg.voxel;
+  CU_TRY(cudaMemsetAsync(&st->n_fin, 0, sizeof(GMapState) - offsetof(GMapState, n_fin), h->stream));
+  const unsigned tb = 256, gb = (unsigned)((n + tb - 1) / tb);
+  if (n) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_transform<<<gb, tb, 0, h->stream>>>(d_in, (unsigned)n, h->d_lv_pose, h->d_lv_reg, h->d_lv_fin, st)));
+  if (n) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_guard<<<1, 32, 0, h->stream>>>(st, voxel)));
+  VoxSorted vs;
+  if ((rc = voxel_pipeline(h, h->d_lv_fin, n, &st->n_fin, 0u, nullptr, nullptr, nullptr, 0.0, voxel, nullptr, &st->n_vox,
+                           h->stream, 0, &vs)) != TLOAM_B200_OK) return rc;
+  if (n) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_emit<<<gb, tb, 0, h->stream>>>(vs.a, vs.slots, h->d_lv_pts, st, h->cap_lv)));
+  int e = 0;
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.commit(&st->n_vox, &st->refused, &st->count, &st->frames, &st->flags, h->d_lv_off, h->cap_lv,
+                                                 h->device, h->stream)));
+  if ((rc = lv_status(h, e, "k_lv_commit")) != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaGetLastError());
+  h->lv_cum += n;
+  tloam_b200_handle::GMapProbe& pr = h->lv_probes[h->lv_probe_next];
+  if (!pr.pending) {
+    CU_TRY(cudaMemcpyAsync(pr.h_count, &st->count, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaEventRecord(pr.ev, h->stream));
+    pr.cum = h->lv_cum; pr.pending = true;
+    h->lv_probe_next = (h->lv_probe_next + 1) & 3;
+  }
+  return TLOAM_B200_OK;
+}
+
+// synchronises and reads keyframe f's range; a store that refused a keyframe for want of room is a bug, not an input error
+static int lv_range(tloam_b200_handle* h, size_t f, unsigned long long* first, unsigned long long* n) {
+  unsigned long long off[2];
+  unsigned flags = 0;
+  CU_TRY(cudaMemcpyAsync(off, h->d_lv_off + f, sizeof(off), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaMemcpyAsync(&flags, &h->d_lv_st->flags, sizeof(flags), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (flags & kGMapOverflow) {
+    snprintf(h->last_error, sizeof(h->last_error), "loop verification: the device-side capacity check refused a keyframe");
+    return TLOAM_B200_ERR_CUDA;
+  }
+  *first = off[0]; *n = off[1] - off[0];
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_loop_keyframe_download(tloam_b200_handle* h, size_t frame, double* out, size_t capacity_points, size_t* n) {
+  if (!h || !n) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->lv_on) return TLOAM_B200_ERR_NOT_READY;
+  if (frame >= h->loop_frames) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  unsigned long long first = 0, cnt = 0;
+  int rc = lv_range(h, frame, &first, &cnt);
+  if (rc != TLOAM_B200_OK) return rc;
+  *n = cnt;
+  if (capacity_points < cnt || (!out && cnt)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (cnt) CU_TRY(cudaMemcpyAsync(out, h->d_lv_pts + 3 * first, cnt * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_loop_verify(tloam_b200_handle* h, long long query, long long candidate, const double guess[16],
+                           tloam_loop_verify_result* out) {
+  if (!h || !out) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->lv_on) return TLOAM_B200_ERR_NOT_READY;
+  if (query < 0 || candidate < 0 || (size_t)query >= h->loop_frames || (size_t)candidate >= h->loop_frames)
+    return TLOAM_B200_ERR_INVALID_ARG;
+  double T[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+  if (guess) memcpy(T, guess, sizeof(T));
+  Pose7 p7;
+  if (!pose_from_matrix(T, p7) || T[3] != 0.0 || T[7] != 0.0 || T[11] != 0.0 || T[15] != 1.0) return TLOAM_B200_ERR_BAD_POSE;
+  LoopvLib lib;
+  int rc = loopv_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  unsigned long long q0 = 0, nq = 0, m0 = 0, nm = 0;
+  if ((rc = lv_range(h, (size_t)query, &q0, &nq)) != TLOAM_B200_OK) return rc;
+  if ((rc = lv_range(h, (size_t)candidate, &m0, &nm)) != TLOAM_B200_OK) return rc;
+  const tloam_loop_verify_config& c = h->lv_cfg;
+  memset(out, 0, sizeof(*out));
+  out->query = query; out->candidate = candidate;
+  memcpy(out->T, T, sizeof(T));
+  out->n_query_points = (long long)nq; out->n_candidate_points = (long long)nm;
+  h->lv_ran = true; h->lv_passes = 0; h->lv_nq = nq;
+  if (nq == 0 || nm == 0) {
+    out->termination = TLOAM_LOOP_VERIFY_EMPTY;
+    out->fitness = INFINITY;
+    return TLOAM_B200_OK;
+  }
+  // M is split over grid y until the search has about four blocks per SM of an H100 SXM (132)
+  const unsigned long long qb = (nq + TLOAM_LV_THREADS - 1) / TLOAM_LV_THREADS, tiles = (nm + TLOAM_LV_THREADS - 1) / TLOAM_LV_THREADS;
+  unsigned long long splits = (4 * 132 + qb - 1) / qb;
+  if (splits > tiles) splits = tiles;
+  if (splits < 1) splits = 1;
+  const size_t passes = (size_t)c.max_iterations + 1;
+  const size_t o_sums = round_up(splits * nq * sizeof(tloam_lv_best), 256);
+  const size_t o_idx = o_sums + round_up(qb * TLOAM_LV_SUMS * sizeof(double), 256);
+  const size_t o_d2 = o_idx + round_up(passes * nq * sizeof(int), 256);
+  const size_t bytes = o_d2 + passes * nq * sizeof(double);
+  if (bytes > h->cap_lv_scratch) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_lv_scratch); h->d_lv_scratch = nullptr; h->cap_lv_scratch = 0;
+    CU_TRY(cudaMalloc(&h->d_lv_scratch, bytes));
+    h->cap_lv_scratch = bytes;
+  }
+  tloam_lv_state s;
+  memset(&s, 0, sizeof(s));
+  for (int r = 0; r < 3; ++r) {
+    for (int k = 0; k < 3; ++k) s.R[3 * r + k] = T[4 * k + r];
+    s.t[r] = T[12 + r];
+  }
+  s.r = c.corr_dist_coarse;
+  s.term = TLOAM_LOOP_VERIFY_ITERATION_LIMIT;
+  CU_TRY(cudaMemcpyAsync(h->d_lv_state, &s, sizeof(s), cudaMemcpyHostToDevice, h->stream));   // pageable: staged before return
+  tloam_lv_args a;
+  a.pts = h->d_lv_pts; a.q0 = q0; a.nq = nq; a.m0 = m0; a.nm = nm;
+  a.corr_dist_coarse = c.corr_dist_coarse; a.corr_dist_fine = c.corr_dist_fine;
+  a.eps_translation = c.eps_translation; a.eps_rotation = c.eps_rotation; a.max_iterations = c.max_iterations;
+  a.splits = (unsigned)splits; a.state = h->d_lv_state;
+  a.part = reinterpret_cast<tloam_lv_best*>(h->d_lv_scratch);
+  a.sums = reinterpret_cast<double*>(h->d_lv_scratch + o_sums);
+  a.match_index = reinterpret_cast<int*>(h->d_lv_scratch + o_idx);
+  a.match_d2 = reinterpret_cast<double*>(h->d_lv_scratch + o_d2);
+  a.device = h->device; a.stream = h->stream;
+  h->lv_match_index = a.match_index; h->lv_match_d2 = a.match_d2;
+  int e = 0, launches = 0;
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.verify(&a, &launches)));
+  h->launches += launches > 0 ? launches - 1 : 0;
+  if ((rc = lv_status(h, e, "k_lv_*")) != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaMemcpyAsync(&s, h->d_lv_state, sizeof(s), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  for (int r = 0; r < 3; ++r) {
+    for (int k = 0; k < 3; ++k) out->T[4 * k + r] = s.R[3 * r + k];
+    out->T[12 + r] = s.t[r];
+  }
+  out->fitness = s.fitness; out->rmse = s.rmse; out->inliers = (long long)s.inliers;
+  out->iterations = s.iter; out->termination = s.term;
+  out->accepted = s.term == TLOAM_LOOP_VERIFY_CONVERGED && s.fitness <= c.max_fitness ? 1 : 0;
+  h->lv_passes = s.iter + 1;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_loop_verify_matches(tloam_b200_handle* h, int pass, int* index, double* d2, size_t capacity, size_t* n) {
+  if (!h || !n) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->lv_on || !h->lv_ran) return TLOAM_B200_ERR_NOT_READY;
+  *n = h->lv_nq;
+  if (pass < 0 || pass >= h->lv_passes || capacity < h->lv_nq) return TLOAM_B200_ERR_INVALID_ARG;
+  const size_t nq = h->lv_nq;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (index) CU_TRY(cudaMemcpyAsync(index, h->lv_match_index + (size_t)pass * nq, nq * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  if (d2) CU_TRY(cudaMemcpyAsync(d2, h->lv_match_d2 + (size_t)pass * nq, nq * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   CU_TRY(cudaStreamSynchronize(h->stream));
   return TLOAM_B200_OK;
 }

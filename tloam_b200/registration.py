@@ -8,6 +8,7 @@ all arithmetic happens in libtloam_b200.so on the GPU.  There is no CPU path.
 """
 import ctypes as C
 import dataclasses
+import math
 
 import numpy as np
 
@@ -118,6 +119,32 @@ class LoopResult:
     yaw: float
     distance: float
     is_loop: bool
+
+
+@dataclasses.dataclass(frozen=True)
+class LoopVerifyResult:
+    """tloam_loop_verify_result: T (4 x 4) = T_cand_query, p_candidate ~ T . p_query; termination is one of
+    LoopVerifyResult.CONVERGED .. EMPTY; accepted = converged and fitness <= max_fitness."""
+    query: int
+    candidate: int
+    T: np.ndarray
+    fitness: float
+    rmse: float
+    inliers: int
+    n_query_points: int
+    n_candidate_points: int
+    iterations: int
+    termination: int
+    accepted: bool
+    CONVERGED, ITERATION_LIMIT, FEW_INLIERS, SINGULAR, EMPTY = range(5)
+
+
+def rz(yaw):
+    """the 4 x 4 rotation about z by yaw (rad); the C library's cos / sin, as the C++ shim's verifyLoop"""
+    c, s = math.cos(yaw), math.sin(yaw)
+    T = np.eye(4)
+    T[:2, :2] = [[c, -s], [s, c]]
+    return T
 
 
 class Frame:
@@ -790,6 +817,58 @@ class LocalRegistration:
         out = np.zeros(R * S + R + S)
         self._check(self._L.tloam_b200_loop_descriptor_download(self._h, int(frame), _dp(out)), "loop_descriptor_download")
         return out[:R * S].reshape(R, S), out[R * S:R * S + R], out[R * S + R:]
+
+    # ---- loop verification (keyframes and a scan-to-scan ICP; include/tloam_b200.h "Loop verification") ----
+    def loop_verify_enable(self, **overrides):
+        """keep a keyframe of every later loop add (only while the database is empty); overrides: fields of
+        tloam_loop_verify_config (voxel, corr_dist_coarse, corr_dist_fine, max_iterations, eps_translation, eps_rotation,
+        max_fitness, initial_capacity_points)"""
+        cfg = _lib.LoopVerifyConfig()
+        self._L.tloam_b200_loop_verify_default_config(C.byref(cfg))
+        for k, v in overrides.items():
+            if not hasattr(cfg, k):
+                raise KeyError(k)
+            setattr(cfg, k, v)
+        self._check(self._L.tloam_b200_loop_verify_enable(self._h, C.byref(cfg)), "loop_verify_enable")
+
+    def loop_keyframe(self, frame):
+        """frame's keyframe (n x 3), sensor frame"""
+        n = C.c_size_t(0)
+        rc = self._L.tloam_b200_loop_keyframe_download(self._h, int(frame), None, 0, C.byref(n))   # the size
+        if rc != _lib.ERR_INVALID_ARG or n.value == 0:
+            self._check(rc, "loop_keyframe_download")
+            return np.zeros((0, 3))
+        out = np.zeros((n.value, 3))
+        self._check(self._L.tloam_b200_loop_keyframe_download(self._h, int(frame), _dp(out), n.value, C.byref(n)),
+                    "loop_keyframe_download")
+        return out
+
+    def loop_verify(self, query, candidate, guess=None, yaw=None):
+        """align keyframe query to keyframe candidate from guess (4 x 4; default identity), or from Rz(yaw) (the loop
+        result's yaw); returns a LoopVerifyResult"""
+        if yaw is not None:
+            if guess is not None:
+                raise ValueError("loop_verify: give guess or yaw, not both")
+            guess = rz(yaw)
+        g = None if guess is None else np.asfortranarray(np.asarray(guess, dtype=np.float64).reshape(4, 4)).ravel(order="F").copy()
+        r = _lib.LoopVerifyResult()
+        self._check(self._L.tloam_b200_loop_verify(self._h, int(query), int(candidate), None if g is None else _dp(g), C.byref(r)),
+                    "loop_verify")
+        T = np.array(r.T[:]).reshape(4, 4, order="F")
+        return LoopVerifyResult(r.query, r.candidate, T, r.fitness, r.rmse, r.inliers, r.n_query_points, r.n_candidate_points,
+                                r.iterations, r.termination, bool(r.accepted))
+
+    def loop_verify_matches(self, k):
+        """the last loop_verify's matches at pass k (the k-th iterate of T; k = iterations: the final pass): per query
+        keyframe point the candidate keyframe row (-1: none) and its d2"""
+        n = C.c_size_t(0)
+        rc = self._L.tloam_b200_loop_verify_matches(self._h, int(k), None, None, 0, C.byref(n))    # the size
+        if rc != _lib.ERR_INVALID_ARG or n.value == 0:
+            self._check(rc, "loop_verify_matches")
+        idx, d2 = np.zeros(n.value, dtype=np.int32), np.zeros(n.value)
+        self._check(self._L.tloam_b200_loop_verify_matches(self._h, int(k), idx.ctypes.data_as(C.POINTER(C.c_int)), _dp(d2), n.value,
+                                                           C.byref(n)), "loop_verify_matches")
+        return idx, d2
 
     # ---- shared map (multi-GPU) ----
     def map_blob_size(self):
