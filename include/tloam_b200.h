@@ -731,6 +731,85 @@ int tloam_b200_loop_verify(tloam_b200_handle* h, long long query, long long cand
  * no pass (an empty keyframe); NOT_READY: no verification since enable. */
 int tloam_b200_loop_verify_matches(tloam_b200_handle* h, int pass, int* index, double* d2, size_t capacity, size_t* n);
 
+/* ---- Pose graph (opt-in): the back end of loop closure.  The odometry chain and the accepted loop verifications are
+ * optimised together on the device; the corrected poses and the map -> odom correction come out.  The global map, the
+ * keyframes and the odometry state are not touched.
+ *   - Nodes.  Node k keeps the pose O_k it was added with for ever.  tloam_b200_pose_graph_add_node records a host pose;
+ *     tloam_b200_pose_graph_add_node_chained records the device pose of the frame the handle enqueued last
+ *     (tloam_b200_get_result's pose, the one tloam_b200_global_map_append_frame_chained reads; identity before the first
+ *     match) by a copy on the handle's stream, without synchronising.  Calling it next to every tloam_b200_loop_add_frame
+ *     keeps node i = loop frame i.  The store grows x1.5 with one synchronisation.
+ *   - Edges.  Odometry (k - 1, k) for every k >= 1 with Z = O_{k-1}^-1 O_k and Omega_odom = diag(1 / sigma_odom_translation^2
+ *     x 3, 1 / sigma_odom_rotation^2 x 3); loop (v->candidate, v->query) with Z = v->T and Omega_loop alike.
+ *   - Cost sum_e r^T Omega r, r = log(Z^-1 T_i^-1 T_j) (se3.cuh's Sophus log, (upsilon, omega) order).
+ *   - Step.  Gauss-Newton with a left perturbation T_k <- exp(delta_k) T_k; node 0 is fixed (the gauge).  First-order
+ *     Jacobians J_j = Ad(T_j^-1), J_i = -J_j (the right-Jacobian inverse of r taken as I).  The normal equations
+ *     H = M + B^T Omega_loop B (M the odometry chain, B the loop rows) are solved exactly by Woodbury: a block LDL^T of M
+ *     along the chain, Y = M^-1 B^T, the capacitance S = Omega_loop^-1 + B Y by a dense Cholesky, delta = u - Y S^-1 B u
+ *     with u = M^-1 b.  Every reduction runs in a fixed order: a run is bit-reproducible.
+ *   - Every optimisation starts from the odometry poses O_k, so a result depends on the graph only.
+ *   - Termination.  CONVERGED: the step's largest |upsilon| component < eps_translation and largest |omega| component
+ *     < eps_rotation (the step is applied).  COST_INCREASED: the cost after a larger step is not <= the cost before; the
+ *     step is reverted.  ITERATION_LIMIT after max_iterations accepted steps.  SINGULAR: an LDL^T or Cholesky pivot that
+ *     is not positive and finite.  NO_LOOPS: no loop edge; nothing is launched and the poses are the O_k bit for bit.
+ *   - Memory per optimisation: Y is 6 (N - 1) x (6 L + 1) doubles and S 6 L x (6 L + 1) doubles for N nodes and L loop
+ *     edges (4 541 nodes, 183 loops: 240 MB; the default max_loop_edges 1 024 allows 6 GB at 20 000 nodes).
+ *   - The kernels live in libtloam_b200_pg.so, loaded from this library's directory on the first optimisation; if it is
+ *     missing tloam_b200_pose_graph_optimize returns ERR_CUDA (tloam_b200_last_error names the file).  Off until enabled:
+ *     nothing is allocated or launched, and every other call returns NOT_READY. */
+typedef struct tloam_pose_graph_config {
+  double sigma_odom_translation;       /* m */
+  double sigma_odom_rotation;          /* rad */
+  double sigma_loop_translation;       /* m */
+  double sigma_loop_rotation;          /* rad */
+  int max_iterations;                  /* Gauss-Newton steps, 1 .. 100 */
+  double eps_translation;              /* m */
+  double eps_rotation;                 /* rad */
+  size_t max_loop_edges;               /* bounds the optimisation's memory (above) */
+  size_t initial_capacity_nodes;       /* node store before the first growth */
+} tloam_pose_graph_config;
+enum {
+  TLOAM_POSE_GRAPH_CONVERGED = 0,
+  TLOAM_POSE_GRAPH_ITERATION_LIMIT = 1,
+  TLOAM_POSE_GRAPH_COST_INCREASED = 2,
+  TLOAM_POSE_GRAPH_SINGULAR = 3,
+  TLOAM_POSE_GRAPH_NO_LOOPS = 4
+};
+typedef struct tloam_pose_graph_result {
+  long long nodes, loop_edges;
+  int iterations;                      /* accepted steps */
+  int termination;                     /* TLOAM_POSE_GRAPH_* */
+  double initial_cost;                 /* at the odometry poses */
+  double final_cost;                   /* at the returned poses */
+  double step_translation;             /* the last step's largest |upsilon| component, m */
+  double step_rotation;                /* the last step's largest |omega| component, rad */
+} tloam_pose_graph_result;
+/* sigma_odom 0.02 m / 0.001 rad, sigma_loop 0.3 m / 0.002 rad, max_iterations 20, eps_translation 1e-4 m, eps_rotation
+ * 1e-6 rad, max_loop_edges 1024, initial_capacity_nodes 4096 (DESIGN.md section 4c has how they were chosen) */
+void tloam_b200_pose_graph_default_config(tloam_pose_graph_config* c);
+/* starts an empty graph (a graph already on is emptied).  INVALID_ARG: cfg null; a sigma or eps not finite or not > 0;
+ * max_iterations outside [1, 100]; max_loop_edges 0. */
+int tloam_b200_pose_graph_enable(tloam_b200_handle* h, const tloam_pose_graph_config* cfg);
+/* empties the graph (nodes, loop edges, the last optimisation) and keeps the configuration */
+int tloam_b200_pose_graph_reset(tloam_b200_handle* h);
+/* node N = pose (column-major 4 x 4).  BAD_POSE: not rigid */
+int tloam_b200_pose_graph_add_node(tloam_b200_handle* h, const double pose[16]);
+/* node N = the device pose of the last enqueued frame (no synchronisation) */
+int tloam_b200_pose_graph_add_node_chained(tloam_b200_handle* h);
+/* loop edge (v->candidate, v->query), Z = v->T.  INVALID_ARG: v null; not v->accepted; an index outside [0, nodes);
+ * candidate == query; max_loop_edges edges already.  BAD_POSE: v->T not rigid. */
+int tloam_b200_pose_graph_add_loop(tloam_b200_handle* h, const tloam_loop_verify_result* v);
+/* either output may be null */
+int tloam_b200_pose_graph_size(tloam_b200_handle* h, size_t* nodes, size_t* loop_edges);
+/* optimises the graph as it stands, enqueued behind every earlier call, and returns once the result is home */
+int tloam_b200_pose_graph_optimize(tloam_b200_handle* h, tloam_pose_graph_result* out);
+/* nodes first .. first + count - 1 (count x 16, column-major) to out (synchronises): the last optimisation's poses, and
+ * O_k for nodes it did not cover (every node before an optimisation or after NO_LOOPS).  INVALID_ARG past the last node. */
+int tloam_b200_pose_graph_download(tloam_b200_handle* h, size_t first, size_t count, double* out);
+/* T = T_opt(N - 1) O_{N-1}^-1 of the last optimisation over N nodes (the map -> odom correction); identity before any
+ * optimisation and after NO_LOOPS (synchronises) */
+int tloam_b200_pose_graph_correction(tloam_b200_handle* h, double T[16]);
+
 /* Pinned host memory helpers (optional; pinned inputs make set_* a direct DMA, no staging threads). */
 int tloam_b200_host_alloc(void** p, size_t bytes);
 int tloam_b200_host_free(void* p);

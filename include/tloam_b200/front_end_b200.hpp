@@ -186,6 +186,25 @@ class FrontEndB200 {
     return report(tloam_b200_loop_verify(h_, lr.query, lr.candidate, guess, &out), "verifyLoop");
   }
 
+  // pose graph (include/tloam_b200.h "Pose graph"): the odometry chain and the accepted loop edges, optimised on the GPU.
+  // The global map and the odometry are left alone; correctedPoses and the map -> odom correction are the output.
+  bool enablePoseGraph(const tloam_pose_graph_config& cfg) { return report(tloam_b200_pose_graph_enable(h_, &cfg), "enablePoseGraph"); }
+  bool enablePoseGraph() {
+    tloam_pose_graph_config c;
+    tloam_b200_pose_graph_default_config(&c);
+    return enablePoseGraph(c);
+  }
+  // a node at the pose of the frame enqueued last, copied on the device; call next to every addLoopFrame
+  bool addPoseGraphNode() { return report(tloam_b200_pose_graph_add_node_chained(h_), "addPoseGraphNode"); }
+  // only an accepted verification is an edge
+  bool addLoopEdge(const tloam_loop_verify_result& v) { return report(tloam_b200_pose_graph_add_loop(h_, &v), "addLoopEdge"); }
+  bool optimizePoseGraph(tloam_pose_graph_result& out) { return report(tloam_b200_pose_graph_optimize(h_, &out), "optimizePoseGraph"); }
+  // nodes first .. first + count - 1 (count x 16, column-major); with `correction`, also T_opt(N-1) . O_{N-1}^-1
+  bool correctedPoses(size_t first, size_t count, double* poses, double* correction = nullptr) {
+    if (!report(tloam_b200_pose_graph_download(h_, first, count, poses), "correctedPoses")) return false;
+    return !correction || report(tloam_b200_pose_graph_correction(h_, correction), "correctedPoses");
+  }
+
   // processCloud + setInputSource (ref: front_end.cpp:181-199, :313): the three clouds the segmentation nodelet publishes
   bool processCloud(CloudData& ground, CloudData& edge, CloudData& general) {
     return report(tloam_b200_process_cloud(h_, &fcfg_, ground_down_sample_, edge_down_sample_, data(ground), size(ground), data(edge),

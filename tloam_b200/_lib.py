@@ -81,6 +81,21 @@ class LoopVerifyResult(C.Structure):
                 ("n_candidate_points", C.c_longlong), ("iterations", C.c_int), ("termination", C.c_int), ("accepted", C.c_int)]
 
 
+class PoseGraphConfig(C.Structure):
+    """tloam_pose_graph_config (include/tloam_b200.h "Pose graph"): the edges' sigmas and the Gauss-Newton schedule."""
+    _fields_ = [("sigma_odom_translation", C.c_double), ("sigma_odom_rotation", C.c_double),
+                ("sigma_loop_translation", C.c_double), ("sigma_loop_rotation", C.c_double), ("max_iterations", C.c_int),
+                ("eps_translation", C.c_double), ("eps_rotation", C.c_double), ("max_loop_edges", C.c_size_t),
+                ("initial_capacity_nodes", C.c_size_t)]
+
+
+class PoseGraphResult(C.Structure):
+    """tloam_pose_graph_result"""
+    _fields_ = [("nodes", C.c_longlong), ("loop_edges", C.c_longlong), ("iterations", C.c_int), ("termination", C.c_int),
+                ("initial_cost", C.c_double), ("final_cost", C.c_double), ("step_translation", C.c_double),
+                ("step_rotation", C.c_double)]
+
+
 class InnerTrace(C.Structure):
     _fields_ = [
         ("x_candidate", C.c_double * 6), ("candidate_cost", C.c_double), ("model_cost_change", C.c_double),
@@ -180,6 +195,10 @@ EXPORTS = [
     "tloam_b200_loop_add", "tloam_b200_loop_result", "tloam_b200_loop_size", "tloam_b200_loop_descriptor_download",
     "tloam_b200_loop_verify_default_config", "tloam_b200_loop_verify_enable", "tloam_b200_loop_keyframe_download",
     "tloam_b200_loop_verify", "tloam_b200_loop_verify_matches",
+    "tloam_b200_pose_graph_default_config", "tloam_b200_pose_graph_enable", "tloam_b200_pose_graph_reset",
+    "tloam_b200_pose_graph_add_node", "tloam_b200_pose_graph_add_node_chained", "tloam_b200_pose_graph_add_loop",
+    "tloam_b200_pose_graph_size", "tloam_b200_pose_graph_optimize", "tloam_b200_pose_graph_download",
+    "tloam_b200_pose_graph_correction",
 ]
 
 _lib = None
@@ -350,5 +369,16 @@ def load():
     L.tloam_b200_loop_keyframe_download.argtypes = [vp, C.c_size_t, dp, C.c_size_t, szp]
     L.tloam_b200_loop_verify.argtypes = [vp, C.c_longlong, C.c_longlong, dp, C.POINTER(LoopVerifyResult)]
     L.tloam_b200_loop_verify_matches.argtypes = [vp, C.c_int, C.POINTER(C.c_int), dp, C.c_size_t, szp]
+    L.tloam_b200_pose_graph_default_config.argtypes = [C.POINTER(PoseGraphConfig)]
+    L.tloam_b200_pose_graph_default_config.restype = None
+    L.tloam_b200_pose_graph_enable.argtypes = [vp, C.POINTER(PoseGraphConfig)]
+    L.tloam_b200_pose_graph_reset.argtypes = [vp]
+    L.tloam_b200_pose_graph_add_node.argtypes = [vp, dp]
+    L.tloam_b200_pose_graph_add_node_chained.argtypes = [vp]
+    L.tloam_b200_pose_graph_add_loop.argtypes = [vp, C.POINTER(LoopVerifyResult)]
+    L.tloam_b200_pose_graph_size.argtypes = [vp, szp, szp]
+    L.tloam_b200_pose_graph_optimize.argtypes = [vp, C.POINTER(PoseGraphResult)]
+    L.tloam_b200_pose_graph_download.argtypes = [vp, C.c_size_t, C.c_size_t, dp]
+    L.tloam_b200_pose_graph_correction.argtypes = [vp, dp]
     _lib = L
     return L

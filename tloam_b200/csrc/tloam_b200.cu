@@ -31,6 +31,7 @@
 #include "deskew.h"
 #include "scan_context.h"
 #include "loop_verify.h"
+#include "pose_graph.h"
 
 
 
@@ -244,6 +245,15 @@ struct tloam_b200_handle {
   unsigned char* d_lv_scratch = nullptr;   size_t cap_lv_scratch = 0;                           // the verification's scratch
   bool lv_ran = false;                     int lv_passes = 0;   unsigned long long lv_nq = 0;   // the last verification
   const int* lv_match_index = nullptr;    const double* lv_match_d2 = nullptr;                 // its matches, pass-major
+  // ---- pose graph (tloam_b200_pose_graph*, libtloam_b200_pg.so): the node store on the device, the loop edges on the
+  //      host until an optimisation uploads them; nothing is allocated or launched until it is enabled ----
+  bool pg_on = false;
+  tloam_pose_graph_config pg_cfg;
+  double* d_pg_O = nullptr;                size_t cap_pg = 0;   size_t pg_nodes = 0;   size_t pg_growths = 0;
+  std::vector<long long> pg_ij;            std::vector<double> pg_Z;                           // the loop edges
+  unsigned char* d_pg_scratch = nullptr;   size_t cap_pg_scratch = 0;
+  tloam_pg_state* d_pg_state = nullptr;
+  const double* d_pg_T = nullptr;          size_t pg_opt_nodes = 0;                            // the last optimisation
 };
 
 // launch bookkeeping: counts the kernel and, in profiling mode, brackets it with events
@@ -446,6 +456,7 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   cudaFree(h->d_lv_st); cudaFree(h->d_lv_pose); cudaFree(h->d_lv_pts); cudaFree(h->d_lv_off); cudaFree(h->d_lv_reg);
   cudaFree(h->d_lv_fin); cudaFree(h->d_lv_state); cudaFree(h->d_lv_scratch);
   for (auto& pr : h->lv_probes) { if (pr.ev) cudaEventDestroy(pr.ev); if (pr.h_count) cudaFreeHost(pr.h_count); }
+  cudaFree(h->d_pg_O); cudaFree(h->d_pg_scratch); cudaFree(h->d_pg_state);
   for (int i = 0; i < 2; ++i) if (h->ev_stage_free[i]) cudaEventDestroy(h->ev_stage_free[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_fit[i]) cudaEventDestroy(h->ev_fit[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_res[i]) cudaEventDestroy(h->ev_res[i]);
@@ -4248,6 +4259,257 @@ int tloam_b200_loop_verify_matches(tloam_b200_handle* h, int pass, int* index, d
   if (index) CU_TRY(cudaMemcpyAsync(index, h->lv_match_index + (size_t)pass * nq, nq * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   if (d2) CU_TRY(cudaMemcpyAsync(d2, h->lv_match_d2 + (size_t)pass * nq, nq * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Pose graph (the node store and the loop edges here; the Gauss-Newton kernels in pose_graph.cu, loaded from
+// libtloam_b200_pg.so on the first optimisation).
+// ---------------------------------------------------------------------------------------------
+struct PgLib { tloam_pg_optimize_fn optimize = nullptr; tloam_pg_chol_blocks_fn chol_blocks = nullptr; };
+static std::mutex g_pg_mu;
+static PgLib g_pg;
+
+static int pg_load(tloam_b200_handle* h, PgLib* out) {
+  std::lock_guard<std::mutex> lk(g_pg_mu);
+  if (!g_pg.optimize) {
+    const std::string path = sibling_path("libtloam_b200_pg.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    PgLib l;
+    if (so) {
+      l.optimize = reinterpret_cast<tloam_pg_optimize_fn>(dlsym(so, "tloam_pg_optimize"));
+      l.chol_blocks = reinterpret_cast<tloam_pg_chol_blocks_fn>(dlsym(so, "tloam_pg_chol_blocks"));
+    }
+    if (!l.optimize || !l.chol_blocks) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "pose graph: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_pg = l;
+  }
+  *out = g_pg;
+  return TLOAM_B200_OK;
+}
+
+static int pg_status(tloam_b200_handle* h, int e, const char* where) {
+  if (e == cudaSuccess) return TLOAM_B200_OK;
+  snprintf(h->last_error, sizeof(h->last_error), "pose graph: %s: %s", where, cudaGetErrorString((cudaError_t)e));
+  return TLOAM_B200_ERR_CUDA;
+}
+
+static bool pg_rigid(const double T[16]) {
+  Pose7 p7;
+  return pose_from_matrix(T, p7) && T[3] == 0.0 && T[7] == 0.0 && T[11] == 0.0 && T[15] == 1.0;
+}
+
+void tloam_b200_pose_graph_default_config(tloam_pose_graph_config* c) {
+  c->sigma_odom_translation = 0.02; c->sigma_odom_rotation = 0.001;
+  c->sigma_loop_translation = 0.3; c->sigma_loop_rotation = 0.002;
+  c->max_iterations = 20;
+  c->eps_translation = 1e-4; c->eps_rotation = 1e-6;
+  c->max_loop_edges = 1024;
+  c->initial_capacity_nodes = 4096;
+}
+
+int tloam_b200_pose_graph_enable(tloam_b200_handle* h, const tloam_pose_graph_config* c) {
+  if (!h || !c) return TLOAM_B200_ERR_INVALID_ARG;
+  const double v[6] = {c->sigma_odom_translation, c->sigma_odom_rotation, c->sigma_loop_translation, c->sigma_loop_rotation,
+                       c->eps_translation, c->eps_rotation};
+  for (double x : v)
+    if (!std::isfinite(x) || !(x > 0.0)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (c->max_iterations < 1 || c->max_iterations > 100 || c->max_loop_edges == 0) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  const size_t cap = c->initial_capacity_nodes ? c->initial_capacity_nodes : 1;
+  if (cap != h->cap_pg) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_pg_O); h->d_pg_O = nullptr; h->cap_pg = 0;
+    CU_TRY(cudaMalloc(&h->d_pg_O, cap * 16 * sizeof(double)));
+    h->cap_pg = cap;
+  }
+  if (!h->d_pg_state) CU_TRY(cudaMalloc(&h->d_pg_state, sizeof(tloam_pg_state)));
+  h->pg_cfg = *c;
+  h->pg_growths = 0;
+  h->pg_on = true;
+  return tloam_b200_pose_graph_reset(h);
+}
+
+int tloam_b200_pose_graph_reset(tloam_b200_handle* h) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->pg_on) return TLOAM_B200_ERR_NOT_READY;
+  h->pg_nodes = 0;
+  h->pg_ij.clear(); h->pg_Z.clear();
+  h->d_pg_T = nullptr; h->pg_opt_nodes = 0;
+  return TLOAM_B200_OK;
+}
+
+// the one place an add synchronises: the store is full and grows x1.5
+static int pg_reserve(tloam_b200_handle* h) {
+  if (h->pg_nodes < h->cap_pg) return TLOAM_B200_OK;
+  const size_t ncap = h->cap_pg + (h->cap_pg + 1) / 2;
+  double* q = nullptr;
+  CU_TRY(cudaMalloc(&q, ncap * 16 * sizeof(double)));
+  CU_TRY(cudaMemcpyAsync(q, h->d_pg_O, h->pg_nodes * 16 * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  cudaFree(h->d_pg_O);
+  h->d_pg_O = q; h->cap_pg = ncap;
+  h->pg_growths++;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_pose_graph_add_node(tloam_b200_handle* h, const double pose[16]) {
+  if (!h || !pose) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->pg_on) return TLOAM_B200_ERR_NOT_READY;
+  if (!pg_rigid(pose)) return TLOAM_B200_ERR_BAD_POSE;
+  CU_TRY(cudaSetDevice(h->device));
+  int rc = pg_reserve(h);
+  if (rc != TLOAM_B200_OK) return rc;
+  double tmp[16];
+  memcpy(tmp, pose, sizeof(tmp));
+  CU_TRY(cudaMemcpyAsync(h->d_pg_O + 16 * h->pg_nodes, tmp, sizeof(tmp), cudaMemcpyHostToDevice, h->stream));   // pageable: staged before return
+  h->pg_nodes++;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_pose_graph_add_node_chained(tloam_b200_handle* h) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->pg_on) return TLOAM_B200_ERR_NOT_READY;
+  CU_TRY(cudaSetDevice(h->device));
+  int rc = pg_reserve(h);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaMemcpyAsync(h->d_pg_O + 16 * h->pg_nodes, reinterpret_cast<const char*>(h->d_state) + offsetof(FrameState, result),
+                         16 * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
+  h->pg_nodes++;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_pose_graph_add_loop(tloam_b200_handle* h, const tloam_loop_verify_result* v) {
+  if (!h || !v) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->pg_on) return TLOAM_B200_ERR_NOT_READY;
+  if (!v->accepted || v->candidate < 0 || v->query < 0 || (size_t)v->candidate >= h->pg_nodes ||
+      (size_t)v->query >= h->pg_nodes || v->candidate == v->query || h->pg_ij.size() / 2 >= h->pg_cfg.max_loop_edges)
+    return TLOAM_B200_ERR_INVALID_ARG;
+  if (!pg_rigid(v->T)) return TLOAM_B200_ERR_BAD_POSE;
+  h->pg_ij.push_back(v->candidate); h->pg_ij.push_back(v->query);
+  h->pg_Z.insert(h->pg_Z.end(), v->T, v->T + 16);
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_pose_graph_size(tloam_b200_handle* h, size_t* nodes, size_t* loop_edges) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->pg_on) return TLOAM_B200_ERR_NOT_READY;
+  if (nodes) *nodes = h->pg_nodes;
+  if (loop_edges) *loop_edges = h->pg_ij.size() / 2;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_pose_graph_optimize(tloam_b200_handle* h, tloam_pose_graph_result* out) {
+  if (!h || !out) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->pg_on) return TLOAM_B200_ERR_NOT_READY;
+  const size_t N = h->pg_nodes, L = h->pg_ij.size() / 2;
+  memset(out, 0, sizeof(*out));
+  out->nodes = (long long)N; out->loop_edges = (long long)L;
+  h->d_pg_T = nullptr; h->pg_opt_nodes = 0;
+  if (L == 0) {
+    out->termination = TLOAM_POSE_GRAPH_NO_LOOPS;
+    return TLOAM_B200_OK;
+  }
+  PgLib lib;
+  int rc = pg_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  const tloam_pose_graph_config& c = h->pg_cfg;
+  const size_t nl = 6 * L, ncol = nl + 1, E = N - 1 + L;
+  size_t o = 0;
+  auto take = [&](size_t bytes) { const size_t at = o; o += round_up(bytes, 256); return at; };
+  const size_t o_T = take(2 * N * 16 * sizeof(double)), o_ij = take(2 * L * sizeof(long long)), o_Z = take(16 * L * sizeof(double));
+  const size_t o_edge = take(E * TLOAM_PG_EDGE * sizeof(double)), o_chain = take(N * TLOAM_PG_CHAIN * sizeof(double));
+  const size_t o_b = take(N * 6 * sizeof(double)), o_Y = take(6 * (N - 1) * ncol * sizeof(double));
+  const size_t o_S = take(nl * ncol * sizeof(double)), o_z = take(nl * sizeof(double)), o_n = take(N * 2 * sizeof(double));
+  if (o > h->cap_pg_scratch) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_pg_scratch); h->d_pg_scratch = nullptr; h->cap_pg_scratch = 0;
+    CU_TRY(cudaMalloc(&h->d_pg_scratch, o));
+    h->cap_pg_scratch = o;
+  }
+  unsigned char* base = h->d_pg_scratch;
+  tloam_pg_args a;
+  memset(&a, 0, sizeof(a));
+  a.O = h->d_pg_O;
+  a.T = reinterpret_cast<double*>(base + o_T);
+  a.loop_ij = reinterpret_cast<const long long*>(base + o_ij);
+  a.loop_Z = reinterpret_cast<const double*>(base + o_Z);
+  a.N = N; a.L = L;
+  for (int k = 0; k < 3; ++k) {
+    a.w_odom[k] = 1.0 / (c.sigma_odom_translation * c.sigma_odom_translation);
+    a.w_odom[3 + k] = 1.0 / (c.sigma_odom_rotation * c.sigma_odom_rotation);
+    a.w_loop[k] = 1.0 / (c.sigma_loop_translation * c.sigma_loop_translation);
+    a.w_loop[3 + k] = 1.0 / (c.sigma_loop_rotation * c.sigma_loop_rotation);
+  }
+  a.eps_translation = c.eps_translation; a.eps_rotation = c.eps_rotation; a.max_iterations = c.max_iterations;
+  if ((rc = pg_status(h, lib.chol_blocks(h->device, &a.chol_blocks), "occupancy")) != TLOAM_B200_OK) return rc;
+  a.state = h->d_pg_state;
+  a.edge = reinterpret_cast<double*>(base + o_edge);
+  a.chain = reinterpret_cast<double*>(base + o_chain);
+  a.b = reinterpret_cast<double*>(base + o_b);
+  a.Y = reinterpret_cast<double*>(base + o_Y);
+  a.S = reinterpret_cast<double*>(base + o_S);
+  a.z = reinterpret_cast<double*>(base + o_z);
+  a.norms = reinterpret_cast<double*>(base + o_n);
+  a.device = h->device; a.stream = h->stream;
+  // pageable sources: staged before each call returns
+  CU_TRY(cudaMemcpyAsync(base + o_ij, h->pg_ij.data(), 2 * L * sizeof(long long), cudaMemcpyHostToDevice, h->stream));
+  CU_TRY(cudaMemcpyAsync(base + o_Z, h->pg_Z.data(), 16 * L * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  CU_TRY(cudaMemcpyAsync(a.T, h->d_pg_O, N * 16 * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
+  tloam_pg_state s;
+  memset(&s, 0, sizeof(s));
+  s.term = TLOAM_POSE_GRAPH_ITERATION_LIMIT;
+  CU_TRY(cudaMemcpyAsync(h->d_pg_state, &s, sizeof(s), cudaMemcpyHostToDevice, h->stream));
+  int e = 0, launches = 0;
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.optimize(&a, &launches)));
+  h->launches += launches > 0 ? launches - 1 : 0;
+  if ((rc = pg_status(h, e, "k_pg_*")) != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaMemcpyAsync(&s, h->d_pg_state, sizeof(s), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  out->iterations = s.iter; out->termination = s.term;
+  out->initial_cost = s.initial_cost; out->final_cost = s.cost;
+  out->step_translation = s.step_t; out->step_rotation = s.step_r;
+  h->d_pg_T = a.T + 16 * N * (size_t)s.cur;
+  h->pg_opt_nodes = N;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_pose_graph_download(tloam_b200_handle* h, size_t first, size_t count, double* out) {
+  if (!h || (!out && count)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->pg_on) return TLOAM_B200_ERR_NOT_READY;
+  if (first > h->pg_nodes || count > h->pg_nodes - first) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  const size_t split = first + count < h->pg_opt_nodes ? first + count : (first > h->pg_opt_nodes ? first : h->pg_opt_nodes);
+  if (split > first)
+    CU_TRY(cudaMemcpyAsync(out, h->d_pg_T + 16 * first, (split - first) * 16 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (first + count > split)
+    CU_TRY(cudaMemcpyAsync(out + 16 * (split - first), h->d_pg_O + 16 * split, (first + count - split) * 16 * sizeof(double),
+                           cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_pose_graph_correction(tloam_b200_handle* h, double T[16]) {
+  if (!h || !T) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->pg_on) return TLOAM_B200_ERR_NOT_READY;
+  for (int k = 0; k < 16; ++k) T[k] = k % 5 == 0 ? 1.0 : 0.0;
+  if (!h->pg_opt_nodes) return TLOAM_B200_OK;
+  const size_t last = h->pg_opt_nodes - 1;
+  double A[16], O[16];
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaMemcpyAsync(A, h->d_pg_T + 16 * last, sizeof(A), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaMemcpyAsync(O, h->d_pg_O + 16 * last, sizeof(O), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  // T = A O^-1: R_A R_O^T, t_A - R_A R_O^T t_O (column-major)
+  for (int r = 0; r < 3; ++r) {
+    for (int c = 0; c < 3; ++c) T[4 * c + r] = A[r] * O[c] + A[4 + r] * O[4 + c] + A[8 + r] * O[8 + c];
+  }
+  for (int r = 0; r < 3; ++r) T[12 + r] = A[12 + r] - (T[r] * O[12] + T[4 + r] * O[13] + T[8 + r] * O[14]);
   return TLOAM_B200_OK;
 }
 

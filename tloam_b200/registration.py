@@ -139,6 +139,21 @@ class LoopVerifyResult:
     CONVERGED, ITERATION_LIMIT, FEW_INLIERS, SINGULAR, EMPTY = range(5)
 
 
+@dataclasses.dataclass(frozen=True)
+class PoseGraphResult:
+    """tloam_pose_graph_result: termination is one of PoseGraphResult.CONVERGED .. NO_LOOPS; the costs are sum r^T Omega r
+    at the odometry poses and at the returned poses; step_* are the last step's largest |upsilon| / |omega| component."""
+    nodes: int
+    loop_edges: int
+    iterations: int
+    termination: int
+    initial_cost: float
+    final_cost: float
+    step_translation: float
+    step_rotation: float
+    CONVERGED, ITERATION_LIMIT, COST_INCREASED, SINGULAR, NO_LOOPS = range(5)
+
+
 def rz(yaw):
     """the 4 x 4 rotation about z by yaw (rad); the C library's cos / sin, as the C++ shim's verifyLoop"""
     c, s = math.cos(yaw), math.sin(yaw)
@@ -869,6 +884,69 @@ class LocalRegistration:
         self._check(self._L.tloam_b200_loop_verify_matches(self._h, int(k), idx.ctypes.data_as(C.POINTER(C.c_int)), _dp(d2), n.value,
                                                            C.byref(n)), "loop_verify_matches")
         return idx, d2
+
+    # ---- pose graph (odometry and verified loop edges, Gauss-Newton; include/tloam_b200.h "Pose graph") ----
+    def pose_graph_enable(self, **overrides):
+        """start an empty pose graph; overrides: fields of tloam_pose_graph_config (sigma_odom_translation,
+        sigma_odom_rotation, sigma_loop_translation, sigma_loop_rotation, max_iterations, eps_translation, eps_rotation,
+        max_loop_edges, initial_capacity_nodes)"""
+        cfg = _lib.PoseGraphConfig()
+        self._L.tloam_b200_pose_graph_default_config(C.byref(cfg))
+        for k, v in overrides.items():
+            if not hasattr(cfg, k):
+                raise KeyError(k)
+            setattr(cfg, k, v)
+        self._check(self._L.tloam_b200_pose_graph_enable(self._h, C.byref(cfg)), "pose_graph_enable")
+
+    def pose_graph_reset(self):
+        self._check(self._L.tloam_b200_pose_graph_reset(self._h), "pose_graph_reset")
+
+    def pose_graph_add_node(self, pose=None):
+        """a node at pose (4 x 4), or, with None, at the device pose of the last enqueued frame (get_result's pose)"""
+        if pose is None:
+            self._check(self._L.tloam_b200_pose_graph_add_node_chained(self._h), "pose_graph_add_node_chained")
+            return
+        p = np.asfortranarray(np.asarray(pose, dtype=np.float64).reshape(4, 4)).ravel(order="F").copy()
+        self._check(self._L.tloam_b200_pose_graph_add_node(self._h, _dp(p)), "pose_graph_add_node")
+
+    def pose_graph_add_loop(self, v):
+        """a loop edge from an accepted LoopVerifyResult (v.candidate, v.query, Z = v.T)"""
+        r = _lib.LoopVerifyResult()
+        r.query, r.candidate = int(v.query), int(v.candidate)
+        r.T[:] = [float(x) for x in np.asarray(v.T, dtype=np.float64).reshape(4, 4).ravel(order="F")]
+        r.fitness, r.rmse, r.inliers = float(v.fitness), float(v.rmse), int(v.inliers)
+        r.n_query_points, r.n_candidate_points = int(v.n_query_points), int(v.n_candidate_points)
+        r.iterations, r.termination, r.accepted = int(v.iterations), int(v.termination), int(bool(v.accepted))
+        self._check(self._L.tloam_b200_pose_graph_add_loop(self._h, C.byref(r)), "pose_graph_add_loop")
+
+    def pose_graph_size(self):
+        """(nodes, loop edges)"""
+        n, l = C.c_size_t(0), C.c_size_t(0)
+        self._check(self._L.tloam_b200_pose_graph_size(self._h, C.byref(n), C.byref(l)), "pose_graph_size")
+        return n.value, l.value
+
+    def pose_graph_optimize(self):
+        r = _lib.PoseGraphResult()
+        self._check(self._L.tloam_b200_pose_graph_optimize(self._h, C.byref(r)), "pose_graph_optimize")
+        return PoseGraphResult(r.nodes, r.loop_edges, r.iterations, r.termination, r.initial_cost, r.final_cost,
+                               r.step_translation, r.step_rotation)
+
+    def pose_graph_poses(self, first=0, count=None):
+        """(count, 4, 4): the last optimisation's poses, the odometry poses for nodes it did not cover"""
+        n = self.pose_graph_size()[0]
+        if count is None:
+            count = n - first
+        if first < 0 or count < 0 or first + count > n:
+            raise RegistrationError(_lib.ERR_INVALID_ARG, "pose_graph_download")
+        out = np.zeros(16 * count)
+        self._check(self._L.tloam_b200_pose_graph_download(self._h, int(first), int(count), _dp(out)), "pose_graph_download")
+        return out.reshape(count, 4, 4).transpose(0, 2, 1).copy()
+
+    def pose_graph_correction(self):
+        """T_opt(N - 1) . O_{N-1}^-1 of the last optimisation (map -> odom); identity before one"""
+        out = np.zeros(16)
+        self._check(self._L.tloam_b200_pose_graph_correction(self._h, _dp(out)), "pose_graph_correction")
+        return out.reshape(4, 4).T.copy()
 
     # ---- shared map (multi-GPU) ----
     def map_blob_size(self):
