@@ -733,7 +733,7 @@ int tloam_b200_loop_verify_matches(tloam_b200_handle* h, int pass, int* index, d
 
 /* ---- Pose graph (opt-in): the back end of loop closure.  The odometry chain and the accepted loop verifications are
  * optimised together on the device; the corrected poses and the map -> odom correction come out.  The global map, the
- * keyframes and the odometry state are not touched.
+ * keyframes and the odometry state are not touched (tloam_b200_global_map_correct, below, moves the map).
  *   - Nodes.  Node k keeps the pose O_k it was added with for ever.  tloam_b200_pose_graph_add_node records a host pose;
  *     tloam_b200_pose_graph_add_node_chained records the device pose of the frame the handle enqueued last
  *     (tloam_b200_get_result's pose, the one tloam_b200_global_map_append_frame_chained reads; identity before the first
@@ -809,6 +809,44 @@ int tloam_b200_pose_graph_download(tloam_b200_handle* h, size_t first, size_t co
 /* T = T_opt(N - 1) O_{N-1}^-1 of the last optimisation over N nodes (the map -> odom correction); identity before any
  * optimisation and after NO_LOOPS (synchronises) */
 int tloam_b200_pose_graph_correction(tloam_b200_handle* h, double T[16]);
+
+/* ---- Loop-corrected global map (opt-in): every frame's block of the global map moved to its pose-graph pose.
+ *   - Tracking.  tloam_b200_global_map_correction_enable is allowed only on an empty map (right after
+ *     tloam_b200_global_map_enable or _reset; otherwise NOT_READY).  From then on every append records two poses at its
+ *     map frame f (the index tloam_b200_global_map_frame_offsets counts; a refused frame takes no slot): O_f, the frame's
+ *     odometry pose (the host pose, or for _chained appends the device pose the append reads), and P_f, the pose its block
+ *     is expressed at.  P_f = M O_f, where M is the map -> odom correction of the last tloam_b200_global_map_correct
+ *     (identity before one).  With M = I bit for bit, P_f is a copy of O_f and the map, the frame table, the intensity
+ *     channel and the registered scan are the bits of the untracked map; otherwise the append's registered scan is P_f p.
+ *     Tracking costs one extra launch per append and no synchronisation.  tloam_b200_global_map_reset empties both tables,
+ *     sets M = I and keeps tracking on; tloam_b200_global_map_enable turns tracking off.
+ *   - Correction.  node[f] is the pose-graph node map frame f moves with, or -1 for none (the mapping loop that appends
+ *     from frame 1 and adds a node from frame 0 binds map frame f to node f + 1).  Per node k:
+ *       Delta_k = T_opt(k) O_k^-1 for a node the last optimisation covered, in the operation order of
+ *                 tloam_b200_pose_graph_correction (so Delta of its last node is that call's T bit for bit);
+ *       Delta   = the map -> odom correction (tloam_b200_pose_graph_correction's T) for nodes added after it;
+ *       Delta   = I for node -1, before any optimisation and after NO_LOOPS.
+ *     C_f = Delta O_f (O_f itself when Delta is I bit for bit), so a frame bound to -1 stays at, or returns to, its
+ *     odometry pose.  A frame whose C_f equals P_f bit for bit is not touched (correcting twice from one optimisation, or
+ *     with Delta = I on a frame still at O_f, changes no bits); every point p of another frame becomes (C_f P_f^-1) p,
+ *     and P_f = C_f.  A corrected frame is its block moved rigidly, not a new down-sampling of its scan.
+ *     Then M = the map -> odom correction.
+ *   - Rounding.  Every product and sum is rounded on its own (no FMA), left to right as written, poses column-major with
+ *     R (r, c) = A[4c + r]:  A B: R = sum_c' R_A(r, c') R_B(c', c) over c' = 0, 1, 2, t = (R_A t_B, summed likewise) + t_A;
+ *     A B^-1: R(r, c) = sum_c' R_A(r, c') R_B(c, c'), t = t_A - R t_B; the bottom row of both is (0, 0, 0, 1).  A point:
+ *     x' = ((M00 x + M01 y) + M02 z) + M03.  tests/map_correct_oracle.py restates it bit for bit.
+ *   - Untouched: the frame offsets and count, the intensity channel, the registered-scan buffer, the loop keyframes, the
+ *     pose graph and the odometry.  The call synchronises.
+ *   - The kernels live in libtloam_b200_gmc.so, loaded from this library's directory by the enable call; if it is missing
+ *     the calls return ERR_CUDA (tloam_b200_last_error names the file). */
+/* NOT_READY: mapping off, or the map is not empty */
+int tloam_b200_global_map_correction_enable(tloam_b200_handle* h);
+/* NOT_READY: mapping, tracking or the pose graph off.  INVALID_ARG: n_frames is not the map's frame count, a node[f]
+ * outside [-1, nodes), or node null with frames present.  An empty map returns OK and launches nothing. */
+int tloam_b200_global_map_correct(tloam_b200_handle* h, const long long* node, size_t n_frames);
+/* O_f and P_f of frames first .. first + count - 1 (count x 16 each, column-major; either output may be null;
+ * synchronises).  NOT_READY: mapping or tracking off.  INVALID_ARG past the last frame. */
+int tloam_b200_global_map_frame_poses(tloam_b200_handle* h, size_t first, size_t count, double* odom, double* current);
 
 /* Pinned host memory helpers (optional; pinned inputs make set_* a direct DMA, no staging threads). */
 int tloam_b200_host_alloc(void** p, size_t bytes);

@@ -187,7 +187,8 @@ class FrontEndB200 {
   }
 
   // pose graph (include/tloam_b200.h "Pose graph"): the odometry chain and the accepted loop edges, optimised on the GPU.
-  // The global map and the odometry are left alone; correctedPoses and the map -> odom correction are the output.
+  // The odometry is left alone; correctedPoses and the map -> odom correction are the output, and correctGlobalMap moves
+  // the global map's frames to them.
   bool enablePoseGraph(const tloam_pose_graph_config& cfg) { return report(tloam_b200_pose_graph_enable(h_, &cfg), "enablePoseGraph"); }
   bool enablePoseGraph() {
     tloam_pose_graph_config c;
@@ -203,6 +204,22 @@ class FrontEndB200 {
   bool correctedPoses(size_t first, size_t count, double* poses, double* correction = nullptr) {
     if (!report(tloam_b200_pose_graph_download(h_, first, count, poses), "correctedPoses")) return false;
     return !correction || report(tloam_b200_pose_graph_correction(h_, correction), "correctedPoses");
+  }
+
+  // loop-corrected global map (include/tloam_b200.h "Loop-corrected global map"): call right after enableGlobalMap (an
+  // empty map); every later updateGlobalMap records the frame's odometry pose and the pose its block is expressed at
+  bool enableGlobalMapCorrection() {
+    return report(tloam_b200_global_map_correction_enable(h_), "enableGlobalMapCorrection");
+  }
+  // moves every map frame f to Delta_{node[f]} . O_f of the last optimizePoseGraph (node[f] = -1: left alone); with
+  // updateGlobalMap from the second frame and addPoseGraphNode from the first, node[f] = f + 1.  Later frames are
+  // appended at the map -> odom correction times their odometry pose.
+  bool correctGlobalMap(const std::vector<long long>& node) {
+    return report(tloam_b200_global_map_correct(h_, node.empty() ? nullptr : node.data(), node.size()), "correctGlobalMap");
+  }
+  // O_f and P_f of map frames first .. first + count - 1 (count x 16 each, column-major; either may be null)
+  bool globalMapFramePoses(size_t first, size_t count, double* odom, double* current) {
+    return report(tloam_b200_global_map_frame_poses(h_, first, count, odom, current), "globalMapFramePoses");
   }
 
   // processCloud + setInputSource (ref: front_end.cpp:181-199, :313): the three clouds the segmentation nodelet publishes

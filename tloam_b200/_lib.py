@@ -199,6 +199,7 @@ EXPORTS = [
     "tloam_b200_pose_graph_add_node", "tloam_b200_pose_graph_add_node_chained", "tloam_b200_pose_graph_add_loop",
     "tloam_b200_pose_graph_size", "tloam_b200_pose_graph_optimize", "tloam_b200_pose_graph_download",
     "tloam_b200_pose_graph_correction",
+    "tloam_b200_global_map_correction_enable", "tloam_b200_global_map_correct", "tloam_b200_global_map_frame_poses",
 ]
 
 _lib = None
@@ -380,5 +381,8 @@ def load():
     L.tloam_b200_pose_graph_optimize.argtypes = [vp, C.POINTER(PoseGraphResult)]
     L.tloam_b200_pose_graph_download.argtypes = [vp, C.c_size_t, C.c_size_t, dp]
     L.tloam_b200_pose_graph_correction.argtypes = [vp, dp]
+    L.tloam_b200_global_map_correction_enable.argtypes = [vp]
+    L.tloam_b200_global_map_correct.argtypes = [vp, C.POINTER(C.c_longlong), C.c_size_t]
+    L.tloam_b200_global_map_frame_poses.argtypes = [vp, C.c_size_t, C.c_size_t, dp, dp]
     _lib = L
     return L

@@ -32,6 +32,7 @@
 #include "scan_context.h"
 #include "loop_verify.h"
 #include "pose_graph.h"
+#include "map_correct.h"
 
 
 
@@ -209,6 +210,12 @@ struct tloam_b200_handle {
   size_t gmap_growths = 0;
   struct GMapProbe { cudaEvent_t ev = nullptr; unsigned long long* h_count = nullptr; unsigned long long cum = 0; bool pending = false; };
   GMapProbe gmap_probes[4];                int gmap_probe_next = 0;
+  // ---- the map's pose tables (tloam_b200_global_map_correction*, libtloam_b200_gmc.so): O_f and P_f of every frame, with
+  //      the capacity of the frame table; M, the pose later appends are expressed in (map <- odom), and whether it is I ----
+  bool gmc_on = false;
+  double* d_gmc_O = nullptr;               double* d_gmc_P = nullptr;   size_t cap_gmc = 0;
+  double gmc_M[16];                        bool gmc_M_identity = true;
+  unsigned char* d_gmc_scratch = nullptr;  size_t cap_gmc_scratch = 0;                         // node table, M_f, moved
   // ---- the map's intensity channel (tloam_b200_global_map_*intensity*, libtloam_b200_gmi.so): allocated on the first
   //      intensity append; d_gmi_map has the capacity of d_gmap ----
   bool gmi_used = false;                   // an intensity frame was appended since enable / reset
@@ -457,6 +464,7 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   cudaFree(h->d_lv_fin); cudaFree(h->d_lv_state); cudaFree(h->d_lv_scratch);
   for (auto& pr : h->lv_probes) { if (pr.ev) cudaEventDestroy(pr.ev); if (pr.h_count) cudaFreeHost(pr.h_count); }
   cudaFree(h->d_pg_O); cudaFree(h->d_pg_scratch); cudaFree(h->d_pg_state);
+  cudaFree(h->d_gmc_O); cudaFree(h->d_gmc_P); cudaFree(h->d_gmc_scratch);
   for (int i = 0; i < 2; ++i) if (h->ev_stage_free[i]) cudaEventDestroy(h->ev_stage_free[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_fit[i]) cudaEventDestroy(h->ev_fit[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_res[i]) cudaEventDestroy(h->ev_res[i]);
@@ -3342,6 +3350,8 @@ static int gmap_clear(tloam_b200_handle* h) {
   for (auto& pr : h->gmap_probes) pr.pending = false;
   h->gmap_reg_valid = false; h->gmap_reg_n = 0;
   h->gmi_used = false;                     // re-arms the intensity channel (the next intensity frame starts it afresh)
+  for (int k = 0; k < 16; ++k) h->gmc_M[k] = k % 5 == 0 ? 1.0 : 0.0;
+  h->gmc_M_identity = true;                // the pose tables are empty with the frame table; tracking stays as it is
   return TLOAM_B200_OK;
 }
 
@@ -3371,6 +3381,7 @@ int tloam_b200_global_map_enable(tloam_b200_handle* h, const tloam_global_map_co
   h->gmap_voxel = cfg->voxel;
   h->gmap_growths = 0;
   h->gmap_on = true;
+  h->gmc_on = false;
   return gmap_clear(h);
 }
 
@@ -3417,6 +3428,17 @@ static int gmap_grow(tloam_b200_handle* h, size_t n) {
     CU_TRY(cudaStreamSynchronize(h->stream));
     cudaFree(h->d_gmap_off);
     h->d_gmap_off = q; h->cap_gmap_off = ncap;
+    if (h->gmc_on) {                       // the pose tables grow with the frame table
+      for (double** t : {&h->d_gmc_O, &h->d_gmc_P}) {
+        double* qt = nullptr;
+        CU_TRY(cudaMalloc(&qt, ncap * 16 * sizeof(double)));
+        if (st.frames) CU_TRY(cudaMemcpyAsync(qt, *t, st.frames * 16 * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
+        CU_TRY(cudaStreamSynchronize(h->stream));
+        cudaFree(*t);
+        *t = qt;
+      }
+      h->cap_gmc = ncap;
+    }
   }
   h->gmap_growths++;
   return TLOAM_B200_OK;
@@ -3455,6 +3477,41 @@ static int gmi_load(tloam_b200_handle* h, GmiLib* out) {
 static int gmi_status(tloam_b200_handle* h, int e, const char* where) {
   if (e == cudaSuccess) return TLOAM_B200_OK;
   snprintf(h->last_error, sizeof(h->last_error), "global map intensity: %s: %s", where, cudaGetErrorString((cudaError_t)e));
+  return TLOAM_B200_ERR_CUDA;
+}
+
+// ---- the pose tables' and the correction's kernels live in libtloam_b200_gmc.so (map_correct.cu), next to this library:
+//      loaded by tloam_b200_global_map_correction_enable, so that the kernels of this library keep their SASS and an append
+//      with tracking on cannot meet a missing library ----
+struct GmcLib { tloam_gmc_pose_fn pose = nullptr; tloam_gmc_correct_fn correct = nullptr; };
+static std::mutex g_gmc_mu;
+static GmcLib g_gmc;
+
+static int gmc_load(tloam_b200_handle* h, GmcLib* out) {
+  std::lock_guard<std::mutex> lk(g_gmc_mu);
+  if (!g_gmc.pose) {
+    const std::string path = sibling_path("libtloam_b200_gmc.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    GmcLib l;
+    if (so) {
+      l.pose = reinterpret_cast<tloam_gmc_pose_fn>(dlsym(so, "tloam_gmc_pose"));
+      l.correct = reinterpret_cast<tloam_gmc_correct_fn>(dlsym(so, "tloam_gmc_correct"));
+    }
+    if (!l.pose || !l.correct) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "global map correction: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_gmc = l;
+  }
+  *out = g_gmc;
+  return TLOAM_B200_OK;
+}
+
+static int gmc_status(tloam_b200_handle* h, int e, const char* where) {
+  if (e == cudaSuccess) return TLOAM_B200_OK;
+  snprintf(h->last_error, sizeof(h->last_error), "global map correction: %s: %s", where, cudaGetErrorString((cudaError_t)e));
   return TLOAM_B200_ERR_CUDA;
 }
 
@@ -3512,6 +3569,17 @@ static int gmap_append_impl(tloam_b200_handle* h, const double* pose_host, const
     d_pose = reinterpret_cast<const double*>(reinterpret_cast<const char*>(h->d_state) + offsetof(FrameState, result));
   }
   GMapState* st = h->d_gmap_st;
+  if (h->gmc_on) {                         // O_f, P_f = M O_f recorded at the frame's slot; the transform reads P_f
+    GmcLib gmc;
+    if ((rc = gmc_load(h, &gmc)) != TLOAM_B200_OK) return rc;
+    tloam_gmc_mat M;
+    memcpy(M.m, h->gmc_M, sizeof(M.m));
+    int e = 0;
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = gmc.pose(d_pose, h->d_gmap_pose, h->d_gmc_O, h->d_gmc_P, &st->frames, h->cap_gmc,
+                                                 h->gmc_M_identity ? nullptr : &M, h->device, h->stream)));
+    if ((rc = gmc_status(h, e, "k_gmc_pose")) != TLOAM_B200_OK) return rc;
+    d_pose = h->d_gmap_pose;
+  }
   CU_TRY(cudaMemsetAsync(&st->n_fin, 0, sizeof(GMapState) - offsetof(GMapState, n_fin), h->stream));
   const unsigned tb = 256, gb = (unsigned)((n + tb - 1) / tb);
   if (n) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_transform<<<gb, tb, 0, h->stream>>>(d_in, (unsigned)n, d_pose, h->d_gmap_reg, h->d_gmap_fin, st)));
@@ -4510,6 +4578,104 @@ int tloam_b200_pose_graph_correction(tloam_b200_handle* h, double T[16]) {
     for (int c = 0; c < 3; ++c) T[4 * c + r] = A[r] * O[c] + A[4 + r] * O[4 + c] + A[8 + r] * O[8 + c];
   }
   for (int r = 0; r < 3; ++r) T[12 + r] = A[12 + r] - (T[r] * O[12] + T[4 + r] * O[13] + T[8 + r] * O[14]);
+  return TLOAM_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Loop-corrected global map (the pose tables here and in gmap_append_impl; the kernels in map_correct.cu, loaded from
+// libtloam_b200_gmc.so when tracking is enabled).
+// ---------------------------------------------------------------------------------------------
+int tloam_b200_global_map_correction_enable(tloam_b200_handle* h) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on || h->gmap_calls != 0) return TLOAM_B200_ERR_NOT_READY;
+  GmcLib lib;
+  int rc = gmc_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  if (h->cap_gmc != h->cap_gmap_off) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_gmc_O); cudaFree(h->d_gmc_P); h->d_gmc_O = h->d_gmc_P = nullptr; h->cap_gmc = 0;
+    CU_TRY(cudaMalloc(&h->d_gmc_O, h->cap_gmap_off * 16 * sizeof(double)));
+    CU_TRY(cudaMalloc(&h->d_gmc_P, h->cap_gmap_off * 16 * sizeof(double)));
+    h->cap_gmc = h->cap_gmap_off;
+  }
+  h->gmc_on = true;
+  return TLOAM_B200_OK;
+}
+
+// the map's exact size, without touching its sticky flags (the next size / download call still reports them)
+static int gmc_read(tloam_b200_handle* h, GMapState* st) {
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaMemcpyAsync(st, h->d_gmap_st, sizeof(*st), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_global_map_correct(tloam_b200_handle* h, const long long* node, size_t n_frames) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on || !h->gmc_on || !h->pg_on) return TLOAM_B200_ERR_NOT_READY;
+  GmcLib lib;
+  int rc = gmc_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  GMapState st;
+  if ((rc = gmc_read(h, &st)) != TLOAM_B200_OK) return rc;
+  if (n_frames != st.frames || (!node && n_frames)) return TLOAM_B200_ERR_INVALID_ARG;
+  for (size_t f = 0; f < n_frames; ++f)
+    if (node[f] < -1 || (node[f] >= 0 && (size_t)node[f] >= h->pg_nodes)) return TLOAM_B200_ERR_INVALID_ARG;
+  double D[16];
+  if ((rc = tloam_b200_pose_graph_correction(h, D)) != TLOAM_B200_OK) return rc;
+  bool ident = true;                       // bit for bit: M = I keeps the appends' copy path
+  for (int k = 0; k < 16; ++k) {
+    const double e = k % 5 == 0 ? 1.0 : 0.0;
+    ident &= memcmp(&D[k], &e, sizeof(double)) == 0;
+  }
+  if (n_frames) {
+    size_t o = 0;
+    auto take = [&](size_t bytes) { const size_t at = o; o += round_up(bytes, 256); return at; };
+    const size_t o_node = take(n_frames * sizeof(long long)), o_M = take(n_frames * 16 * sizeof(double));
+    const size_t o_moved = take(n_frames * sizeof(unsigned));
+    if (o > h->cap_gmc_scratch) {
+      cudaFree(h->d_gmc_scratch); h->d_gmc_scratch = nullptr; h->cap_gmc_scratch = 0;
+      CU_TRY(cudaMalloc(&h->d_gmc_scratch, o + o / 2));
+      h->cap_gmc_scratch = o + o / 2;
+    }
+    unsigned char* base = h->d_gmc_scratch;
+    tloam_gmc_args a;
+    memset(&a, 0, sizeof(a));
+    a.node = reinterpret_cast<const long long*>(base + o_node);
+    a.node_O = h->d_pg_O; a.node_T = h->d_pg_T; a.n_opt = h->pg_opt_nodes;
+    memcpy(a.delta_new.m, D, sizeof(D));
+    a.O = h->d_gmc_O; a.P = h->d_gmc_P;
+    a.M = reinterpret_cast<double*>(base + o_M);
+    a.moved = reinterpret_cast<unsigned*>(base + o_moved);
+    a.frames = st.frames; a.points = st.count;
+    a.offsets = h->d_gmap_off; a.map = h->d_gmap;
+    a.device = h->device; a.stream = h->stream;
+    // pageable source: staged before the call returns
+    CU_TRY(cudaMemcpyAsync(base + o_node, node, n_frames * sizeof(long long), cudaMemcpyHostToDevice, h->stream));
+    int e = 0, launches = 0;
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.correct(&a, &launches)));
+    h->launches += launches > 0 ? launches - 1 : 0;
+    if ((rc = gmc_status(h, e, "k_gmc_*")) != TLOAM_B200_OK) return rc;
+    CU_TRY(cudaStreamSynchronize(h->stream));
+  }
+  memcpy(h->gmc_M, D, sizeof(D));
+  h->gmc_M_identity = ident;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_global_map_frame_poses(tloam_b200_handle* h, size_t first, size_t count, double* odom, double* current) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on || !h->gmc_on) return TLOAM_B200_ERR_NOT_READY;
+  GMapState st;
+  int rc = gmc_read(h, &st);
+  if (rc != TLOAM_B200_OK) return rc;
+  if (first > st.frames || count > st.frames - first) return TLOAM_B200_ERR_INVALID_ARG;
+  if (count && odom)
+    CU_TRY(cudaMemcpyAsync(odom, h->d_gmc_O + 16 * first, count * 16 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (count && current)
+    CU_TRY(cudaMemcpyAsync(current, h->d_gmc_P + 16 * first, count * 16 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
   return TLOAM_B200_OK;
 }
 

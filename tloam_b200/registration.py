@@ -948,6 +948,29 @@ class LocalRegistration:
         self._check(self._L.tloam_b200_pose_graph_correction(self._h, _dp(out)), "pose_graph_correction")
         return out.reshape(4, 4).T.copy()
 
+    # ---- loop-corrected global map (include/tloam_b200.h "Loop-corrected global map") ----
+    def global_map_correction_enable(self):
+        """record every later append's odometry and current pose (only on an empty map)"""
+        self._check(self._L.tloam_b200_global_map_correction_enable(self._h), "global_map_correction_enable")
+
+    def global_map_correct(self, nodes):
+        """move every map frame f to Delta_{nodes[f]} O_f of the last pose-graph optimisation (nodes[f] = -1: leave it);
+        len(nodes) must be the map's frame count"""
+        n = np.ascontiguousarray(np.asarray(nodes, dtype=np.int64).reshape(-1))
+        p = n.ctypes.data_as(C.POINTER(C.c_longlong)) if n.size else None
+        self._check(self._L.tloam_b200_global_map_correct(self._h, p, n.size), "global_map_correct")
+
+    def global_map_frame_poses(self, first=0, count=None):
+        """(odometry poses, current poses) of map frames [first, first + count), each (count, 4, 4)"""
+        if count is None:
+            count = self.global_map_size()[1] - first
+        if first < 0 or count < 0:
+            raise RegistrationError(_lib.ERR_INVALID_ARG, "global_map_frame_poses")
+        o, c = np.zeros(16 * count), np.zeros(16 * count)
+        self._check(self._L.tloam_b200_global_map_frame_poses(self._h, int(first), int(count), _dp(o), _dp(c)),
+                    "global_map_frame_poses")
+        return tuple(x.reshape(count, 4, 4).transpose(0, 2, 1).copy() for x in (o, c))
+
     # ---- shared map (multi-GPU) ----
     def map_blob_size(self):
         n = C.c_size_t(0)
