@@ -810,6 +810,66 @@ int tloam_b200_pose_graph_download(tloam_b200_handle* h, size_t first, size_t co
  * optimisation and after NO_LOOPS (synchronises) */
 int tloam_b200_pose_graph_correction(tloam_b200_handle* h, double T[16]);
 
+/* ---- Robust pose graph: graduated non-convexity (GNC) with a truncated-least-squares (TLS) cost over the loop edges, so
+ * that a loop edge that passed verification but closes the wrong place (perceptual aliasing) is rejected instead of bending
+ * the trajectory.  It optimises the graph tloam_b200_pose_graph_* built, with that graph's configuration.
+ *   - Residual.  Loop edge l has the unweighted squared Mahalanobis residual rho_l = r_l^T Omega_loop r_l, r as above.
+ *     Odometry edges are never robustified: they are consecutive scan matches, not place recognition.
+ *   - Weights w_l in [0, 1]: cost = sum_odom r^T Omega r + sum_loop w_l r^T Omega r, and its Hessian and gradient alike
+ *     (loop edge l's rows are scaled by sqrt(w_l)).
+ *   - TLS rule (T-LOAM's updateWeight) with c2 = chi2_threshold, th1 = (mu + 1) / mu c2, th2 = mu / (mu + 1) c2:
+ *     w = 1 at rho = 0; w = 0 at rho >= th1; w = 1 at rho <= th2; otherwise w = sqrt(c2 mu (mu + 1) / rho) - mu.
+ *   - Schedule.  Every run starts from the odometry poses.
+ *       1. Stage 0: all weights 1, the Gauss-Newton schedule of tloam_b200_pose_graph_optimize (max_iterations, the same
+ *          accept / revert / converge rules) from the odometry poses; exactly what that call computes.
+ *       2. max rho <= c2 at the accepted poses: stop, ALL_INLIERS (the result is stage 0's).
+ *       3. mu_0 = c2 / (2 max rho - c2) (<= 0: 1e-10).
+ *       4. Outer step: the weights from rho at the current poses; then up to inner_iterations weighted Gauss-Newton steps
+ *          from the current poses with the weights fixed (each stage evaluates its start cost under its own weights, and
+ *          the accept rule compares weighted costs); then mu <- gnc_factor mu.
+ *       5. An update that leaves every weight exactly 0 or 1 is followed by one last stage of up to max_iterations steps at
+ *          those weights: CONVERGED.  Otherwise the run stops after max_outer_iterations outer steps: OUTER_LIMIT.  A
+ *          singular solve anywhere stops the run: SINGULAR.  No loop edge: NO_LOOPS, nothing is launched.
+ *     A stage that ends in COST_INCREASED (its last step reverted) or its own convergence does not stop the run.
+ *   - The robust run is the last optimisation: tloam_b200_pose_graph_download, _correction and
+ *     tloam_b200_global_map_correct read its poses.  tloam_b200_pose_graph_loop_weights reads its weights.
+ *   - Every reduction runs in a fixed order: a run is bit-reproducible.  The outer loop runs on the host, reading a few
+ *     bytes of device state after every stage.  The residual and weight kernels live in libtloam_b200_pgr.so, loaded from
+ *     this library's directory on the first robust optimisation (missing: ERR_CUDA, tloam_b200_last_error names it). */
+typedef struct tloam_pose_graph_robust_config {
+  double chi2_threshold;               /* c2, on rho (a squared Mahalanobis distance, 6 degrees of freedom) */
+  double gnc_factor;                   /* mu grows by this factor per outer step, > 1 */
+  int inner_iterations;                /* Gauss-Newton steps per outer step, 1 .. 100 */
+  int max_outer_iterations;            /* 1 .. 1000 */
+} tloam_pose_graph_robust_config;
+enum {
+  TLOAM_POSE_GRAPH_GNC_CONVERGED = 0,
+  TLOAM_POSE_GRAPH_GNC_OUTER_LIMIT = 1,
+  TLOAM_POSE_GRAPH_GNC_ALL_INLIERS = 2,
+  TLOAM_POSE_GRAPH_GNC_SINGULAR = 3,
+  TLOAM_POSE_GRAPH_GNC_NO_LOOPS = 4
+};
+typedef struct tloam_pose_graph_robust_result {
+  tloam_pose_graph_result pg;          /* iterations: accepted steps over all stages; termination: the last stage's;
+                                          initial_cost: stage 0's (unit weights); final_cost: the last stage's, weighted */
+  int outer_iterations;                /* weight updates */
+  int gnc_termination;                 /* TLOAM_POSE_GRAPH_GNC_* */
+  double mu_final;                     /* the mu of the last weight update (0 when there was none) */
+  long long inliers;                   /* loop edges with w == 1 */
+  long long rejected;                  /* loop edges with w == 0 */
+} tloam_pose_graph_robust_result;
+/* chi2_threshold 16.81 (the chi-square 99 % quantile at 6 degrees of freedom), gnc_factor 1.4 (the TLS default of Yang et
+ * al., RA-L 2020), inner_iterations 2, max_outer_iterations 100 */
+void tloam_b200_pose_graph_robust_default_config(tloam_pose_graph_robust_config* c);
+/* optimises the graph as it stands (returns once the result is home).  NOT_READY: the pose graph off.  INVALID_ARG: a null
+ * argument; chi2_threshold not finite or not > 0; gnc_factor not finite or <= 1; inner_iterations outside [1, 100];
+ * max_outer_iterations outside [1, 1000]. */
+int tloam_b200_pose_graph_optimize_robust(tloam_b200_handle* h, const tloam_pose_graph_robust_config* cfg,
+                                          tloam_pose_graph_robust_result* out);
+/* loop edges first .. first + count - 1: the last optimisation's weights (1.0 for every edge after a plain optimisation,
+ * before any, after NO_LOOPS, and for edges added after it).  Synchronises.  INVALID_ARG past the last edge. */
+int tloam_b200_pose_graph_loop_weights(tloam_b200_handle* h, size_t first, size_t count, double* w);
+
 /* ---- Loop-corrected global map (opt-in): every frame's block of the global map moved to its pose-graph pose.
  *   - Tracking.  tloam_b200_global_map_correction_enable is allowed only on an empty map (right after
  *     tloam_b200_global_map_enable or _reset; otherwise NOT_READY).  From then on every append records two poses at its

@@ -200,6 +200,21 @@ class FrontEndB200 {
   // only an accepted verification is an edge
   bool addLoopEdge(const tloam_loop_verify_result& v) { return report(tloam_b200_pose_graph_add_loop(h_, &v), "addLoopEdge"); }
   bool optimizePoseGraph(tloam_pose_graph_result& out) { return report(tloam_b200_pose_graph_optimize(h_, &out), "optimizePoseGraph"); }
+  // graduated non-convexity with a truncated-least-squares cost over the loop edges (include/tloam_b200.h "Robust pose
+  // graph"): a loop edge that verification accepted at the wrong place ends with weight 0; correctedPoses and
+  // correctGlobalMap then read this run
+  bool optimizePoseGraphRobust(const tloam_pose_graph_robust_config& cfg, tloam_pose_graph_robust_result& out) {
+    return report(tloam_b200_pose_graph_optimize_robust(h_, &cfg, &out), "optimizePoseGraphRobust");
+  }
+  bool optimizePoseGraphRobust(tloam_pose_graph_robust_result& out) {
+    tloam_pose_graph_robust_config c;
+    tloam_b200_pose_graph_robust_default_config(&c);
+    return optimizePoseGraphRobust(c, out);
+  }
+  // the last optimisation's weights of loop edges first .. first + count - 1 (1 after optimizePoseGraph)
+  bool loopEdgeWeights(size_t first, size_t count, double* w) {
+    return report(tloam_b200_pose_graph_loop_weights(h_, first, count, w), "loopEdgeWeights");
+  }
   // nodes first .. first + count - 1 (count x 16, column-major); with `correction`, also T_opt(N-1) . O_{N-1}^-1
   bool correctedPoses(size_t first, size_t count, double* poses, double* correction = nullptr) {
     if (!report(tloam_b200_pose_graph_download(h_, first, count, poses), "correctedPoses")) return false;

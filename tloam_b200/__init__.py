@@ -5,4 +5,5 @@ include/tloam_b200.h).  This package is only the Python host-side mirror of the 
 synthetic-scene generator used by tests and bench.py.  Importing it never touches oracle/.
 """
 from .registration import (BatchRegistration, Frame, LocalRegistration, LoopResult, LoopVerifyResult,  # noqa: F401
-                           PoseGraphResult, RegistrationError, default_config, packed_scan, packed_time)
+                           PoseGraphResult, PoseGraphRobustResult, RegistrationError, default_config, packed_scan,
+                           packed_time)

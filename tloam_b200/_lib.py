@@ -96,6 +96,18 @@ class PoseGraphResult(C.Structure):
                 ("step_rotation", C.c_double)]
 
 
+class PoseGraphRobustConfig(C.Structure):
+    """tloam_pose_graph_robust_config (include/tloam_b200.h "Robust pose graph"): the TLS threshold and the GNC schedule."""
+    _fields_ = [("chi2_threshold", C.c_double), ("gnc_factor", C.c_double), ("inner_iterations", C.c_int),
+                ("max_outer_iterations", C.c_int)]
+
+
+class PoseGraphRobustResult(C.Structure):
+    """tloam_pose_graph_robust_result"""
+    _fields_ = [("pg", PoseGraphResult), ("outer_iterations", C.c_int), ("gnc_termination", C.c_int),
+                ("mu_final", C.c_double), ("inliers", C.c_longlong), ("rejected", C.c_longlong)]
+
+
 class InnerTrace(C.Structure):
     _fields_ = [
         ("x_candidate", C.c_double * 6), ("candidate_cost", C.c_double), ("model_cost_change", C.c_double),
@@ -198,7 +210,8 @@ EXPORTS = [
     "tloam_b200_pose_graph_default_config", "tloam_b200_pose_graph_enable", "tloam_b200_pose_graph_reset",
     "tloam_b200_pose_graph_add_node", "tloam_b200_pose_graph_add_node_chained", "tloam_b200_pose_graph_add_loop",
     "tloam_b200_pose_graph_size", "tloam_b200_pose_graph_optimize", "tloam_b200_pose_graph_download",
-    "tloam_b200_pose_graph_correction",
+    "tloam_b200_pose_graph_correction", "tloam_b200_pose_graph_robust_default_config",
+    "tloam_b200_pose_graph_optimize_robust", "tloam_b200_pose_graph_loop_weights",
     "tloam_b200_global_map_correction_enable", "tloam_b200_global_map_correct", "tloam_b200_global_map_frame_poses",
 ]
 
@@ -381,6 +394,10 @@ def load():
     L.tloam_b200_pose_graph_optimize.argtypes = [vp, C.POINTER(PoseGraphResult)]
     L.tloam_b200_pose_graph_download.argtypes = [vp, C.c_size_t, C.c_size_t, dp]
     L.tloam_b200_pose_graph_correction.argtypes = [vp, dp]
+    L.tloam_b200_pose_graph_robust_default_config.argtypes = [C.POINTER(PoseGraphRobustConfig)]
+    L.tloam_b200_pose_graph_robust_default_config.restype = None
+    L.tloam_b200_pose_graph_optimize_robust.argtypes = [vp, C.POINTER(PoseGraphRobustConfig), C.POINTER(PoseGraphRobustResult)]
+    L.tloam_b200_pose_graph_loop_weights.argtypes = [vp, C.c_size_t, C.c_size_t, dp]
     L.tloam_b200_global_map_correction_enable.argtypes = [vp]
     L.tloam_b200_global_map_correct.argtypes = [vp, C.POINTER(C.c_longlong), C.c_size_t]
     L.tloam_b200_global_map_frame_poses.argtypes = [vp, C.c_size_t, C.c_size_t, dp, dp]

@@ -13,6 +13,7 @@
 #include <math.h>
 
 #include "ldlt6.cuh"
+#include "pose_graph.cuh"
 #include "pose_graph.h"
 #include "se3.cuh"
 
@@ -23,23 +24,11 @@ namespace tloam {
 enum { kPgConverged = 0, kPgIterationLimit = 1, kPgCostIncreased = 2, kPgSingular = 3 };
 constexpr unsigned kPgT = 256;
 
-#define PGM(m, r, c) (m)[4 * (c) + (r)]
-
-// C = A^-1 B of rigid column-major 4 x 4 matrices: R_A^T R_B, R_A^T (t_B - t_A)
-__device__ void pg_inv_mul(const double* A, const double* B, double* C) {
-  for (int r = 0; r < 3; ++r) {
-    for (int c = 0; c < 3; ++c) PGM(C, r, c) = PGM(A, 0, r) * PGM(B, 0, c) + PGM(A, 1, r) * PGM(B, 1, c) + PGM(A, 2, r) * PGM(B, 2, c);
-    PGM(C, r, 3) = PGM(A, 0, r) * (PGM(B, 0, 3) - PGM(A, 0, 3)) + PGM(A, 1, r) * (PGM(B, 1, 3) - PGM(A, 1, 3)) +
-                   PGM(A, 2, r) * (PGM(B, 2, 3) - PGM(A, 2, 3));
-    PGM(C, 3, r) = 0.0;
-  }
-  PGM(C, 3, 3) = 1.0;
-}
-
 __device__ __forceinline__ const double* pg_T(const tloam_pg_args& a, int buf) { return a.T + 16ull * a.N * (unsigned)buf; }
 
 // one thread per edge (odometry edges first): r = log(Z^-1 T_i^-1 T_j), A = Ad(T_j^-1), r^T Omega r.  candidate: read the
-// round's candidate poses T[cur ^ 1], else T[cur]
+// round's candidate poses T[cur ^ 1], else T[cur].  With loop_w, loop edge l stores sqrt(w_l) A and sqrt(w_l) r, so every
+// later kernel solves the weighted system and the cost term is w_l r^T Omega r
 __global__ void __launch_bounds__(kPgT) k_pg_linearize(tloam_pg_args a, int candidate) {
   const tloam_pg_state* s = a.state;
   if (candidate && s->done) return;
@@ -81,6 +70,11 @@ __global__ void __launch_bounds__(kPgT) k_pg_linearize(tloam_pg_args a, int cand
       out[6 * (u + 3) + v] = 0.0;
       out[6 * (u + 3) + v + 3] = R[3 * u + v];
     }
+  if (a.loop_w && e >= no) {
+    const double sw = sqrt(a.loop_w[e - no]);
+    for (int k = 0; k < 36; ++k) out[k] *= sw;
+    for (int k = 0; k < 6; ++k) r[k] *= sw;
+  }
   double c = 0.0;
   for (int k = 0; k < 6; ++k) {
     out[36 + k] = r[k];

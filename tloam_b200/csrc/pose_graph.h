@@ -27,12 +27,13 @@ typedef struct tloam_pg_args {
   double* T;                          // 2 x N poses, column-major 4 x 4 (buffer b at T + 16 N b)
   const long long* loop_ij;           // L x (candidate i, query j)
   const double* loop_Z;               // L x 16: Z = T_i^-1 T_j measured, column-major
+  const double* loop_w;               // L: the loop edges' weights in [0, 1], read by k_pg_linearize only; null: all 1
   unsigned long long N, L;
   double w_odom[6], w_loop[6];        // the diagonals of Omega_odom and Omega_loop, (upsilon, omega) order
   double eps_translation, eps_rotation;
   int max_iterations;
   unsigned chol_blocks;               // k_pg_dense_chol's cooperative grid
-  tloam_pg_state* state;              // initialised by the caller: T[0] = O, cur 0, the rest 0
+  tloam_pg_state* state;              // initialised by the caller: T[cur] = the start poses (O for a plain run), the rest 0
   double* edge;                       // (N - 1 + L) x TLOAM_PG_EDGE; odometry edge k - 1 is (k - 1, k)
   double* chain;                      // N x TLOAM_PG_CHAIN (slot 0 unused)
   double* b;                          // N x 6: -g (slot 0 unused)

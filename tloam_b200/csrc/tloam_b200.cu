@@ -32,6 +32,7 @@
 #include "scan_context.h"
 #include "loop_verify.h"
 #include "pose_graph.h"
+#include "pose_graph_robust.h"
 #include "map_correct.h"
 
 
@@ -261,6 +262,7 @@ struct tloam_b200_handle {
   unsigned char* d_pg_scratch = nullptr;   size_t cap_pg_scratch = 0;
   tloam_pg_state* d_pg_state = nullptr;
   const double* d_pg_T = nullptr;          size_t pg_opt_nodes = 0;                            // the last optimisation
+  const double* d_pgr_w = nullptr;         size_t pgr_w_edges = 0;                             // its loop weights (robust)
 };
 
 // launch bookkeeping: counts the kernel and, in profiling mode, brackets it with events
@@ -4408,6 +4410,7 @@ int tloam_b200_pose_graph_reset(tloam_b200_handle* h) {
   h->pg_nodes = 0;
   h->pg_ij.clear(); h->pg_Z.clear();
   h->d_pg_T = nullptr; h->pg_opt_nodes = 0;
+  h->d_pgr_w = nullptr; h->pgr_w_edges = 0;
   return TLOAM_B200_OK;
 }
 
@@ -4471,20 +4474,12 @@ int tloam_b200_pose_graph_size(tloam_b200_handle* h, size_t* nodes, size_t* loop
   return TLOAM_B200_OK;
 }
 
-int tloam_b200_pose_graph_optimize(tloam_b200_handle* h, tloam_pose_graph_result* out) {
-  if (!h || !out) return TLOAM_B200_ERR_INVALID_ARG;
-  if (!h->pg_on) return TLOAM_B200_ERR_NOT_READY;
+// the device buffers of one optimisation over the graph as it stands, the loop edges uploaded and T[0] = O; robust: after
+// them, the loop edges' weights (set to 1), residuals and the GNC state
+struct PgrBufs { double* w = nullptr; double* rho = nullptr; tloam_pgr_state* state = nullptr; };
+
+static int pg_prepare(tloam_b200_handle* h, const PgLib& lib, tloam_pg_args* ap, PgrBufs* robust) {
   const size_t N = h->pg_nodes, L = h->pg_ij.size() / 2;
-  memset(out, 0, sizeof(*out));
-  out->nodes = (long long)N; out->loop_edges = (long long)L;
-  h->d_pg_T = nullptr; h->pg_opt_nodes = 0;
-  if (L == 0) {
-    out->termination = TLOAM_POSE_GRAPH_NO_LOOPS;
-    return TLOAM_B200_OK;
-  }
-  PgLib lib;
-  int rc = pg_load(h, &lib);
-  if (rc != TLOAM_B200_OK) return rc;
   CU_TRY(cudaSetDevice(h->device));
   const tloam_pose_graph_config& c = h->pg_cfg;
   const size_t nl = 6 * L, ncol = nl + 1, E = N - 1 + L;
@@ -4494,6 +4489,8 @@ int tloam_b200_pose_graph_optimize(tloam_b200_handle* h, tloam_pose_graph_result
   const size_t o_edge = take(E * TLOAM_PG_EDGE * sizeof(double)), o_chain = take(N * TLOAM_PG_CHAIN * sizeof(double));
   const size_t o_b = take(N * 6 * sizeof(double)), o_Y = take(6 * (N - 1) * ncol * sizeof(double));
   const size_t o_S = take(nl * ncol * sizeof(double)), o_z = take(nl * sizeof(double)), o_n = take(N * 2 * sizeof(double));
+  size_t o_w = 0, o_rho = 0, o_g = 0;
+  if (robust) { o_w = take(L * sizeof(double)); o_rho = take(L * sizeof(double)); o_g = take(sizeof(tloam_pgr_state)); }
   if (o > h->cap_pg_scratch) {
     CU_TRY(cudaStreamSynchronize(h->stream));
     cudaFree(h->d_pg_scratch); h->d_pg_scratch = nullptr; h->cap_pg_scratch = 0;
@@ -4501,7 +4498,7 @@ int tloam_b200_pose_graph_optimize(tloam_b200_handle* h, tloam_pose_graph_result
     h->cap_pg_scratch = o;
   }
   unsigned char* base = h->d_pg_scratch;
-  tloam_pg_args a;
+  tloam_pg_args& a = *ap;
   memset(&a, 0, sizeof(a));
   a.O = h->d_pg_O;
   a.T = reinterpret_cast<double*>(base + o_T);
@@ -4515,6 +4512,7 @@ int tloam_b200_pose_graph_optimize(tloam_b200_handle* h, tloam_pose_graph_result
     a.w_loop[3 + k] = 1.0 / (c.sigma_loop_rotation * c.sigma_loop_rotation);
   }
   a.eps_translation = c.eps_translation; a.eps_rotation = c.eps_rotation; a.max_iterations = c.max_iterations;
+  int rc;
   if ((rc = pg_status(h, lib.chol_blocks(h->device, &a.chol_blocks), "occupancy")) != TLOAM_B200_OK) return rc;
   a.state = h->d_pg_state;
   a.edge = reinterpret_cast<double*>(base + o_edge);
@@ -4529,14 +4527,54 @@ int tloam_b200_pose_graph_optimize(tloam_b200_handle* h, tloam_pose_graph_result
   CU_TRY(cudaMemcpyAsync(base + o_ij, h->pg_ij.data(), 2 * L * sizeof(long long), cudaMemcpyHostToDevice, h->stream));
   CU_TRY(cudaMemcpyAsync(base + o_Z, h->pg_Z.data(), 16 * L * sizeof(double), cudaMemcpyHostToDevice, h->stream));
   CU_TRY(cudaMemcpyAsync(a.T, h->d_pg_O, N * 16 * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
+  if (robust) {
+    robust->w = reinterpret_cast<double*>(base + o_w);
+    robust->rho = reinterpret_cast<double*>(base + o_rho);
+    robust->state = reinterpret_cast<tloam_pgr_state*>(base + o_g);
+    const std::vector<double> ones(L, 1.0);
+    CU_TRY(cudaMemcpyAsync(robust->w, ones.data(), L * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  }
+  return TLOAM_B200_OK;
+}
+
+// enqueues one Gauss-Newton stage of up to max_iterations steps from T[cur]: the state reset (cost and initial_cost are
+// evaluated at T[cur] by the stage), then the launcher
+static int pg_stage(tloam_b200_handle* h, const PgLib& lib, tloam_pg_args& a, int cur, int max_iterations) {
   tloam_pg_state s;
   memset(&s, 0, sizeof(s));
+  s.cur = cur;
   s.term = TLOAM_POSE_GRAPH_ITERATION_LIMIT;
   CU_TRY(cudaMemcpyAsync(h->d_pg_state, &s, sizeof(s), cudaMemcpyHostToDevice, h->stream));
+  a.max_iterations = max_iterations;
   int e = 0, launches = 0;
   TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.optimize(&a, &launches)));
   h->launches += launches > 0 ? launches - 1 : 0;
-  if ((rc = pg_status(h, e, "k_pg_*")) != TLOAM_B200_OK) return rc;
+  return pg_status(h, e, "k_pg_*");
+}
+
+static void pg_forget(tloam_b200_handle* h) {
+  h->d_pg_T = nullptr; h->pg_opt_nodes = 0;
+  h->d_pgr_w = nullptr; h->pgr_w_edges = 0;
+}
+
+int tloam_b200_pose_graph_optimize(tloam_b200_handle* h, tloam_pose_graph_result* out) {
+  if (!h || !out) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->pg_on) return TLOAM_B200_ERR_NOT_READY;
+  const size_t N = h->pg_nodes, L = h->pg_ij.size() / 2;
+  memset(out, 0, sizeof(*out));
+  out->nodes = (long long)N; out->loop_edges = (long long)L;
+  pg_forget(h);
+  if (L == 0) {
+    out->termination = TLOAM_POSE_GRAPH_NO_LOOPS;
+    return TLOAM_B200_OK;
+  }
+  PgLib lib;
+  int rc = pg_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  tloam_pg_args a;
+  if ((rc = pg_prepare(h, lib, &a, nullptr)) != TLOAM_B200_OK) return rc;
+  if ((rc = pg_stage(h, lib, a, 0, h->pg_cfg.max_iterations)) != TLOAM_B200_OK) return rc;
+  tloam_pg_state s;
   CU_TRY(cudaMemcpyAsync(&s, h->d_pg_state, sizeof(s), cudaMemcpyDeviceToHost, h->stream));
   CU_TRY(cudaStreamSynchronize(h->stream));
   out->iterations = s.iter; out->termination = s.term;
@@ -4544,6 +4582,137 @@ int tloam_b200_pose_graph_optimize(tloam_b200_handle* h, tloam_pose_graph_result
   out->step_translation = s.step_t; out->step_rotation = s.step_r;
   h->d_pg_T = a.T + 16 * N * (size_t)s.cur;
   h->pg_opt_nodes = N;
+  return TLOAM_B200_OK;
+}
+
+// ---- robust pose graph (the outer GNC loop here; the residual and weight kernels in pose_graph_robust.cu, loaded from
+//      libtloam_b200_pgr.so on the first robust optimisation) ----
+struct PgrLib { tloam_pgr_update_fn update = nullptr; };
+static std::mutex g_pgr_mu;
+static PgrLib g_pgr;
+
+static int pgr_load(tloam_b200_handle* h, PgrLib* out) {
+  std::lock_guard<std::mutex> lk(g_pgr_mu);
+  if (!g_pgr.update) {
+    const std::string path = sibling_path("libtloam_b200_pgr.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    PgrLib l;
+    if (so) l.update = reinterpret_cast<tloam_pgr_update_fn>(dlsym(so, "tloam_pgr_update"));
+    if (!l.update) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "robust pose graph: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_pgr = l;
+  }
+  *out = g_pgr;
+  return TLOAM_B200_OK;
+}
+
+void tloam_b200_pose_graph_robust_default_config(tloam_pose_graph_robust_config* c) {
+  c->chi2_threshold = 16.81;
+  c->gnc_factor = 1.4;
+  c->inner_iterations = 2;
+  c->max_outer_iterations = 100;
+}
+
+int tloam_b200_pose_graph_optimize_robust(tloam_b200_handle* h, const tloam_pose_graph_robust_config* cfg,
+                                          tloam_pose_graph_robust_result* out) {
+  if (!h || !cfg || !out) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->pg_on) return TLOAM_B200_ERR_NOT_READY;
+  if (!std::isfinite(cfg->chi2_threshold) || !(cfg->chi2_threshold > 0.0) || !std::isfinite(cfg->gnc_factor) ||
+      !(cfg->gnc_factor > 1.0) || cfg->inner_iterations < 1 || cfg->inner_iterations > 100 || cfg->max_outer_iterations < 1 ||
+      cfg->max_outer_iterations > 1000)
+    return TLOAM_B200_ERR_INVALID_ARG;
+  const size_t N = h->pg_nodes, L = h->pg_ij.size() / 2;
+  memset(out, 0, sizeof(*out));
+  out->pg.nodes = (long long)N; out->pg.loop_edges = (long long)L;
+  pg_forget(h);
+  if (L == 0) {
+    out->pg.termination = TLOAM_POSE_GRAPH_NO_LOOPS;
+    out->gnc_termination = TLOAM_POSE_GRAPH_GNC_NO_LOOPS;
+    return TLOAM_B200_OK;
+  }
+  PgLib lib;
+  PgrLib rlib;
+  int rc = pg_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  if ((rc = pgr_load(h, &rlib)) != TLOAM_B200_OK) return rc;
+  tloam_pg_args a;
+  PgrBufs buf;
+  if ((rc = pg_prepare(h, lib, &a, &buf)) != TLOAM_B200_OK) return rc;
+  a.loop_w = buf.w;
+  tloam_pgr_args r;
+  memset(&r, 0, sizeof(r));
+  r.T = a.T; r.pg_state = a.state; r.loop_ij = a.loop_ij; r.loop_Z = a.loop_Z; r.N = N; r.L = L;
+  memcpy(r.w_loop, a.w_loop, sizeof(r.w_loop));
+  r.chi2_threshold = cfg->chi2_threshold; r.gnc_factor = cfg->gnc_factor;
+  r.rho = buf.rho; r.w = buf.w; r.state = buf.state;
+  r.device = h->device; r.stream = h->stream;
+  const int max_iterations = h->pg_cfg.max_iterations;
+  tloam_pg_state s;
+  tloam_pgr_state g;
+  memset(&g, 0, sizeof(g));
+  // one stage; update: then the weights at its poses (nothing when the stage was singular); then both states home
+  auto stage = [&](int cur, int iterations, int update, int first) -> int {
+    int rc2 = pg_stage(h, lib, a, cur, iterations);
+    if (rc2 != TLOAM_B200_OK) return rc2;
+    if (update) {
+      int e = 0, launches = 0;
+      TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = rlib.update(&r, first, &launches)));
+      h->launches += launches > 0 ? launches - 1 : 0;
+      if (e != cudaSuccess) {
+        snprintf(h->last_error, sizeof(h->last_error), "robust pose graph: k_pgr_*: %s", cudaGetErrorString((cudaError_t)e));
+        return TLOAM_B200_ERR_CUDA;
+      }
+      CU_TRY(cudaMemcpyAsync(&g, buf.state, sizeof(g), cudaMemcpyDeviceToHost, h->stream));
+    }
+    CU_TRY(cudaMemcpyAsync(&s, h->d_pg_state, sizeof(s), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    out->pg.iterations += s.iter;
+    return TLOAM_B200_OK;
+  };
+  if ((rc = stage(0, max_iterations, 1, 1)) != TLOAM_B200_OK) return rc;
+  out->pg.initial_cost = s.initial_cost;
+  int gnc = -1;
+  if (s.term == TLOAM_POSE_GRAPH_SINGULAR) gnc = TLOAM_POSE_GRAPH_GNC_SINGULAR;
+  else if (g.all_inliers) { gnc = TLOAM_POSE_GRAPH_GNC_ALL_INLIERS; out->inliers = (long long)L; }
+  while (gnc < 0) {
+    // g holds the weights the next stage runs with
+    out->outer_iterations++;
+    out->mu_final = g.mu; out->inliers = g.inliers; out->rejected = g.rejected;
+    if (g.binary) {
+      if ((rc = stage(s.cur, max_iterations, 0, 0)) != TLOAM_B200_OK) return rc;
+      gnc = s.term == TLOAM_POSE_GRAPH_SINGULAR ? TLOAM_POSE_GRAPH_GNC_SINGULAR : TLOAM_POSE_GRAPH_GNC_CONVERGED;
+      break;
+    }
+    const bool last = out->outer_iterations >= cfg->max_outer_iterations;
+    if ((rc = stage(s.cur, cfg->inner_iterations, !last, 0)) != TLOAM_B200_OK) return rc;
+    if (s.term == TLOAM_POSE_GRAPH_SINGULAR) gnc = TLOAM_POSE_GRAPH_GNC_SINGULAR;
+    else if (last) gnc = TLOAM_POSE_GRAPH_GNC_OUTER_LIMIT;
+  }
+  out->gnc_termination = gnc;
+  out->pg.termination = s.term;
+  out->pg.final_cost = s.cost;
+  out->pg.step_translation = s.step_t; out->pg.step_rotation = s.step_r;
+  h->d_pg_T = a.T + 16 * N * (size_t)s.cur;
+  h->pg_opt_nodes = N;
+  h->d_pgr_w = buf.w; h->pgr_w_edges = L;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_pose_graph_loop_weights(tloam_b200_handle* h, size_t first, size_t count, double* w) {
+  if (!h || (!w && count)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->pg_on) return TLOAM_B200_ERR_NOT_READY;
+  const size_t L = h->pg_ij.size() / 2;
+  if (first > L || count > L - first) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  const size_t split = first + count < h->pgr_w_edges ? first + count : (first > h->pgr_w_edges ? first : h->pgr_w_edges);
+  if (split > first)
+    CU_TRY(cudaMemcpyAsync(w, h->d_pgr_w + first, (split - first) * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  for (size_t l = split; l < first + count; ++l) w[l - first] = 1.0;
+  CU_TRY(cudaStreamSynchronize(h->stream));
   return TLOAM_B200_OK;
 }
 

@@ -154,6 +154,20 @@ class PoseGraphResult:
     CONVERGED, ITERATION_LIMIT, COST_INCREASED, SINGULAR, NO_LOOPS = range(5)
 
 
+@dataclasses.dataclass(frozen=True)
+class PoseGraphRobustResult:
+    """tloam_pose_graph_robust_result: pg is the PoseGraphResult of the whole run (iterations over every stage, the last
+    stage's termination, weighted costs); gnc_termination is one of PoseGraphRobustResult.CONVERGED .. NO_LOOPS; inliers
+    and rejected count the loop edges with weight exactly 1 and exactly 0; mu_final is the mu of the last weight update."""
+    pg: PoseGraphResult
+    outer_iterations: int
+    gnc_termination: int
+    mu_final: float
+    inliers: int
+    rejected: int
+    CONVERGED, OUTER_LIMIT, ALL_INLIERS, SINGULAR, NO_LOOPS = range(5)
+
+
 def rz(yaw):
     """the 4 x 4 rotation about z by yaw (rad); the C library's cos / sin, as the C++ shim's verifyLoop"""
     c, s = math.cos(yaw), math.sin(yaw)
@@ -930,6 +944,33 @@ class LocalRegistration:
         self._check(self._L.tloam_b200_pose_graph_optimize(self._h, C.byref(r)), "pose_graph_optimize")
         return PoseGraphResult(r.nodes, r.loop_edges, r.iterations, r.termination, r.initial_cost, r.final_cost,
                                r.step_translation, r.step_rotation)
+
+    def pose_graph_optimize_robust(self, **overrides):
+        """GNC with a TLS cost over the loop edges (include/tloam_b200.h "Robust pose graph"); overrides: fields of
+        tloam_pose_graph_robust_config (chi2_threshold, gnc_factor, inner_iterations, max_outer_iterations)"""
+        cfg = _lib.PoseGraphRobustConfig()
+        self._L.tloam_b200_pose_graph_robust_default_config(C.byref(cfg))
+        for k, v in overrides.items():
+            if not hasattr(cfg, k):
+                raise KeyError(k)
+            setattr(cfg, k, v)
+        r = _lib.PoseGraphRobustResult()
+        self._check(self._L.tloam_b200_pose_graph_optimize_robust(self._h, C.byref(cfg), C.byref(r)), "pose_graph_optimize_robust")
+        p = r.pg
+        return PoseGraphRobustResult(PoseGraphResult(p.nodes, p.loop_edges, p.iterations, p.termination, p.initial_cost,
+                                                     p.final_cost, p.step_translation, p.step_rotation),
+                                     r.outer_iterations, r.gnc_termination, r.mu_final, r.inliers, r.rejected)
+
+    def pose_graph_loop_weights(self, first=0, count=None):
+        """(count,): the last optimisation's loop-edge weights (1.0 after a plain one and for edges added after it)"""
+        n = self.pose_graph_size()[1]
+        if count is None:
+            count = n - first
+        if first < 0 or count < 0 or first + count > n:
+            raise RegistrationError(_lib.ERR_INVALID_ARG, "pose_graph_loop_weights")
+        out = np.zeros(count)
+        self._check(self._L.tloam_b200_pose_graph_loop_weights(self._h, int(first), int(count), _dp(out)), "pose_graph_loop_weights")
+        return out
 
     def pose_graph_poses(self, first=0, count=None):
         """(count, 4, 4): the last optimisation's poses, the odometry poses for nodes it did not cover"""
