@@ -908,6 +908,89 @@ int tloam_b200_global_map_correct(tloam_b200_handle* h, const long long* node, s
  * synchronises).  NOT_READY: mapping or tracking off.  INVALID_ARG past the last frame. */
 int tloam_b200_global_map_frame_poses(tloam_b200_handle* h, size_t first, size_t count, double* odom, double* current);
 
+/* ---- Loop verification against a submap (opt-in, on top of loop verification): the query keyframe is aligned to the
+ * keyframes of the loop frames around the candidate, moved into the candidate's sensor frame by their odometry poses, with
+ * a point-to-plane residual.  One sparse keyframe leaves gaps between the sensor's rings that a point-to-point ICP locks
+ * onto; the union of 2k + 1 keyframes fills them and the plane residual lets the query slide along a surface.  The
+ * result is a tloam_loop_verify_result, so tloam_b200_pose_graph_add_loop takes it as it is.  tloam_b200_loop_verify is
+ * not changed by any of this.
+ *   - Window.  For candidate c, half window k and F loop frames: frames lo = max(0, c - k) .. hi = min(c + k, F - 1),
+ *     without `query` if it lies inside.  Every window frame j has a pose O_j: with poses == NULL the pose graph's node j
+ *     (node i = loop frame i), read on the device from the node store -- the odometry pose the node was added with, never
+ *     an optimised one, so a verification does not depend on the optimisations before it; otherwise poses[j - lo], a host
+ *     array of hi - lo + 1 column-major 4 x 4 poses (the query's entry is not read but must be rigid too).
+ *   - Target.  A_j = O_c^-1 O_j, every product and sum rounded on its own, left to right, R (r, c) = O[4c + r]:
+ *       R_A(r, c) = (R_c(0, r) R_j(0, c) + R_c(1, r) R_j(1, c)) + R_c(2, r) R_j(2, c)
+ *       t_A(r)    = (R_c(0, r) d0 + R_c(1, r) d1) + R_c(2, r) d2,  d = t_j - t_c
+ *     The target is the concatenation, in frame order then keyframe row order, of A_j p for every row p of keyframe j:
+ *     x' = ((A00 x + A01 y) + A02 z) + A03.  Keyframe c's rows are copied, so k = 0 gives keyframe c bit for bit.  An empty
+ *     keyframe contributes nothing; the union is not down-sampled again.
+ *   - Normals.  For target row i, the rows j (i among them) with d2(i, j) <= normal_radius * normal_radius, d2 as in "Loop
+ *     verification", are visited in ascending j: n_i their number; mean = (sum x_j) / n_i per axis, the sum running from
+ *     0.0 in that order; C_ab = (sum (a_j - mean_a) (b_j - mean_b)) / n_i for ab = xx, xy, xz, yy, yz, zz, each product
+ *     rounded and added to a sum running from 0.0 in the same order (two passes over the neighbourhood).  The eigenvalues
+ *     l0 <= l1 <= l2 and the eigenvector of l0 come from a cyclic Jacobi iteration: at most 32 sweeps over the entries
+ *     (0,1), (0,2), (1,2); a sweep starts only while off = (a01^2 + a02^2) + a12^2 > 1e-32 * ((a00^2 + a11^2) + a22^2) and
+ *     off != 0; an entry that is 0 is skipped; theta = (a_qq - a_pp) / (2 a_pq), t = sign(theta) / (|theta| +
+ *     sqrt(theta^2 + 1)), c = 1 / sqrt(t^2 + 1), s = t c; columns p, q of a, then rows p, q of a, then columns p, q of the
+ *     eigenvector matrix become (c x_p - s x_q, s x_p + c x_q); the eigenvalues are sorted by the compare-exchanges (0,1),
+ *     (1,2), (0,1), a tie keeping the lower axis first.  Every operation is rounded on its own.  The row's normal is that
+ *     eigenvector; it is valid iff n_i >= min_normal_neighbours and l0 <= max_planarity * l1.  Its sign is whatever the
+ *     iteration gives and does not enter the result (e and J change sign together).
+ *   - Pass.  As in "Loop verification": p = R q + t for every row q of the query keyframe, its match the nearest target
+ *     row by (d2, index) over the whole target, an inlier iff d2 <= r * r.
+ *   - Step.  Over the inliers whose match m has a valid normal n (the contributing rows): e = (nx (px - mx) + ny (py - my))
+ *     + nz (pz - mz), J = [n^T, (p x n)^T] for the left perturbation delta = (upsilon, omega); H = sum J^T J, g = sum J^T e
+ *     in a fixed reduction order; delta = -H^-1 g by LDL^T; T <- exp(delta) . T.  Fewer than 6 contributing rows stop the
+ *     run with FEW_INLIERS, a pivot that is not positive and finite with SINGULAR.  The radius schedule, the convergence
+ *     test and the iteration limit are those of "Loop verification".
+ *   - Result, at the final T with one more pass at r = corr_dist_fine: T = T_cand_query; fitness = the mean nearest-neighbour
+ *     d2 (point to point, to the target) over ALL query rows; inliers = the contributing rows; rmse = sqrt(sum of their
+ *     e^2 / inliers); n_candidate_points = the target's rows; accepted = converged && fitness <= max_fitness.  An empty
+ *     query keyframe or an empty target: EMPTY, T = guess, fitness +inf, not accepted.
+ *   - One verification is k_lvs_poses, k_lvs_assemble, k_lvs_normals (the normals are computed once, not per pass), then
+ *     the rounds of k_lvs_match / k_lvs_reduce / k_lvs_step and the final pass, all on the handle's stream with one copy
+ *     home.  The normals' neighbour search is exhaustive: its cost grows with the square of the target's rows.  The
+ *     kernels live in libtloam_b200_loopvs.so, loaded from this library's directory by the enable call; if it is missing
+ *     the calls return ERR_CUDA (tloam_b200_last_error names the file).  The scratch (target, normals, partials, match
+ *     records) is allocated by the first run and grown when a run needs more.  Off until enabled: nothing is allocated or
+ *     launched, and every other call gives the bits and launch counts it gives without it. */
+typedef struct tloam_loop_verify_submap_config {
+  int half_window;                     /* k, 0 .. 50 */
+  double normal_radius;                /* m */
+  int min_normal_neighbours;           /* >= 3 */
+  double max_planarity;                /* a normal is valid iff l0 <= max_planarity * l1 */
+  double corr_dist_coarse;             /* first correspondence radius, m */
+  double corr_dist_fine;               /* last correspondence radius, m (<= corr_dist_coarse) */
+  int max_iterations;                  /* Gauss-Newton steps, 1 .. 200 */
+  double eps_translation;              /* m */
+  double eps_rotation;                 /* rad */
+  double max_fitness;                  /* m^2 */
+} tloam_loop_verify_submap_config;
+/* half_window 5, normal_radius 1 m, min_normal_neighbours 5, max_planarity 0.1, corr_dist_coarse 4 m, corr_dist_fine 1 m,
+ * max_iterations 40, eps_translation 1e-4 m, eps_rotation 1e-5 rad, max_fitness 0.5 m^2 (DESIGN.md section 4c has how they
+ * were chosen) */
+void tloam_b200_loop_verify_submap_default_config(tloam_loop_verify_submap_config* c);
+/* allowed at any database size.  NOT_READY unless loop verification is on; tloam_b200_loop_enable turns it off with loop
+ * verification, tloam_b200_loop_reset keeps it on.  INVALID_ARG: cfg null; half_window outside [0, 50];
+ * min_normal_neighbours < 3; another value not finite or not > 0; corr_dist_fine > corr_dist_coarse; max_iterations
+ * outside [1, 200]. */
+int tloam_b200_loop_verify_submap_enable(tloam_b200_handle* h, const tloam_loop_verify_submap_config* cfg);
+/* aligns keyframe query to the submap around keyframe candidate from guess (column-major 4 x 4; null: identity), enqueued
+ * behind every earlier add, and returns once the result is home.  NOT_READY: submap verification off, or poses null and
+ * the pose graph off or with fewer than hi + 1 nodes; INVALID_ARG: an index out of range; BAD_POSE: guess or one of poses
+ * not rigid. */
+int tloam_b200_loop_verify_submap(tloam_b200_handle* h, long long query, long long candidate, const double guess[16],
+                                  const double* poses, tloam_loop_verify_result* out);
+/* the last tloam_b200_loop_verify_submap's target: per row its xyz (3), normal (3), validity and neighbour count n_i
+ * (synchronises; *n = the target's rows, 0 after an EMPTY run; any output may be null).  INVALID_ARG: capacity < *n;
+ * NOT_READY: no submap verification since enable.  For tests and viewers. */
+int tloam_b200_loop_verify_submap_target(tloam_b200_handle* h, double* xyz, double* normal, unsigned char* valid, int* neighbours,
+                                         size_t capacity, size_t* n);
+/* the last tloam_b200_loop_verify_submap's matches at pass k, as tloam_b200_loop_verify_matches: per query keyframe point the
+ * target row and its d2 */
+int tloam_b200_loop_verify_submap_matches(tloam_b200_handle* h, int pass, int* index, double* d2, size_t capacity, size_t* n);
+
 /* Pinned host memory helpers (optional; pinned inputs make set_* a direct DMA, no staging threads). */
 int tloam_b200_host_alloc(void** p, size_t bytes);
 int tloam_b200_host_free(void* p);

@@ -16,7 +16,8 @@
 // the driver's sensor_msgs/PointCloud2 as it arrived (packed_scan_b200.hpp): one upload, unpacked on the device, its
 // intensity field (if any) carried into the map.  enableLoopDetection / addLoopFrame / loopResult add loop closure: a Scan
 // Context descriptor per frame and an exact search over every earlier frame, on the GPU; enableLoopVerification / verifyLoop
-// check a candidate by a scan-to-scan ICP of down-sampled keyframes kept on the GPU and give the relative pose.
+// check a candidate by a scan-to-scan ICP of down-sampled keyframes kept on the GPU and give the relative pose;
+// enableSubmapVerification / verifyLoopSubmap check it against the keyframes around the candidate, point to plane.
 // Without the reference headers (this repository's tests) define TLOAM_B200_MOCK_HOST_TYPES and provide the host types
 // (tests/mock/mock_tloam.hpp).
 #ifndef TLOAM_B200_FRONT_END_B200_HPP
@@ -184,6 +185,25 @@ class FrontEndB200 {
     const double c = std::cos(lr.yaw), s = std::sin(lr.yaw);
     const double guess[16] = {c, s, 0, 0, -s, c, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
     return report(tloam_b200_loop_verify(h_, lr.query, lr.candidate, guess, &out), "verifyLoop");
+  }
+
+  // loop verification against a submap (include/tloam_b200.h "Loop verification against a submap"): the query keyframe is
+  // aligned, point to plane, to the keyframes of the frames around the candidate, placed by the pose graph's odometry
+  // nodes.  Needs enableLoopVerification, and a pose-graph node next to every added loop frame (addPoseGraphNode).
+  bool enableSubmapVerification(const tloam_loop_verify_submap_config& cfg) {
+    return report(tloam_b200_loop_verify_submap_enable(h_, &cfg), "enableSubmapVerification");
+  }
+  bool enableSubmapVerification() {
+    tloam_loop_verify_submap_config c;
+    tloam_b200_loop_verify_submap_default_config(&c);
+    return enableSubmapVerification(c);
+  }
+  // as verifyLoop, against the submap around the candidate; out.T is T_cand_query, to be handed to addLoopEdge when
+  // out.accepted
+  bool verifyLoopSubmap(const tloam_loop_result& lr, tloam_loop_verify_result& out) {
+    const double c = std::cos(lr.yaw), s = std::sin(lr.yaw);
+    const double guess[16] = {c, s, 0, 0, -s, c, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+    return report(tloam_b200_loop_verify_submap(h_, lr.query, lr.candidate, guess, nullptr, &out), "verifyLoopSubmap");
   }
 
   // pose graph (include/tloam_b200.h "Pose graph"): the odometry chain and the accepted loop edges, optimised on the GPU.

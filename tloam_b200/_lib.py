@@ -74,6 +74,14 @@ class LoopVerifyConfig(C.Structure):
                 ("max_fitness", C.c_double), ("initial_capacity_points", C.c_size_t)]
 
 
+class LoopVerifySubmapConfig(C.Structure):
+    """tloam_loop_verify_submap_config (include/tloam_b200.h "Loop verification against a submap")."""
+    _fields_ = [("half_window", C.c_int), ("normal_radius", C.c_double), ("min_normal_neighbours", C.c_int),
+                ("max_planarity", C.c_double), ("corr_dist_coarse", C.c_double), ("corr_dist_fine", C.c_double),
+                ("max_iterations", C.c_int), ("eps_translation", C.c_double), ("eps_rotation", C.c_double),
+                ("max_fitness", C.c_double)]
+
+
 class LoopVerifyResult(C.Structure):
     """tloam_loop_verify_result: T_cand_query (column-major) and the ICP's verdict."""
     _fields_ = [("query", C.c_longlong), ("candidate", C.c_longlong), ("T", C.c_double * 16), ("fitness", C.c_double),
@@ -213,6 +221,8 @@ EXPORTS = [
     "tloam_b200_pose_graph_correction", "tloam_b200_pose_graph_robust_default_config",
     "tloam_b200_pose_graph_optimize_robust", "tloam_b200_pose_graph_loop_weights",
     "tloam_b200_global_map_correction_enable", "tloam_b200_global_map_correct", "tloam_b200_global_map_frame_poses",
+    "tloam_b200_loop_verify_submap_default_config", "tloam_b200_loop_verify_submap_enable", "tloam_b200_loop_verify_submap",
+    "tloam_b200_loop_verify_submap_target", "tloam_b200_loop_verify_submap_matches",
 ]
 
 _lib = None
@@ -401,5 +411,11 @@ def load():
     L.tloam_b200_global_map_correction_enable.argtypes = [vp]
     L.tloam_b200_global_map_correct.argtypes = [vp, C.POINTER(C.c_longlong), C.c_size_t]
     L.tloam_b200_global_map_frame_poses.argtypes = [vp, C.c_size_t, C.c_size_t, dp, dp]
+    L.tloam_b200_loop_verify_submap_default_config.argtypes = [C.POINTER(LoopVerifySubmapConfig)]
+    L.tloam_b200_loop_verify_submap_default_config.restype = None
+    L.tloam_b200_loop_verify_submap_enable.argtypes = [vp, C.POINTER(LoopVerifySubmapConfig)]
+    L.tloam_b200_loop_verify_submap.argtypes = [vp, C.c_longlong, C.c_longlong, dp, dp, C.POINTER(LoopVerifyResult)]
+    L.tloam_b200_loop_verify_submap_target.argtypes = [vp, dp, dp, C.POINTER(C.c_ubyte), C.POINTER(C.c_int), C.c_size_t, szp]
+    L.tloam_b200_loop_verify_submap_matches.argtypes = [vp, C.c_int, C.POINTER(C.c_int), dp, C.c_size_t, szp]
     _lib = L
     return L

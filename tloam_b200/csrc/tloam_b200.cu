@@ -31,6 +31,7 @@
 #include "deskew.h"
 #include "scan_context.h"
 #include "loop_verify.h"
+#include "loop_verify_submap.h"
 #include "pose_graph.h"
 #include "pose_graph_robust.h"
 #include "map_correct.h"
@@ -253,6 +254,13 @@ struct tloam_b200_handle {
   unsigned char* d_lv_scratch = nullptr;   size_t cap_lv_scratch = 0;                           // the verification's scratch
   bool lv_ran = false;                     int lv_passes = 0;   unsigned long long lv_nq = 0;   // the last verification
   const int* lv_match_index = nullptr;    const double* lv_match_d2 = nullptr;                 // its matches, pass-major
+  // ---- loop verification against a submap (tloam_b200_loop_verify_submap*, libtloam_b200_loopvs.so): reads the keyframe
+  //      store above and the pose graph's node store; its scratch is allocated by the first run and grown ----
+  bool lvs_on = false;
+  tloam_loop_verify_submap_config lvs_cfg;
+  unsigned char* d_lvs_scratch = nullptr;  size_t cap_lvs_scratch = 0;
+  bool lvs_ran = false;                    int lvs_passes = 0;   unsigned long long lvs_nq = 0, lvs_nm = 0;   // the last run
+  tloam_lvs_args lvs_last;                 // its buffers (target, normals, matches)
   // ---- pose graph (tloam_b200_pose_graph*, libtloam_b200_pg.so): the node store on the device, the loop edges on the
   //      host until an optimisation uploads them; nothing is allocated or launched until it is enabled ----
   bool pg_on = false;
@@ -463,7 +471,7 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   if (h->h_loop_best) cudaFreeHost(h->h_loop_best);
   if (h->ev_loop) cudaEventDestroy(h->ev_loop);
   cudaFree(h->d_lv_st); cudaFree(h->d_lv_pose); cudaFree(h->d_lv_pts); cudaFree(h->d_lv_off); cudaFree(h->d_lv_reg);
-  cudaFree(h->d_lv_fin); cudaFree(h->d_lv_state); cudaFree(h->d_lv_scratch);
+  cudaFree(h->d_lv_fin); cudaFree(h->d_lv_state); cudaFree(h->d_lv_scratch); cudaFree(h->d_lvs_scratch);
   for (auto& pr : h->lv_probes) { if (pr.ev) cudaEventDestroy(pr.ev); if (pr.h_count) cudaFreeHost(pr.h_count); }
   cudaFree(h->d_pg_O); cudaFree(h->d_pg_scratch); cudaFree(h->d_pg_state);
   cudaFree(h->d_gmc_O); cudaFree(h->d_gmc_P); cudaFree(h->d_gmc_scratch);
@@ -3911,6 +3919,7 @@ int tloam_b200_loop_enable(tloam_b200_handle* h, const tloam_loop_config* cfg) {
   h->loop_frames = 0; h->loop_growths = 0; h->loop_has_result = false; h->loop_query = -1;
   h->loop_on = true;
   h->lv_on = false;                        // verification is enabled anew on the empty database
+  h->lvs_on = false;
   return TLOAM_B200_OK;
 }
 
@@ -4083,6 +4092,7 @@ static int lv_clear(tloam_b200_handle* h) {
   h->lv_cum = h->lv_known_cum = h->lv_known = 0;
   for (auto& pr : h->lv_probes) pr.pending = false;
   h->lv_ran = false; h->lv_passes = 0; h->lv_nq = 0;
+  h->lvs_ran = false; h->lvs_passes = 0;
   return TLOAM_B200_OK;
 }
 
@@ -4844,6 +4854,208 @@ int tloam_b200_global_map_frame_poses(tloam_b200_handle* h, size_t first, size_t
     CU_TRY(cudaMemcpyAsync(odom, h->d_gmc_O + 16 * first, count * 16 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   if (count && current)
     CU_TRY(cudaMemcpyAsync(current, h->d_gmc_P + 16 * first, count * 16 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Loop verification against a submap (the window, the checks and the scratch here; the kernels in loop_verify_submap.cu,
+// loaded from libtloam_b200_loopvs.so on the first call).
+// ---------------------------------------------------------------------------------------------
+static std::mutex g_loopvs_mu;
+static tloam_lvs_verify_fn g_loopvs = nullptr;
+
+static int loopvs_load(tloam_b200_handle* h, tloam_lvs_verify_fn* out) {
+  std::lock_guard<std::mutex> lk(g_loopvs_mu);
+  if (!g_loopvs) {
+    const std::string path = sibling_path("libtloam_b200_loopvs.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    tloam_lvs_verify_fn f = so ? reinterpret_cast<tloam_lvs_verify_fn>(dlsym(so, "tloam_lvs_verify")) : nullptr;
+    if (!f) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "loop verification against a submap: cannot load %s: %s", path.c_str(),
+               why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_loopvs = f;
+  }
+  *out = g_loopvs;
+  return TLOAM_B200_OK;
+}
+
+void tloam_b200_loop_verify_submap_default_config(tloam_loop_verify_submap_config* c) {
+  c->half_window = 5;
+  c->normal_radius = 1.0; c->min_normal_neighbours = 5; c->max_planarity = 0.1;
+  c->corr_dist_coarse = 4.0; c->corr_dist_fine = 1.0;
+  c->max_iterations = 40;
+  c->eps_translation = 1e-4; c->eps_rotation = 1e-5;
+  c->max_fitness = 0.5;
+}
+
+int tloam_b200_loop_verify_submap_enable(tloam_b200_handle* h, const tloam_loop_verify_submap_config* c) {
+  if (!h || !c) return TLOAM_B200_ERR_INVALID_ARG;
+  const double v[7] = {c->normal_radius, c->max_planarity, c->corr_dist_coarse, c->corr_dist_fine, c->eps_translation,
+                       c->eps_rotation, c->max_fitness};
+  for (double x : v)
+    if (!std::isfinite(x) || !(x > 0.0)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (c->half_window < 0 || c->half_window > TLOAM_LVS_MAX_HALF_WINDOW || c->min_normal_neighbours < 3 ||
+      c->corr_dist_fine > c->corr_dist_coarse || c->max_iterations < 1 || c->max_iterations > 200)
+    return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->lv_on) return TLOAM_B200_ERR_NOT_READY;
+  tloam_lvs_verify_fn fn;
+  int rc = loopvs_load(h, &fn);
+  if (rc != TLOAM_B200_OK) return rc;
+  h->lvs_cfg = *c;
+  h->lvs_on = true;
+  h->lvs_ran = false; h->lvs_passes = 0;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_loop_verify_submap(tloam_b200_handle* h, long long query, long long candidate, const double guess[16],
+                                  const double* poses, tloam_loop_verify_result* out) {
+  if (!h || !out) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->lv_on || !h->lvs_on) return TLOAM_B200_ERR_NOT_READY;
+  if (query < 0 || candidate < 0 || (size_t)query >= h->loop_frames || (size_t)candidate >= h->loop_frames)
+    return TLOAM_B200_ERR_INVALID_ARG;
+  double T[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+  if (guess) memcpy(T, guess, sizeof(T));
+  if (!pg_rigid(T)) return TLOAM_B200_ERR_BAD_POSE;
+  const tloam_loop_verify_submap_config& c = h->lvs_cfg;
+  const size_t k = (size_t)c.half_window, cand = (size_t)candidate;
+  const size_t lo = cand > k ? cand - k : 0, hi = cand + k < h->loop_frames - 1 ? cand + k : h->loop_frames - 1;
+  const size_t n_win = hi - lo + 1;
+  if (poses) {
+    for (size_t w = 0; w < n_win; ++w)
+      if (!pg_rigid(poses + 16 * w)) return TLOAM_B200_ERR_BAD_POSE;
+  } else if (!h->pg_on || h->pg_nodes < hi + 1) {
+    return TLOAM_B200_ERR_NOT_READY;
+  }
+  tloam_lvs_verify_fn fn;
+  int rc = loopvs_load(h, &fn);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  // the window's slice of the keyframe table and the query's range (synchronises, as tloam_b200_loop_verify does)
+  unsigned long long off[2 * TLOAM_LVS_MAX_HALF_WINDOW + 2], q0 = 0, nq = 0;
+  if ((rc = lv_range(h, (size_t)query, &q0, &nq)) != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaMemcpyAsync(off, h->d_lv_off + lo, (n_win + 1) * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  const bool inside = (size_t)query >= lo && (size_t)query <= hi;
+  const unsigned long long nm = off[n_win] - off[0] - (inside ? nq : 0);
+  memset(out, 0, sizeof(*out));
+  out->query = query; out->candidate = candidate;
+  memcpy(out->T, T, sizeof(T));
+  out->n_query_points = (long long)nq; out->n_candidate_points = (long long)nm;
+  h->lvs_ran = true; h->lvs_passes = 0; h->lvs_nq = nq; h->lvs_nm = 0;
+  if (nq == 0 || nm == 0) {
+    out->termination = TLOAM_LOOP_VERIFY_EMPTY;
+    out->fitness = INFINITY;
+    return TLOAM_B200_OK;
+  }
+  // the target is split over grid y until the search has about four blocks per SM of an H100 SXM (132)
+  const unsigned long long qb = (nq + TLOAM_LVS_THREADS - 1) / TLOAM_LVS_THREADS, tiles = (nm + TLOAM_LVS_THREADS - 1) / TLOAM_LVS_THREADS;
+  unsigned long long splits = (4 * 132 + qb - 1) / qb;
+  if (splits > tiles) splits = tiles;
+  if (splits < 1) splits = 1;
+  const size_t passes = (size_t)c.max_iterations + 1;
+  size_t o = round_up(sizeof(tloam_lv_state), 256);
+  const size_t o_poses = o;   o += round_up(n_win * 16 * sizeof(double), 256);
+  const size_t o_A = o;       o += round_up(n_win * 16 * sizeof(double), 256);
+  const size_t o_target = o;  o += round_up(nm * 3 * sizeof(double), 256);
+  const size_t o_normal = o;  o += round_up(nm * 3 * sizeof(double), 256);
+  const size_t o_neigh = o;   o += round_up(nm * sizeof(int), 256);
+  const size_t o_valid = o;   o += round_up(nm, 256);
+  const size_t o_part = o;    o += round_up(splits * nq * sizeof(tloam_lv_best), 256);
+  const size_t o_sums = o;    o += round_up(qb * TLOAM_LVS_SUMS * sizeof(double), 256);
+  const size_t o_idx = o;     o += round_up(passes * nq * sizeof(int), 256);
+  const size_t o_d2 = o;      o += passes * nq * sizeof(double);
+  if (o > h->cap_lvs_scratch) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_lvs_scratch); h->d_lvs_scratch = nullptr; h->cap_lvs_scratch = 0;
+    const size_t bytes = o + o / 2;
+    CU_TRY(cudaMalloc(&h->d_lvs_scratch, bytes));
+    h->cap_lvs_scratch = bytes;
+  }
+  unsigned char* base = h->d_lvs_scratch;
+  tloam_lv_state s;
+  memset(&s, 0, sizeof(s));
+  for (int r = 0; r < 3; ++r) {
+    for (int j = 0; j < 3; ++j) s.R[3 * r + j] = T[4 * j + r];
+    s.t[r] = T[12 + r];
+  }
+  s.r = c.corr_dist_coarse;
+  s.term = TLOAM_LOOP_VERIFY_ITERATION_LIMIT;
+  CU_TRY(cudaMemcpyAsync(base, &s, sizeof(s), cudaMemcpyHostToDevice, h->stream));   // pageable: staged before return
+  if (poses) CU_TRY(cudaMemcpyAsync(base + o_poses, poses, n_win * 16 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  tloam_lvs_args a;
+  memset(&a, 0, sizeof(a));
+  a.pts = h->d_lv_pts; a.offsets = h->d_lv_off;
+  a.lo = lo; a.hi = hi; a.candidate = cand;
+  a.q0 = q0; a.nq = nq; a.query_in_window = inside ? 1 : 0; a.base = off[0]; a.nm = nm;
+  a.poses = poses ? reinterpret_cast<const double*>(base + o_poses) : h->d_pg_O + 16 * lo;
+  a.A = reinterpret_cast<double*>(base + o_A);
+  a.target = reinterpret_cast<double*>(base + o_target);
+  a.normal = reinterpret_cast<double*>(base + o_normal);
+  a.neighbours = reinterpret_cast<int*>(base + o_neigh);
+  a.valid = base + o_valid;
+  a.normal_radius = c.normal_radius; a.max_planarity = c.max_planarity; a.min_normal_neighbours = c.min_normal_neighbours;
+  a.corr_dist_coarse = c.corr_dist_coarse; a.corr_dist_fine = c.corr_dist_fine;
+  a.eps_translation = c.eps_translation; a.eps_rotation = c.eps_rotation; a.max_iterations = c.max_iterations;
+  a.splits = (unsigned)splits;
+  a.state = reinterpret_cast<tloam_lv_state*>(base);
+  a.part = reinterpret_cast<tloam_lv_best*>(base + o_part);
+  a.sums = reinterpret_cast<double*>(base + o_sums);
+  a.match_index = reinterpret_cast<int*>(base + o_idx);
+  a.match_d2 = reinterpret_cast<double*>(base + o_d2);
+  a.device = h->device; a.stream = h->stream;
+  h->lvs_last = a; h->lvs_nm = nm;
+  int e = 0, launches = 0;
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = fn(&a, &launches)));
+  h->launches += launches > 0 ? launches - 1 : 0;
+  if ((rc = lv_status(h, e, "k_lvs_*")) != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaMemcpyAsync(&s, a.state, sizeof(s), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  for (int r = 0; r < 3; ++r) {
+    for (int j = 0; j < 3; ++j) out->T[4 * j + r] = s.R[3 * r + j];
+    out->T[12 + r] = s.t[r];
+  }
+  out->fitness = s.fitness; out->rmse = s.rmse; out->inliers = (long long)s.inliers;
+  out->iterations = s.iter; out->termination = s.term;
+  out->accepted = s.term == TLOAM_LOOP_VERIFY_CONVERGED && s.fitness <= c.max_fitness ? 1 : 0;
+  h->lvs_passes = s.iter + 1;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_loop_verify_submap_target(tloam_b200_handle* h, double* xyz, double* normal, unsigned char* valid, int* neighbours,
+                                         size_t capacity, size_t* n) {
+  if (!h || !n) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->lv_on || !h->lvs_on || !h->lvs_ran) return TLOAM_B200_ERR_NOT_READY;
+  const size_t nm = h->lvs_nm;
+  *n = nm;
+  if (capacity < nm) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!nm) return TLOAM_B200_OK;
+  const tloam_lvs_args& a = h->lvs_last;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (xyz) CU_TRY(cudaMemcpyAsync(xyz, a.target, nm * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (normal) CU_TRY(cudaMemcpyAsync(normal, a.normal, nm * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (valid) CU_TRY(cudaMemcpyAsync(valid, a.valid, nm, cudaMemcpyDeviceToHost, h->stream));
+  if (neighbours) CU_TRY(cudaMemcpyAsync(neighbours, a.neighbours, nm * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_loop_verify_submap_matches(tloam_b200_handle* h, int pass, int* index, double* d2, size_t capacity, size_t* n) {
+  if (!h || !n) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->lv_on || !h->lvs_on || !h->lvs_ran) return TLOAM_B200_ERR_NOT_READY;
+  *n = h->lvs_nq;
+  if (pass < 0 || pass >= h->lvs_passes || capacity < h->lvs_nq) return TLOAM_B200_ERR_INVALID_ARG;
+  const size_t nq = h->lvs_nq;
+  const tloam_lvs_args& a = h->lvs_last;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (index) CU_TRY(cudaMemcpyAsync(index, a.match_index + (size_t)pass * nq, nq * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  if (d2) CU_TRY(cudaMemcpyAsync(d2, a.match_d2 + (size_t)pass * nq, nq * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   CU_TRY(cudaStreamSynchronize(h->stream));
   return TLOAM_B200_OK;
 }

@@ -899,6 +899,62 @@ class LocalRegistration:
                                                            C.byref(n)), "loop_verify_matches")
         return idx, d2
 
+    # ---- loop verification against a submap (the keyframes around the candidate, point to plane; include/tloam_b200.h
+    #      "Loop verification against a submap") ----
+    def loop_verify_submap_enable(self, **overrides):
+        """needs loop_verify_enable; overrides: fields of tloam_loop_verify_submap_config (half_window, normal_radius,
+        min_normal_neighbours, max_planarity, corr_dist_coarse, corr_dist_fine, max_iterations, eps_translation,
+        eps_rotation, max_fitness)"""
+        cfg = _lib.LoopVerifySubmapConfig()
+        self._L.tloam_b200_loop_verify_submap_default_config(C.byref(cfg))
+        for k, v in overrides.items():
+            if not hasattr(cfg, k):
+                raise KeyError(k)
+            setattr(cfg, k, v)
+        self._check(self._L.tloam_b200_loop_verify_submap_enable(self._h, C.byref(cfg)), "loop_verify_submap_enable")
+
+    def loop_verify_submap(self, query, candidate, guess=None, yaw=None, poses=None):
+        """align keyframe query to the submap around keyframe candidate from guess (4 x 4; default identity) or Rz(yaw).
+        poses: the (hi - lo + 1) x 4 x 4 poses of the window's frames lo .. hi; None: the pose graph's nodes.  Returns a
+        LoopVerifyResult"""
+        if yaw is not None:
+            if guess is not None:
+                raise ValueError("loop_verify_submap: give guess or yaw, not both")
+            guess = rz(yaw)
+        g = None if guess is None else np.asfortranarray(np.asarray(guess, dtype=np.float64).reshape(4, 4)).ravel(order="F").copy()
+        p = None if poses is None else np.ascontiguousarray(np.asarray(poses, dtype=np.float64).reshape(-1, 4, 4).transpose(0, 2, 1))
+        r = _lib.LoopVerifyResult()
+        self._check(self._L.tloam_b200_loop_verify_submap(self._h, int(query), int(candidate), None if g is None else _dp(g),
+                                                          None if p is None else _dp(p), C.byref(r)), "loop_verify_submap")
+        T = np.array(r.T[:]).reshape(4, 4, order="F")
+        return LoopVerifyResult(r.query, r.candidate, T, r.fitness, r.rmse, r.inliers, r.n_query_points, r.n_candidate_points,
+                                r.iterations, r.termination, bool(r.accepted))
+
+    def loop_verify_submap_target(self):
+        """the last loop_verify_submap's target: (xyz (n x 3), normal (n x 3), valid (n,) bool, neighbours (n,))"""
+        n = C.c_size_t(0)
+        rc = self._L.tloam_b200_loop_verify_submap_target(self._h, None, None, None, None, 0, C.byref(n))   # the size
+        if rc != _lib.ERR_INVALID_ARG or n.value == 0:
+            self._check(rc, "loop_verify_submap_target")
+        xyz, nrm = np.zeros((n.value, 3)), np.zeros((n.value, 3))
+        valid, cnt = np.zeros(n.value, dtype=np.uint8), np.zeros(n.value, dtype=np.int32)
+        self._check(self._L.tloam_b200_loop_verify_submap_target(
+            self._h, _dp(xyz), _dp(nrm), valid.ctypes.data_as(C.POINTER(C.c_ubyte)), cnt.ctypes.data_as(C.POINTER(C.c_int)),
+            n.value, C.byref(n)), "loop_verify_submap_target")
+        return xyz, nrm, valid.astype(bool), cnt
+
+    def loop_verify_submap_matches(self, k):
+        """the last loop_verify_submap's matches at pass k (k = iterations: the final pass): per query keyframe point the
+        target row (-1: none) and its d2"""
+        n = C.c_size_t(0)
+        rc = self._L.tloam_b200_loop_verify_submap_matches(self._h, int(k), None, None, 0, C.byref(n))    # the size
+        if rc != _lib.ERR_INVALID_ARG or n.value == 0:
+            self._check(rc, "loop_verify_submap_matches")
+        idx, d2 = np.zeros(n.value, dtype=np.int32), np.zeros(n.value)
+        self._check(self._L.tloam_b200_loop_verify_submap_matches(self._h, int(k), idx.ctypes.data_as(C.POINTER(C.c_int)), _dp(d2),
+                                                                  n.value, C.byref(n)), "loop_verify_submap_matches")
+        return idx, d2
+
     # ---- pose graph (odometry and verified loop edges, Gauss-Newton; include/tloam_b200.h "Pose graph") ----
     def pose_graph_enable(self, **overrides):
         """start an empty pose graph; overrides: fields of tloam_pose_graph_config (sigma_odom_translation,
