@@ -908,6 +908,73 @@ int tloam_b200_global_map_correct(tloam_b200_handle* h, const long long* node, s
  * synchronises).  NOT_READY: mapping or tracking off.  INVALID_ARG past the last frame. */
 int tloam_b200_global_map_frame_poses(tloam_b200_handle* h, size_t first, size_t count, double* odom, double* current);
 
+/* ---- Dynamic-point removal (opt-in): free-space votes from every appended scan's range image.  A map point is dynamic
+ * when later scans look through the place where it sits: the ray in its direction returns from something clearly
+ * farther away.  The map itself is never edited: it stays append-only, and the map, its frame table, the intensity
+ * channel, the pose tables, the registered scan and the odometry keep the bits they have with removal off.  Two counters
+ * per map row, (through, hits), are kept next to it, and tloam_b200_global_map_static_download returns the map without
+ * the rows judged dynamic.
+ *   - Enable.  tloam_b200_global_map_dynamic_enable is allowed only on an empty map (right after
+ *     tloam_b200_global_map_enable or _reset; otherwise NOT_READY).  tloam_b200_global_map_reset zeroes the counters and
+ *     keeps removal on; tloam_b200_global_map_enable turns it off.  While it is off nothing is allocated or launched.
+ *   - Per append.  Every tloam_b200_global_map_append* variant (host, chained, _frame, intensity, packed) votes with the
+ *     sensor-frame rows it transforms (read before the transform) and the pose it places the block at: the host pose, the
+ *     device pose for _chained appends, or P_f with correction tracking on.  The votes go to the map rows [0, count)
+ *     present before the append; the rows the append adds start at (0, 0).  Voting adds four launches per append with at
+ *     least one row and no synchronisation; an append of no rows votes nothing.  When the map grows, the counters are copied
+ *     with it.
+ *   - Range of a row (x, y, z): r = sqrt((x x + y y) + z z); the row is used iff min_range <= r <= max_range (a NaN or
+ *     infinite row never is).
+ *   - Pixel of a used row.  Column: Scan Context's sector rule with n_cols sectors (see "Loop closure"): the boundaries
+ *     (cos, sin) of 2 pi k / n_cols, k = 1 .. n_cols - 1, by the C library on the host; rows with y > 0 or (y = 0 and
+ *     x >= 0) count the k in 1 .. (n_cols - 1) / 2 with c_k y - s_k x > 0, the others (n_cols - 1) / 2 plus the count
+ *     over the remaining k.  The sign sequence is monotone within a half-plane, so the device counts it by binary search.
+ *     Row: s = z / r against b_k = sin(lo + k (hi - lo) / n_rows), k = 0 .. n_rows, lo / hi = fov_down / fov_up times
+ *     (pi / 180), by the C library on the host.  The row is outside the image unless b_0 <= s <= b_n_rows; otherwise its
+ *     image row is the number of k in 1 .. n_rows - 1 with s > b_k.
+ *   - Range image (n_rows x n_cols, +inf = empty): the minimum r of the scan's used rows per pixel, independent of order.
+ *     Window image: for pixel (i, j) the minimum over rows i - window_rows .. i + window_rows clipped to the image and
+ *     columns j - window_cols .. j + window_cols wrapped around the azimuth; "unknown" if any pixel of that window is empty.
+ *   - Vote of map row m at pose T (R (r, c) = T[4c + r], t = T[12 ..]): d = m - t, q_r = (R(0, r) d0 + R(1, r) d1) +
+ *     R(2, r) d2, r_m its range as above.  No vote if r_m is outside [min_range, max_range] or q is outside the image.
+ *     Else mg = max(margin_abs, margin_rel r_m); through += 1 iff the window value is known and > r_m + mg; hits += 1 iff
+ *     the centre pixel c is not empty and |c - r_m| <= mg.
+ *   - Rounding.  Every product, sum, quotient and square root is rounded on its own (no FMA), left to right as written, so
+ *     tests/map_dynamic_oracle.py reproduces every counter bit for bit.
+ *   - Decision.  A row is dynamic iff through >= min_through and through > hits.
+ *   - With correction.  tloam_b200_global_map_correct moves blocks and leaves their counters as they are; later votes see
+ *     the moved points.  Votes are not recomputed after a correction.
+ *   - The kernels live in libtloam_b200_gmd.so, loaded from this library's directory by the enable call; if it is missing
+ *     the calls return ERR_CUDA (tloam_b200_last_error names the file). */
+typedef struct tloam_global_map_dynamic_config {
+  int n_rows;                          /* range-image rows, 1 .. 1024 */
+  double fov_up;                       /* degrees, <= 90 */
+  double fov_down;                     /* degrees, >= -90, < fov_up */
+  int n_cols;                          /* range-image columns (azimuth sectors), 1 .. 16384 */
+  int window_rows;                     /* 0 .. n_rows - 1 */
+  int window_cols;                     /* >= 0, 2 window_cols + 1 <= n_cols */
+  double margin_abs;                   /* m, >= 0 */
+  double margin_rel;                   /* fraction of the range, >= 0 */
+  double min_range;                    /* m, > 0 */
+  double max_range;                    /* m, >= min_range */
+  int min_through;                     /* >= 1 */
+} tloam_global_map_dynamic_config;
+/* an HDL-64E at the map's 1 m voxel: n_rows 64, fov_up 2.0, fov_down -24.9, n_cols 1024, window_rows 1, window_cols 2,
+ * margin_abs 1.0 m, margin_rel 0.02, min_range 3 m, max_range 60 m, min_through 3 (DESIGN.md section 6 has how they were
+ * chosen) */
+void tloam_b200_global_map_dynamic_default_config(tloam_global_map_dynamic_config* c);
+/* NOT_READY: mapping off, or the map is not empty.  INVALID_ARG: cfg null, a value outside its range above, or a row
+ * table that is not non-decreasing. */
+int tloam_b200_global_map_dynamic_enable(tloam_b200_handle* h, const tloam_global_map_dynamic_config* cfg);
+/* the counters of map rows first .. first + count - 1 (either output may be null; synchronises).  NOT_READY: mapping or
+ * removal off.  INVALID_ARG past the last row. */
+int tloam_b200_global_map_votes_download(tloam_b200_handle* h, size_t first, size_t count, unsigned* through, unsigned* hits);
+/* the rows that are not dynamic, in map row order: xyz (*n x 3) and, when the map has an intensity channel, their intensity
+ * (intensity may be null; it is not written when the map has no channel).  A count, a scan and a scatter on the device,
+ * deterministic; synchronises.  *n is set first: INVALID_ARG when capacity < *n (or xyz null with *n > 0).  NOT_READY:
+ * mapping or removal off.  The map's sticky refusal flag is left for the next tloam_b200_global_map_size / _download. */
+int tloam_b200_global_map_static_download(tloam_b200_handle* h, double* xyz, double* intensity, size_t capacity, size_t* n);
+
 /* ---- Loop verification against a submap (opt-in, on top of loop verification): the query keyframe is aligned to the
  * keyframes of the loop frames around the candidate, moved into the candidate's sensor frame by their odometry poses, with
  * a point-to-plane residual.  One sparse keyframe leaves gaps between the sensor's rings that a point-to-point ICP locks

@@ -257,6 +257,43 @@ class FrontEndB200 {
     return report(tloam_b200_global_map_frame_poses(h_, first, count, odom, current), "globalMapFramePoses");
   }
 
+  // Dynamic-point removal (include/tloam_b200.h "Dynamic-point removal"): right after enableGlobalMap, every later
+  // updateGlobalMap* casts free-space votes on the map points before it; staticGlobalMap reads the map without the points
+  // later scans looked through.  The map globalMap returns is not changed.
+  bool enableDynamicRemoval(const tloam_global_map_dynamic_config& cfg) {
+    return report(tloam_b200_global_map_dynamic_enable(h_, &cfg), "enableDynamicRemoval");
+  }
+  bool enableDynamicRemoval() {
+    tloam_global_map_dynamic_config c;
+    tloam_b200_global_map_dynamic_default_config(&c);
+    return enableDynamicRemoval(c);
+  }
+  // the (through, hits) counters of map points first .. first + count - 1 (either may be null)
+  bool globalMapVotes(size_t first, size_t count, unsigned* through, unsigned* hits) {
+    return report(tloam_b200_global_map_votes_download(h_, first, count, through, hits), "globalMapVotes");
+  }
+  bool staticGlobalMap(std::vector<Eigen::Vector3d>& out) {
+    size_t n = 0;
+    const int rc = tloam_b200_global_map_static_download(h_, nullptr, nullptr, 0, &n);
+    if (rc != TLOAM_B200_ERR_INVALID_ARG && !report(rc, "staticGlobalMap")) return false;
+    out.resize(n);
+    return report(tloam_b200_global_map_static_download(h_, reinterpret_cast<double*>(out.data()), nullptr, n, &n),
+                  "staticGlobalMap");
+  }
+  // with the intensity of every kept point (empty when the map has no intensity channel)
+  bool staticGlobalMap(std::vector<Eigen::Vector3d>& out, std::vector<double>& intensity) {
+    intensity.clear();
+    int has = 0;
+    if (!report(tloam_b200_global_map_has_intensity(h_, &has), "staticGlobalMap")) return false;
+    size_t n = 0;
+    const int rc = tloam_b200_global_map_static_download(h_, nullptr, nullptr, 0, &n);
+    if (rc != TLOAM_B200_ERR_INVALID_ARG && !report(rc, "staticGlobalMap")) return false;
+    out.resize(n);
+    if (has) intensity.resize(n);
+    return report(tloam_b200_global_map_static_download(h_, reinterpret_cast<double*>(out.data()),
+                                                        has ? intensity.data() : nullptr, n, &n), "staticGlobalMap");
+  }
+
   // processCloud + setInputSource (ref: front_end.cpp:181-199, :313): the three clouds the segmentation nodelet publishes
   bool processCloud(CloudData& ground, CloudData& edge, CloudData& general) {
     return report(tloam_b200_process_cloud(h_, &fcfg_, ground_down_sample_, edge_down_sample_, data(ground), size(ground), data(edge),

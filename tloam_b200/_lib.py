@@ -82,6 +82,13 @@ class LoopVerifySubmapConfig(C.Structure):
                 ("max_fitness", C.c_double)]
 
 
+class GlobalMapDynamicConfig(C.Structure):
+    """tloam_global_map_dynamic_config (include/tloam_b200.h "Dynamic-point removal")."""
+    _fields_ = [("n_rows", C.c_int), ("fov_up", C.c_double), ("fov_down", C.c_double), ("n_cols", C.c_int),
+                ("window_rows", C.c_int), ("window_cols", C.c_int), ("margin_abs", C.c_double), ("margin_rel", C.c_double),
+                ("min_range", C.c_double), ("max_range", C.c_double), ("min_through", C.c_int)]
+
+
 class LoopVerifyResult(C.Structure):
     """tloam_loop_verify_result: T_cand_query (column-major) and the ICP's verdict."""
     _fields_ = [("query", C.c_longlong), ("candidate", C.c_longlong), ("T", C.c_double * 16), ("fitness", C.c_double),
@@ -223,6 +230,8 @@ EXPORTS = [
     "tloam_b200_global_map_correction_enable", "tloam_b200_global_map_correct", "tloam_b200_global_map_frame_poses",
     "tloam_b200_loop_verify_submap_default_config", "tloam_b200_loop_verify_submap_enable", "tloam_b200_loop_verify_submap",
     "tloam_b200_loop_verify_submap_target", "tloam_b200_loop_verify_submap_matches",
+    "tloam_b200_global_map_dynamic_default_config", "tloam_b200_global_map_dynamic_enable",
+    "tloam_b200_global_map_votes_download", "tloam_b200_global_map_static_download",
 ]
 
 _lib = None
@@ -417,5 +426,11 @@ def load():
     L.tloam_b200_loop_verify_submap.argtypes = [vp, C.c_longlong, C.c_longlong, dp, dp, C.POINTER(LoopVerifyResult)]
     L.tloam_b200_loop_verify_submap_target.argtypes = [vp, dp, dp, C.POINTER(C.c_ubyte), C.POINTER(C.c_int), C.c_size_t, szp]
     L.tloam_b200_loop_verify_submap_matches.argtypes = [vp, C.c_int, C.POINTER(C.c_int), dp, C.c_size_t, szp]
+    L.tloam_b200_global_map_dynamic_default_config.argtypes = [C.POINTER(GlobalMapDynamicConfig)]
+    L.tloam_b200_global_map_dynamic_default_config.restype = None
+    L.tloam_b200_global_map_dynamic_enable.argtypes = [vp, C.POINTER(GlobalMapDynamicConfig)]
+    up = C.POINTER(C.c_uint)
+    L.tloam_b200_global_map_votes_download.argtypes = [vp, C.c_size_t, C.c_size_t, up, up]
+    L.tloam_b200_global_map_static_download.argtypes = [vp, dp, dp, C.c_size_t, szp]
     _lib = L
     return L

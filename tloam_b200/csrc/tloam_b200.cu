@@ -35,6 +35,7 @@
 #include "pose_graph.h"
 #include "pose_graph_robust.h"
 #include "map_correct.h"
+#include "map_dynamic.h"
 
 
 
@@ -218,6 +219,14 @@ struct tloam_b200_handle {
   double* d_gmc_O = nullptr;               double* d_gmc_P = nullptr;   size_t cap_gmc = 0;
   double gmc_M[16];                        bool gmc_M_identity = true;
   unsigned char* d_gmc_scratch = nullptr;  size_t cap_gmc_scratch = 0;                         // node table, M_f, moved
+  // ---- dynamic-point removal (tloam_b200_global_map_dynamic*, libtloam_b200_gmd.so): two counters per map row with the
+  //      capacity of d_gmap (zero past the map's count), the range and window images, the row and column boundary tables ----
+  bool gmd_on = false;
+  tloam_global_map_dynamic_config gmd_cfg;
+  unsigned* d_gmd_through = nullptr;       unsigned* d_gmd_hits = nullptr;   size_t cap_gmd = 0;
+  unsigned long long* d_gmd_image = nullptr; double* d_gmd_window = nullptr; double* d_gmd_bounds = nullptr;
+  size_t cap_gmd_image = 0, cap_gmd_bounds = 0;
+  unsigned char* d_gmd_scratch = nullptr;  size_t cap_gmd_scratch = 0;                         // the static download
   // ---- the map's intensity channel (tloam_b200_global_map_*intensity*, libtloam_b200_gmi.so): allocated on the first
   //      intensity append; d_gmi_map has the capacity of d_gmap ----
   bool gmi_used = false;                   // an intensity frame was appended since enable / reset
@@ -475,6 +484,8 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   for (auto& pr : h->lv_probes) { if (pr.ev) cudaEventDestroy(pr.ev); if (pr.h_count) cudaFreeHost(pr.h_count); }
   cudaFree(h->d_pg_O); cudaFree(h->d_pg_scratch); cudaFree(h->d_pg_state);
   cudaFree(h->d_gmc_O); cudaFree(h->d_gmc_P); cudaFree(h->d_gmc_scratch);
+  cudaFree(h->d_gmd_through); cudaFree(h->d_gmd_hits); cudaFree(h->d_gmd_image); cudaFree(h->d_gmd_window);
+  cudaFree(h->d_gmd_bounds); cudaFree(h->d_gmd_scratch);
   for (int i = 0; i < 2; ++i) if (h->ev_stage_free[i]) cudaEventDestroy(h->ev_stage_free[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_fit[i]) cudaEventDestroy(h->ev_fit[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_res[i]) cudaEventDestroy(h->ev_res[i]);
@@ -3362,6 +3373,10 @@ static int gmap_clear(tloam_b200_handle* h) {
   h->gmi_used = false;                     // re-arms the intensity channel (the next intensity frame starts it afresh)
   for (int k = 0; k < 16; ++k) h->gmc_M[k] = k % 5 == 0 ? 1.0 : 0.0;
   h->gmc_M_identity = true;                // the pose tables are empty with the frame table; tracking stays as it is
+  if (h->gmd_on) {                         // every row starts at (0, 0); removal stays on
+    CU_TRY(cudaMemsetAsync(h->d_gmd_through, 0, h->cap_gmd * sizeof(unsigned), h->stream));
+    CU_TRY(cudaMemsetAsync(h->d_gmd_hits, 0, h->cap_gmd * sizeof(unsigned), h->stream));
+  }
   return TLOAM_B200_OK;
 }
 
@@ -3392,6 +3407,7 @@ int tloam_b200_global_map_enable(tloam_b200_handle* h, const tloam_global_map_co
   h->gmap_growths = 0;
   h->gmap_on = true;
   h->gmc_on = false;
+  h->gmd_on = false;
   return gmap_clear(h);
 }
 
@@ -3427,6 +3443,18 @@ static int gmap_grow(tloam_b200_handle* h, size_t n) {
       CU_TRY(cudaStreamSynchronize(h->stream));
       cudaFree(h->d_gmi_map);
       h->d_gmi_map = qi;
+    }
+    if (h->gmd_on) {                       // the removal counters grow with the map; rows past the count stay (0, 0)
+      for (unsigned** t : {&h->d_gmd_through, &h->d_gmd_hits}) {
+        unsigned* qt = nullptr;
+        CU_TRY(cudaMalloc(&qt, ncap * sizeof(unsigned)));
+        CU_TRY(cudaMemsetAsync(qt, 0, ncap * sizeof(unsigned), h->stream));
+        if (st.count) CU_TRY(cudaMemcpyAsync(qt, *t, st.count * sizeof(unsigned), cudaMemcpyDeviceToDevice, h->stream));
+        CU_TRY(cudaStreamSynchronize(h->stream));
+        cudaFree(*t);
+        *t = qt;
+      }
+      h->cap_gmd = ncap;
     }
   }
   if (h->gmap_calls + 2 > h->cap_gmap_off) {
@@ -3525,6 +3553,42 @@ static int gmc_status(tloam_b200_handle* h, int e, const char* where) {
   return TLOAM_B200_ERR_CUDA;
 }
 
+// ---- the removal's kernels live in libtloam_b200_gmd.so (map_dynamic.cu), next to this library: loaded by
+//      tloam_b200_global_map_dynamic_enable, so that the kernels of this library keep their SASS and an append with removal
+//      on cannot meet a missing library ----
+struct GmdLib { tloam_gmd_vote_fn vote = nullptr; tloam_gmd_static_blocks_fn blocks = nullptr; tloam_gmd_static_fn compact = nullptr; };
+static std::mutex g_gmd_mu;
+static GmdLib g_gmd;
+
+static int gmd_load(tloam_b200_handle* h, GmdLib* out) {
+  std::lock_guard<std::mutex> lk(g_gmd_mu);
+  if (!g_gmd.vote) {
+    const std::string path = sibling_path("libtloam_b200_gmd.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    GmdLib l;
+    if (so) {
+      l.vote = reinterpret_cast<tloam_gmd_vote_fn>(dlsym(so, "tloam_gmd_vote"));
+      l.blocks = reinterpret_cast<tloam_gmd_static_blocks_fn>(dlsym(so, "tloam_gmd_static_blocks"));
+      l.compact = reinterpret_cast<tloam_gmd_static_fn>(dlsym(so, "tloam_gmd_static"));
+    }
+    if (!l.vote || !l.blocks || !l.compact) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "global map dynamic removal: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_gmd = l;
+  }
+  *out = g_gmd;
+  return TLOAM_B200_OK;
+}
+
+static int gmd_status(tloam_b200_handle* h, int e, const char* where) {
+  if (e == cudaSuccess) return TLOAM_B200_OK;
+  snprintf(h->last_error, sizeof(h->last_error), "global map dynamic removal: %s: %s", where, cudaGetErrorString((cudaError_t)e));
+  return TLOAM_B200_ERR_CUDA;
+}
+
 // device buffers of an intensity frame of n rows (after gmap_grow: d_gmi_map takes the map's current capacity)
 static int gmi_prepare(tloam_b200_handle* h, const GmiLib& lib, size_t n) {
   if (!h->d_gmi_st) {
@@ -3589,6 +3653,23 @@ static int gmap_append_impl(tloam_b200_handle* h, const double* pose_host, const
                                                  h->gmc_M_identity ? nullptr : &M, h->device, h->stream)));
     if ((rc = gmc_status(h, e, "k_gmc_pose")) != TLOAM_B200_OK) return rc;
     d_pose = h->d_gmap_pose;
+  }
+  if (h->gmd_on && n) {                    // free-space votes of the sensor-frame rows (before the transform below) at the
+    GmdLib gmd;                            // block's pose, on the rows [0, count) present before this append
+    if ((rc = gmd_load(h, &gmd)) != TLOAM_B200_OK) return rc;
+    const tloam_global_map_dynamic_config& c = h->gmd_cfg;
+    tloam_gmd_vote_args a;
+    memset(&a, 0, sizeof(a));
+    a.p.n_rows = c.n_rows; a.p.n_cols = c.n_cols; a.p.wr = c.window_rows; a.p.wc = c.window_cols;
+    a.p.margin_abs = c.margin_abs; a.p.margin_rel = c.margin_rel; a.p.min_range = c.min_range; a.p.max_range = c.max_range;
+    a.p.row_bounds = h->d_gmd_bounds; a.p.col_bounds = h->d_gmd_bounds + (c.n_rows + 1);
+    a.scan = d_in; a.n = (unsigned)n; a.pose = d_pose; a.map = h->d_gmap; a.count = &st->count;
+    a.through = h->d_gmd_through; a.hits = h->d_gmd_hits; a.image = h->d_gmd_image; a.window = h->d_gmd_window;
+    a.device = h->device; a.stream = h->stream;
+    int launches = 0, e = 0;
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = gmd.vote(&a, &launches)));
+    h->launches += launches > 0 ? launches - 1 : 0;
+    if ((rc = gmd_status(h, e, "k_gmd_vote")) != TLOAM_B200_OK) return rc;
   }
   CU_TRY(cudaMemsetAsync(&st->n_fin, 0, sizeof(GMapState) - offsetof(GMapState, n_fin), h->stream));
   const unsigned tb = 256, gb = (unsigned)((n + tb - 1) / tb);
@@ -4854,6 +4935,146 @@ int tloam_b200_global_map_frame_poses(tloam_b200_handle* h, size_t first, size_t
     CU_TRY(cudaMemcpyAsync(odom, h->d_gmc_O + 16 * first, count * 16 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   if (count && current)
     CU_TRY(cudaMemcpyAsync(current, h->d_gmc_P + 16 * first, count * 16 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Dynamic-point removal (the counters, images and tables here and in gmap_append_impl / gmap_grow / gmap_clear; the kernels
+// in map_dynamic.cu, loaded from libtloam_b200_gmd.so when removal is enabled).
+// ---------------------------------------------------------------------------------------------
+void tloam_b200_global_map_dynamic_default_config(tloam_global_map_dynamic_config* c) {
+  c->n_rows = 64; c->fov_up = 2.0; c->fov_down = -24.9; c->n_cols = 1024;   // an HDL-64E at the map's 1 m voxel
+  c->window_rows = 1; c->window_cols = 2;
+  c->margin_abs = 1.0; c->margin_rel = 0.02;
+  c->min_range = 3.0; c->max_range = 60.0;
+  c->min_through = 3;
+}
+
+static bool gmd_config_valid(const tloam_global_map_dynamic_config* c) {
+  const auto fin = [](double v) { return std::isfinite(v); };
+  if (c->n_rows < 1 || c->n_rows > 1024 || c->n_cols < 1 || c->n_cols > 16384) return false;
+  if (!fin(c->fov_up) || !fin(c->fov_down) || !(c->fov_down < c->fov_up) || c->fov_down < -90.0 || c->fov_up > 90.0) return false;
+  if (c->window_rows < 0 || c->window_rows >= c->n_rows || c->window_cols < 0 || 2 * c->window_cols + 1 > c->n_cols) return false;
+  if (!fin(c->margin_abs) || !(c->margin_abs >= 0.0) || !fin(c->margin_rel) || !(c->margin_rel >= 0.0)) return false;
+  if (!fin(c->min_range) || !fin(c->max_range) || !(c->min_range > 0.0) || !(c->min_range <= c->max_range)) return false;
+  return c->min_through >= 1;
+}
+
+int tloam_b200_global_map_dynamic_enable(tloam_b200_handle* h, const tloam_global_map_dynamic_config* cfg) {
+  if (!h || !cfg) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!gmd_config_valid(cfg)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on || h->gmap_calls != 0) return TLOAM_B200_ERR_NOT_READY;
+  GmdLib lib;
+  int rc = gmd_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  // the host tables: b_k = sin(lo + k (hi - lo) / n_rows) and Scan Context's sector boundaries (cos, sin of 2 pi k / n_cols)
+  std::vector<double> tab((size_t)(cfg->n_rows + 1) + 2 * (size_t)(cfg->n_cols - 1));
+  const double lo = cfg->fov_down * (M_PI / 180.0), hi = cfg->fov_up * (M_PI / 180.0);
+  for (int k = 0; k <= cfg->n_rows; ++k) tab[k] = std::sin(lo + k * (hi - lo) / cfg->n_rows);
+  for (int k = 1; k <= cfg->n_rows; ++k)
+    if (!(tab[k] >= tab[k - 1])) return TLOAM_B200_ERR_INVALID_ARG;     // the row search needs a non-decreasing table
+  double* dirs = tab.data() + (cfg->n_rows + 1);
+  for (int k = 1; k < cfg->n_cols; ++k) {
+    const double t = 2.0 * M_PI * k / cfg->n_cols;
+    dirs[2 * (k - 1)] = std::cos(t);
+    dirs[2 * (k - 1) + 1] = std::sin(t);
+  }
+  if (tab.size() > h->cap_gmd_bounds) {
+    cudaFree(h->d_gmd_bounds); h->d_gmd_bounds = nullptr; h->cap_gmd_bounds = 0;
+    CU_TRY(cudaMalloc(&h->d_gmd_bounds, tab.size() * sizeof(double)));
+    h->cap_gmd_bounds = tab.size();
+  }
+  CU_TRY(cudaMemcpy(h->d_gmd_bounds, tab.data(), tab.size() * sizeof(double), cudaMemcpyHostToDevice));
+  const size_t pix = (size_t)cfg->n_rows * cfg->n_cols;
+  if (pix > h->cap_gmd_image) {
+    cudaFree(h->d_gmd_image); cudaFree(h->d_gmd_window); h->d_gmd_image = nullptr; h->d_gmd_window = nullptr;
+    h->cap_gmd_image = 0;
+    CU_TRY(cudaMalloc(&h->d_gmd_image, pix * sizeof(unsigned long long)));
+    CU_TRY(cudaMalloc(&h->d_gmd_window, pix * sizeof(double)));
+    h->cap_gmd_image = pix;
+  }
+  if (h->cap_gmd != h->cap_gmap) {
+    cudaFree(h->d_gmd_through); cudaFree(h->d_gmd_hits); h->d_gmd_through = h->d_gmd_hits = nullptr; h->cap_gmd = 0;
+    CU_TRY(cudaMalloc(&h->d_gmd_through, h->cap_gmap * sizeof(unsigned)));
+    CU_TRY(cudaMalloc(&h->d_gmd_hits, h->cap_gmap * sizeof(unsigned)));
+    h->cap_gmd = h->cap_gmap;
+  }
+  CU_TRY(cudaMemsetAsync(h->d_gmd_through, 0, h->cap_gmd * sizeof(unsigned), h->stream));
+  CU_TRY(cudaMemsetAsync(h->d_gmd_hits, 0, h->cap_gmd * sizeof(unsigned), h->stream));
+  h->gmd_cfg = *cfg;
+  h->gmd_on = true;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_global_map_votes_download(tloam_b200_handle* h, size_t first, size_t count, unsigned* through, unsigned* hits) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on || !h->gmd_on) return TLOAM_B200_ERR_NOT_READY;
+  GMapState st;
+  int rc = gmc_read(h, &st);
+  if (rc != TLOAM_B200_OK) return rc;
+  if (first > st.count || count > st.count - first) return TLOAM_B200_ERR_INVALID_ARG;
+  if (count && through)
+    CU_TRY(cudaMemcpyAsync(through, h->d_gmd_through + first, count * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+  if (count && hits)
+    CU_TRY(cudaMemcpyAsync(hits, h->d_gmd_hits + first, count * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_global_map_static_download(tloam_b200_handle* h, double* xyz, double* intensity, size_t capacity, size_t* n) {
+  if (!h || !n) return TLOAM_B200_ERR_INVALID_ARG;
+  *n = 0;
+  if (!h->gmap_on || !h->gmd_on) return TLOAM_B200_ERR_NOT_READY;
+  GmdLib lib;
+  int rc = gmd_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  GMapState st;
+  if ((rc = gmc_read(h, &st)) != TLOAM_B200_OK) return rc;   // the sticky flags stay for the next size / download call
+  bool has = false;                                           // the map has the intensity channel (gmi_read's rule)
+  if (h->gmi_used && st.count) {
+    unsigned s0 = 0;
+    CU_TRY(cudaMemcpyAsync(&s0, h->d_gmi_st, sizeof(s0), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    has = s0 != 0u;
+  }
+  const size_t count = st.count;
+  const unsigned blocks = lib.blocks(count);
+  size_t o = 0;
+  auto take = [&](size_t bytes) { const size_t at = o; o += round_up(bytes, 256); return at; };
+  const size_t o_blocks = take((size_t)blocks * sizeof(unsigned)), o_total = take(sizeof(unsigned long long));
+  const size_t o_xyz = take(count * 3 * sizeof(double)), o_int = take(has ? count * sizeof(double) : 0);
+  if (o > h->cap_gmd_scratch) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_gmd_scratch); h->d_gmd_scratch = nullptr; h->cap_gmd_scratch = 0;
+    CU_TRY(cudaMalloc(&h->d_gmd_scratch, o + o / 2));
+    h->cap_gmd_scratch = o + o / 2;
+  }
+  unsigned char* base = h->d_gmd_scratch;
+  tloam_gmd_static_args a;
+  memset(&a, 0, sizeof(a));
+  a.map = h->d_gmap; a.intensity = has ? h->d_gmi_map : nullptr;
+  a.through = h->d_gmd_through; a.hits = h->d_gmd_hits;
+  a.count = count; a.min_through = (unsigned)h->gmd_cfg.min_through;
+  a.block_counts = reinterpret_cast<unsigned*>(base + o_blocks);
+  a.total = reinterpret_cast<unsigned long long*>(base + o_total);
+  a.out_xyz = reinterpret_cast<double*>(base + o_xyz);
+  a.out_intensity = has ? reinterpret_cast<double*>(base + o_int) : nullptr;
+  a.device = h->device; a.stream = h->stream;
+  int e = 0, launches = 0;
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.compact(&a, &launches)));
+  h->launches += launches > 0 ? launches - 1 : 0;
+  if ((rc = gmd_status(h, e, "k_gmd_count / k_gmd_scatter")) != TLOAM_B200_OK) return rc;
+  unsigned long long total = 0;
+  CU_TRY(cudaMemcpyAsync(&total, a.total, sizeof(total), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  *n = (size_t)total;
+  if (capacity < *n || (!xyz && *n)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (*n) CU_TRY(cudaMemcpyAsync(xyz, a.out_xyz, *n * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (*n && intensity && has)
+    CU_TRY(cudaMemcpyAsync(intensity, a.out_intensity, *n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   CU_TRY(cudaStreamSynchronize(h->stream));
   return TLOAM_B200_OK;
 }

@@ -1068,6 +1068,44 @@ class LocalRegistration:
                     "global_map_frame_poses")
         return tuple(x.reshape(count, 4, 4).transpose(0, 2, 1).copy() for x in (o, c))
 
+    # ---- dynamic-point removal (include/tloam_b200.h "Dynamic-point removal") ----
+    def global_map_dynamic_enable(self, **overrides):
+        """free-space votes from every later append on the map rows before it (only on an empty map); overrides: fields of
+        tloam_global_map_dynamic_config (n_rows, fov_up, fov_down, n_cols, window_rows, window_cols, margin_abs,
+        margin_rel, min_range, max_range, min_through)"""
+        cfg = _lib.GlobalMapDynamicConfig()
+        self._L.tloam_b200_global_map_dynamic_default_config(C.byref(cfg))
+        for k, v in overrides.items():
+            if not any(f[0] == k for f in cfg._fields_):
+                raise TypeError(f"unknown dynamic-removal field {k!r}")
+            setattr(cfg, k, v)
+        self._check(self._L.tloam_b200_global_map_dynamic_enable(self._h, C.byref(cfg)), "global_map_dynamic_enable")
+
+    def global_map_votes(self, first=0, count=None):
+        """(through, hits) of map rows [first, first + count), uint32 each"""
+        if count is None:
+            count = self.global_map_size()[0] - first
+        if first < 0 or count < 0:
+            raise RegistrationError(_lib.ERR_INVALID_ARG, "global_map_votes_download")
+        t, h = np.zeros(count, dtype=np.uint32), np.zeros(count, dtype=np.uint32)
+        up = C.POINTER(C.c_uint)
+        self._check(self._L.tloam_b200_global_map_votes_download(self._h, int(first), int(count), t.ctypes.data_as(up),
+                                                                 h.ctypes.data_as(up)), "global_map_votes_download")
+        return t, h
+
+    def global_map_static(self):
+        """(xyz (n, 3), intensity (n,) or None): the map rows not judged dynamic, in row order"""
+        n = C.c_size_t(0)
+        rc = self._L.tloam_b200_global_map_static_download(self._h, None, None, 0, C.byref(n))
+        if rc != _lib.ERR_INVALID_ARG or n.value == 0:
+            self._check(rc, "global_map_static_download")
+        has = self.global_map_has_intensity()
+        xyz = np.zeros((n.value, 3))
+        inten = np.zeros(n.value) if has else None
+        self._check(self._L.tloam_b200_global_map_static_download(self._h, _dp(xyz), _dp(inten) if has else None, n.value,
+                                                                  C.byref(n)), "global_map_static_download")
+        return xyz[:n.value], (inten[:n.value] if has else None)
+
     # ---- shared map (multi-GPU) ----
     def map_blob_size(self):
         n = C.c_size_t(0)
