@@ -58,7 +58,8 @@ typedef enum tloam_b200_status {
   TLOAM_B200_ERR_NOT_READY = 6,      /* scan_match before set_source / set_target */
   TLOAM_B200_ERR_NUMERIC = 7,        /* non-finite value met inside the solve */
   TLOAM_B200_ERR_MAP_DENSITY = 8,    /* a map cell (edge = search radius) holds more than 65535 points */
-  TLOAM_B200_ERR_VOXEL_RANGE = 9     /* a global-map frame spans 2^21 or more voxels on an axis (voxel too small): not appended */
+  TLOAM_B200_ERR_VOXEL_RANGE = 9     /* a global-map frame, or the map being merged, spans 2^21 or more voxels on an axis
+                                        (voxel too small): the frame is not appended, the merge produces nothing */
 } tloam_b200_status;
 
 /* The "TLS:" YAML block (ref: config/mapping/lidar_odometry.yaml:23-39, read at registration.cpp:212-230)
@@ -974,6 +975,47 @@ int tloam_b200_global_map_votes_download(tloam_b200_handle* h, size_t first, siz
  * deterministic; synchronises.  *n is set first: INVALID_ARG when capacity < *n (or xyz null with *n > 0).  NOT_READY:
  * mapping or removal off.  The map's sticky refusal flag is left for the next tloam_b200_global_map_size / _download. */
 int tloam_b200_global_map_static_download(tloam_b200_handle* h, double* xyz, double* intensity, size_t capacity, size_t* n);
+
+/* ---- Merged global map: the map's frames merged into one voxel grid, the map a user publishes or saves.  The map is a
+ * concatenation of per-frame down-samples, so every place several frames saw appears once per frame; the merge is
+ * VoxelDownSample of the whole map (ref: src/open3d/PointCloud2.cpp:358-403), after correction and, optionally, without
+ * the rows dynamic-point removal judges dynamic.
+ *   - Input cloud C.  The map as it stands in stream order, after every enqueued append and correction: all rows in map
+ *     row order, or with static_only the rows tloam_b200_global_map_static_download keeps (through >= min_through and
+ *     through > hits is dynamic), still in map row order.
+ *   - Bounds.  mb = min(C) - voxel * 0.5 per axis: voxel * 0.5 rounded on its own, then the subtraction.
+ *   - Index.  floor((p - mb) / voxel) per axis, the subtraction and the division each rounded on its own (no FMA); every
+ *     index is >= 0.
+ *   - Key range.  If the index of the max row reaches 2^21 on an axis ((max - mb) / voxel >= 2^21, the limit the frame
+ *     appends use), the merge refuses with TLOAM_B200_ERR_VOXEL_RANGE and produces nothing.  The reference's limit is
+ *     INT_MAX (it logs "voxel_size is too small").  A selected row with a NaN or infinite coordinate, which no append
+ *     produces, has an infinite extent and is refused the same way.
+ *   - Averages (AccumulatedPoint, :246-294).  x, y, z and, when the map has a channel, the intensity are each summed with
+ *     += over the voxel's rows in ascending row order, from +0.0, then divided by (double)count.  Every operation is
+ *     rounded on its own; NaN and Inf intensities propagate.  tests/global_map_merge_oracle.py restates it bit for bit.
+ *   - Order.  Voxels in ascending (ix, iy, iz), the order of the per-frame blocks (the reference iterates an
+ *     unordered_map: its order is implementation-defined).
+ *   - Intensity.  The merged cloud has a channel iff the map has one at merge time (tloam_b200_global_map_has_intensity).
+ *   - Nothing else moves: the map, the frame table, the intensity channel, the vote counters, the pose tables, the
+ *     registered scan, the keyframes, the pose graph and the odometry keep every bit.  The map's sticky refusal flag is
+ *     left for the next tloam_b200_global_map_size / _download.
+ *   - Snapshot.  The result stays on the device until the next merge (a refused merge leaves none),
+ *     tloam_b200_global_map_reset or tloam_b200_global_map_enable.
+ *   - Device.  A bounds pass (one small read-back), one key per row, a stable LSD radix sort on 8-bit digits
+ *     (ceil((bits of ix + iy + iz, + 1 with static_only) / 8) passes), a scan of the voxel heads and one thread per voxel;
+ *     three synchronisations.  Scratch: 24 B per map row (two key / row-index buffers) plus 1 KiB per 2 048 rows of
+ *     radix histograms; output: 32 B per voxel (xyz and intensity).  Both are allocated by the first merge with half as
+ *     much again, grow only and are freed by tloam_b200_destroy; a handle that never merges allocates and launches nothing
+ *     for it.
+ *   - The kernels live in libtloam_b200_gmm.so, loaded from this library's directory by the first merge; if it is missing
+ *     the calls return ERR_CUDA (tloam_b200_last_error names the file). */
+/* builds the merged cloud and sets *n_voxels; synchronises.  NOT_READY: mapping off, or static_only with removal off.
+ * INVALID_ARG: n_voxels null, voxel <= 0 or not finite.  VOXEL_RANGE: extent >= 2^21 voxels on an axis (*n_voxels = 0).
+ * An empty selection gives 0 voxels and OK. */
+int tloam_b200_global_map_merge(tloam_b200_handle* h, double voxel, int static_only, size_t* n_voxels);
+/* voxels [first, first + count) of the last merge: xyz (count x 3) and, when it has a channel, intensity (may be null; not
+ * written without a channel).  Synchronises.  NOT_READY: no merge since enable / reset.  INVALID_ARG past the end. */
+int tloam_b200_global_map_merged_download(tloam_b200_handle* h, size_t first, size_t count, double* xyz, double* intensity);
 
 /* ---- Loop verification against a submap (opt-in, on top of loop verification): the query keyframe is aligned to the
  * keyframes of the loop frames around the candidate, moved into the candidate's sensor frame by their odometry poses, with

@@ -294,6 +294,28 @@ class FrontEndB200 {
                                                         has ? intensity.data() : nullptr, n, &n), "staticGlobalMap");
   }
 
+  // The merged map (include/tloam_b200.h "Merged global map"): the whole map, or with static_only the points
+  // staticGlobalMap keeps, merged into one voxel grid -- VoxelDownSample(voxel) of the map, the cloud to publish or save.
+  bool mergedGlobalMap(double voxel, bool static_only, std::vector<Eigen::Vector3d>& out) {
+    size_t n = 0;
+    if (!report(tloam_b200_global_map_merge(h_, voxel, static_only ? 1 : 0, &n), "mergedGlobalMap")) return false;
+    out.resize(n);
+    return report(tloam_b200_global_map_merged_download(h_, 0, n, reinterpret_cast<double*>(out.data()), nullptr),
+                  "mergedGlobalMap");
+  }
+  // with the average intensity of every voxel (empty when the map has no intensity channel)
+  bool mergedGlobalMap(double voxel, bool static_only, std::vector<Eigen::Vector3d>& out, std::vector<double>& intensity) {
+    intensity.clear();
+    size_t n = 0;
+    if (!report(tloam_b200_global_map_merge(h_, voxel, static_only ? 1 : 0, &n), "mergedGlobalMap")) return false;
+    int has = 0;
+    if (!report(tloam_b200_global_map_has_intensity(h_, &has), "mergedGlobalMap")) return false;
+    out.resize(n);
+    if (has) intensity.resize(n);
+    return report(tloam_b200_global_map_merged_download(h_, 0, n, reinterpret_cast<double*>(out.data()),
+                                                        has ? intensity.data() : nullptr), "mergedGlobalMap");
+  }
+
   // processCloud + setInputSource (ref: front_end.cpp:181-199, :313): the three clouds the segmentation nodelet publishes
   bool processCloud(CloudData& ground, CloudData& edge, CloudData& general) {
     return report(tloam_b200_process_cloud(h_, &fcfg_, ground_down_sample_, edge_down_sample_, data(ground), size(ground), data(edge),

@@ -232,6 +232,7 @@ EXPORTS = [
     "tloam_b200_loop_verify_submap_target", "tloam_b200_loop_verify_submap_matches",
     "tloam_b200_global_map_dynamic_default_config", "tloam_b200_global_map_dynamic_enable",
     "tloam_b200_global_map_votes_download", "tloam_b200_global_map_static_download",
+    "tloam_b200_global_map_merge", "tloam_b200_global_map_merged_download",
 ]
 
 _lib = None
@@ -432,5 +433,7 @@ def load():
     up = C.POINTER(C.c_uint)
     L.tloam_b200_global_map_votes_download.argtypes = [vp, C.c_size_t, C.c_size_t, up, up]
     L.tloam_b200_global_map_static_download.argtypes = [vp, dp, dp, C.c_size_t, szp]
+    L.tloam_b200_global_map_merge.argtypes = [vp, C.c_double, C.c_int, szp]
+    L.tloam_b200_global_map_merged_download.argtypes = [vp, C.c_size_t, C.c_size_t, dp, dp]
     _lib = L
     return L

@@ -36,6 +36,7 @@
 #include "pose_graph_robust.h"
 #include "map_correct.h"
 #include "map_dynamic.h"
+#include "map_merge.h"
 
 
 
@@ -227,6 +228,12 @@ struct tloam_b200_handle {
   unsigned long long* d_gmd_image = nullptr; double* d_gmd_window = nullptr; double* d_gmd_bounds = nullptr;
   size_t cap_gmd_image = 0, cap_gmd_bounds = 0;
   unsigned char* d_gmd_scratch = nullptr;  size_t cap_gmd_scratch = 0;                         // the static download
+  // ---- the merged map (tloam_b200_global_map_merge*, libtloam_b200_gmm.so): the radix sort's scratch (24 B per map row)
+  //      and the last merge's voxels (32 B each), allocated by the first merge and grown; the snapshot is dropped by
+  //      enable / reset and by the next merge ----
+  unsigned char* d_gmm_scratch = nullptr;  size_t cap_gmm_scratch = 0;
+  double* d_gmm_out = nullptr;             size_t cap_gmm_out = 0;                             // n x 3 xyz, then n intensity
+  bool gmm_valid = false;                  bool gmm_has = false;   size_t gmm_n = 0;
   // ---- the map's intensity channel (tloam_b200_global_map_*intensity*, libtloam_b200_gmi.so): allocated on the first
   //      intensity append; d_gmi_map has the capacity of d_gmap ----
   bool gmi_used = false;                   // an intensity frame was appended since enable / reset
@@ -486,6 +493,7 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   cudaFree(h->d_gmc_O); cudaFree(h->d_gmc_P); cudaFree(h->d_gmc_scratch);
   cudaFree(h->d_gmd_through); cudaFree(h->d_gmd_hits); cudaFree(h->d_gmd_image); cudaFree(h->d_gmd_window);
   cudaFree(h->d_gmd_bounds); cudaFree(h->d_gmd_scratch);
+  cudaFree(h->d_gmm_scratch); cudaFree(h->d_gmm_out);
   for (int i = 0; i < 2; ++i) if (h->ev_stage_free[i]) cudaEventDestroy(h->ev_stage_free[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_fit[i]) cudaEventDestroy(h->ev_fit[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_res[i]) cudaEventDestroy(h->ev_res[i]);
@@ -3373,6 +3381,7 @@ static int gmap_clear(tloam_b200_handle* h) {
   h->gmi_used = false;                     // re-arms the intensity channel (the next intensity frame starts it afresh)
   for (int k = 0; k < 16; ++k) h->gmc_M[k] = k % 5 == 0 ? 1.0 : 0.0;
   h->gmc_M_identity = true;                // the pose tables are empty with the frame table; tracking stays as it is
+  h->gmm_valid = false;                    // the merged snapshot belonged to the map before
   if (h->gmd_on) {                         // every row starts at (0, 0); removal stays on
     CU_TRY(cudaMemsetAsync(h->d_gmd_through, 0, h->cap_gmd * sizeof(unsigned), h->stream));
     CU_TRY(cudaMemsetAsync(h->d_gmd_hits, 0, h->cap_gmd * sizeof(unsigned), h->stream));
@@ -5075,6 +5084,141 @@ int tloam_b200_global_map_static_download(tloam_b200_handle* h, double* xyz, dou
   if (*n) CU_TRY(cudaMemcpyAsync(xyz, a.out_xyz, *n * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   if (*n && intensity && has)
     CU_TRY(cudaMemcpyAsync(intensity, a.out_intensity, *n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Merged global map (the checks, the key range and the buffers here; the kernels in map_merge.cu, loaded from
+// libtloam_b200_gmm.so by the first merge, so that the kernels of this library keep their SASS).
+// ---------------------------------------------------------------------------------------------
+struct GmmLib {
+  tloam_gmm_scratch_bytes_fn scratch_bytes = nullptr; tloam_gmm_state_of_fn state_of = nullptr;
+  tloam_gmm_launch_fn bounds = nullptr, sort = nullptr, average = nullptr;
+};
+static std::mutex g_gmm_mu;
+static GmmLib g_gmm;
+
+static int gmm_load(tloam_b200_handle* h, GmmLib* out) {
+  std::lock_guard<std::mutex> lk(g_gmm_mu);
+  if (!g_gmm.bounds) {
+    const std::string path = sibling_path("libtloam_b200_gmm.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    GmmLib l;
+    if (so) {
+      l.scratch_bytes = reinterpret_cast<tloam_gmm_scratch_bytes_fn>(dlsym(so, "tloam_gmm_scratch_bytes"));
+      l.state_of = reinterpret_cast<tloam_gmm_state_of_fn>(dlsym(so, "tloam_gmm_state_of"));
+      l.bounds = reinterpret_cast<tloam_gmm_launch_fn>(dlsym(so, "tloam_gmm_bounds"));
+      l.sort = reinterpret_cast<tloam_gmm_launch_fn>(dlsym(so, "tloam_gmm_sort"));
+      l.average = reinterpret_cast<tloam_gmm_launch_fn>(dlsym(so, "tloam_gmm_average"));
+    }
+    if (!l.scratch_bytes || !l.state_of || !l.bounds || !l.sort || !l.average) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "global map merge: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_gmm = l;
+  }
+  *out = g_gmm;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_global_map_merge(tloam_b200_handle* h, double voxel, int static_only, size_t* n_voxels) {
+  if (!h || !n_voxels) return TLOAM_B200_ERR_INVALID_ARG;
+  *n_voxels = 0;
+  if (!(voxel > 0.0) || !std::isfinite(voxel)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on || (static_only && !h->gmd_on)) return TLOAM_B200_ERR_NOT_READY;
+  GmmLib lib;
+  int rc = gmm_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  h->gmm_valid = false;                                       // a refused merge leaves no snapshot
+  GMapState st;
+  if ((rc = gmc_read(h, &st)) != TLOAM_B200_OK) return rc;   // the sticky flags stay for the next size / download call
+  const size_t count = st.count;
+  if (count >> 32) {                                          // the sort's row payload is a u32 (2^32 rows: 103 GB of xyz)
+    snprintf(h->last_error, sizeof(h->last_error), "global map merge: %zu rows do not fit a 32-bit row index", count);
+    return TLOAM_B200_ERR_CUDA;
+  }
+  bool has = false;                                           // the map has the intensity channel (gmi_read's rule)
+  if (h->gmi_used && count) {
+    unsigned s0 = 0;
+    CU_TRY(cudaMemcpyAsync(&s0, h->d_gmi_st, sizeof(s0), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    has = s0 != 0u;
+  }
+  size_t n_vox = 0;
+  if (count) {
+    const size_t bytes = lib.scratch_bytes(count);
+    if (bytes > h->cap_gmm_scratch) {
+      CU_TRY(cudaStreamSynchronize(h->stream));
+      cudaFree(h->d_gmm_scratch); h->d_gmm_scratch = nullptr; h->cap_gmm_scratch = 0;
+      CU_TRY(cudaMalloc(&h->d_gmm_scratch, bytes + bytes / 2));
+      h->cap_gmm_scratch = bytes + bytes / 2;
+    }
+    tloam_gmm_args a;
+    memset(&a, 0, sizeof(a));
+    a.map = h->d_gmap; a.intensity = has ? h->d_gmi_map : nullptr;
+    if (static_only) { a.through = h->d_gmd_through; a.hits = h->d_gmd_hits; a.min_through = (unsigned)h->gmd_cfg.min_through; }
+    a.count = count; a.voxel = voxel;
+    a.scratch = h->d_gmm_scratch; a.state = lib.state_of(h->d_gmm_scratch, count);
+    a.device = h->device; a.stream = h->stream;
+    auto run = [&](tloam_gmm_launch_fn f, const char* where) -> int {
+      int e = 0, launches = 0;
+      TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = f(&a, &launches)));
+      h->launches += launches > 0 ? launches - 1 : 0;
+      if (e == cudaSuccess) return TLOAM_B200_OK;
+      snprintf(h->last_error, sizeof(h->last_error), "global map merge: %s: %s", where, cudaGetErrorString((cudaError_t)e));
+      return TLOAM_B200_ERR_CUDA;
+    };
+    if ((rc = run(lib.bounds, "k_gmm_bounds")) != TLOAM_B200_OK) return rc;
+    tloam_gmm_state gs;
+    CU_TRY(cudaMemcpyAsync(&gs, a.state, sizeof(gs), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    if (gs.nonfinite) return TLOAM_B200_ERR_VOXEL_RANGE;        // an infinite extent (no append produces such a row)
+    if (gs.n_sel) {
+      // voxel_min_bound = min - voxel * 0.5 (ref: PointCloud2.cpp:367); the max row has the largest index per axis, as in
+      // k_gmap_guard, and fixes the bits of that axis in the key
+      for (int d = 0; d < 3; ++d) {
+        const double half = voxel * 0.5;
+        a.mb[d] = dec_ordered(~gs.lo[d]) - half;
+        const double ref = (dec_ordered(gs.hi[d]) - a.mb[d]) / voxel;
+        if (!(ref < (double)(1u << kGMapKeyBits))) return TLOAM_B200_ERR_VOXEL_RANGE;
+        const unsigned long long top = (unsigned long long)std::floor(ref);
+        int bits = 0;
+        while (bits < 64 && (top >> bits)) ++bits;
+        a.bits[d] = bits;
+      }
+      a.n_sel = gs.n_sel;
+      if ((rc = run(lib.sort, "k_gmm_keys / k_gmm_hist / k_gmm_offsets / k_gmm_scatter / k_gmm_head_*")) != TLOAM_B200_OK) return rc;
+      unsigned long long nv = 0;
+      CU_TRY(cudaMemcpyAsync(&nv, &a.state->n_vox, sizeof(nv), cudaMemcpyDeviceToHost, h->stream));
+      CU_TRY(cudaStreamSynchronize(h->stream));
+      n_vox = (size_t)nv;
+      if (4 * n_vox > h->cap_gmm_out) {
+        cudaFree(h->d_gmm_out); h->d_gmm_out = nullptr; h->cap_gmm_out = 0;
+        CU_TRY(cudaMalloc(&h->d_gmm_out, (4 * n_vox + 2 * n_vox) * sizeof(double)));
+        h->cap_gmm_out = 4 * n_vox + 2 * n_vox;
+      }
+      a.n_vox = nv; a.out_xyz = h->d_gmm_out; a.out_intensity = has ? h->d_gmm_out + 3 * n_vox : nullptr;
+      if ((rc = run(lib.average, "k_gmm_average")) != TLOAM_B200_OK) return rc;
+      CU_TRY(cudaStreamSynchronize(h->stream));
+    }
+  }
+  h->gmm_n = n_vox; h->gmm_has = has; h->gmm_valid = true;
+  *n_voxels = n_vox;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_global_map_merged_download(tloam_b200_handle* h, size_t first, size_t count, double* xyz, double* intensity) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmm_valid) return TLOAM_B200_ERR_NOT_READY;
+  if (first > h->gmm_n || count > h->gmm_n - first || (count && !xyz)) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  const size_t n = h->gmm_n;
+  if (count) CU_TRY(cudaMemcpyAsync(xyz, h->d_gmm_out + 3 * first, count * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (count && intensity && h->gmm_has)
+    CU_TRY(cudaMemcpyAsync(intensity, h->d_gmm_out + 3 * n + first, count * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   CU_TRY(cudaStreamSynchronize(h->stream));
   return TLOAM_B200_OK;
 }

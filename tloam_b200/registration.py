@@ -693,6 +693,7 @@ class LocalRegistration:
         """start an empty map: every appended raw scan is transformed, VoxelDownSample(voxel)'d on its own and concatenated"""
         cfg = _lib.GlobalMapConfig(float(voxel), int(initial_capacity))
         self._check(self._L.tloam_b200_global_map_enable(self._h, C.byref(cfg)), "global_map_enable")
+        self._global_map_voxel = float(voxel)                          # global_map_merged's default
 
     def reset_global_map(self):
         self._check(self._L.tloam_b200_global_map_reset(self._h), "global_map_reset")
@@ -1105,6 +1106,20 @@ class LocalRegistration:
         self._check(self._L.tloam_b200_global_map_static_download(self._h, _dp(xyz), _dp(inten) if has else None, n.value,
                                                                   C.byref(n)), "global_map_static_download")
         return xyz[:n.value], (inten[:n.value] if has else None)
+
+    # ---- merged global map (include/tloam_b200.h "Merged global map") ----
+    def global_map_merged(self, voxel=None, static=False):
+        """(xyz (n, 3), intensity (n,) or None): the map (or with static=True its rows not judged dynamic) merged into one
+        voxel grid, VoxelDownSample(voxel) of the whole map, voxels in ascending (ix, iy, iz).  voxel=None: the map's own"""
+        v = getattr(self, "_global_map_voxel", 1.0) if voxel is None else float(voxel)
+        n = C.c_size_t(0)
+        self._check(self._L.tloam_b200_global_map_merge(self._h, v, 1 if static else 0, C.byref(n)), "global_map_merge")
+        has = self.global_map_has_intensity()
+        xyz = np.zeros((n.value, 3))
+        inten = np.zeros(n.value) if has else None
+        self._check(self._L.tloam_b200_global_map_merged_download(self._h, 0, n.value, _dp(xyz), _dp(inten) if has else None),
+                    "global_map_merged_download")
+        return xyz, inten
 
     # ---- shared map (multi-GPU) ----
     def map_blob_size(self):
