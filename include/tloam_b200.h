@@ -1100,6 +1100,106 @@ int tloam_b200_loop_verify_submap_target(tloam_b200_handle* h, double* xyz, doub
  * target row and its d2 */
 int tloam_b200_loop_verify_submap_matches(tloam_b200_handle* h, int pass, int* index, double* d2, size_t capacity, size_t* n);
 
+/* ---- Localization in a prior map (opt-in): each frame's scan is registered, point to plane, against a map loaded once --
+ * for example the merged map of an earlier session -- and the pose comes out in the map's frame, with the map <- odom
+ * correction.  Nothing here writes the odometry, the pose history, the submap, the global map and its tables, the loop
+ * database or the pose graph; every other call keeps its bits and launch counts.
+ *   - Map.  n x 3 FP64 rows, fixed after the load; row i's identity is its index.  A non-finite row is INVALID_ARG.
+ *   - Index, built once per load.  mb = the rows' min per axis; a row's cell is i_d = floor((x_d - mb_d) / cell), the
+ *     subtraction and the quotient each rounded; the largest index per axis must stay below 2^21 and every coordinate's
+ *     unit of rounding (|x| 2^-52) below 1e-6 cell (VOXEL_RANGE otherwise);
+ *     key = ix << (by + bz) | iy << bz | iz with b_d the bits of the largest index.  The rows are sorted by key by a
+ *     stable LSD radix sort (a cell's rows stay in row order); the occupied cells' keys ascend and cell j holds sorted
+ *     positions [start_j, start_(j+1)).
+ *   - Search.  For a point p and a radius r: the nearest map row with d2 <= r * r (d2 as in "Loop verification", r * r
+ *     rounded), by (d2, row index); none when no row is that close.  The cells visited on axis d run from the cell of
+ *     p_d - rr rounded down to the cell of p_d + rr rounded up, rr = r (1 + 1e-7) rounded up, clipped to the map's cells;
+ *     since the cell index is monotone in x, the result is that of an exhaustive scan limited to d2 <= r * r.  Both radii
+ *     a search uses (corr_dist_coarse, normal_radius) must be at most 3 cells.
+ *   - Normals, computed once per load for every map row: the rule of "Loop verification against a submap" (ascending row
+ *     order, the two-pass covariance, the cyclic Jacobi, validity from min_normal_neighbours and max_planarity) with the
+ *     neighbourhood within normal_radius taken from the grid.
+ *   - Query.  VoxelDownSample(voxel) of the finite rows of the scan by the ordered path of the loop keyframes: the scan
+ *     tloam_b200_process_raw_scan* left on the device (tloam_b200_localize_frame, under the NOT_READY rule of
+ *     tloam_b200_global_map_append_frame) or a host cloud (tloam_b200_localize).  An extent of 2^21 voxels is VOXEL_RANGE.
+ *   - Guess.  A host guess G (map <- sensor, column-major, rigid), or with guess == NULL the prediction
+ *     G = L_prev . (O_prev^-1 . O_now), each product and sum rounded on its own, left to right (R (r, c) = O[4c + r]):
+ *       R_D(r, c) = (R_p(0, r) R_n(0, c) + R_p(1, r) R_n(1, c)) + R_p(2, r) R_n(2, c),  t_D(r) = the same with e = t_n - t_p
+ *       R_G(r, c) = (R_L(r, 0) R_D(0, c) + R_L(r, 1) R_D(1, c)) + R_L(r, 2) R_D(2, c)
+ *       t_G(r)    = ((R_L(r, 0) t_D(0) + R_L(r, 1) t_D(1)) + R_L(r, 2) t_D(2)) + t_L(r)
+ *     O_now is the odometry pose of the frame the handle registered last (the pose tloam_b200_pose_graph_add_node_chained
+ *     records; identity before the first frame), O_prev the O_now of the previous localization, L_prev its T if it was
+ *     accepted and its G otherwise.  Without a host guess, the first localization after a load is NOT_READY.
+ *   - Passes, steps, radius schedule, convergence and termination: those of "Loop verification against a submap" with the
+ *     map in place of the target and the grid search in place of the exhaustive one.  Pass k's match is the nearest map
+ *     row within the pass's radius r_k (index -1 and d2 = +inf when none); the final pass searches within corr_dist_coarse
+ *     and counts inliers within corr_dist_fine.
+ *   - Result.  T (map <- sensor); T_map_odom = T . O_now^-1: R_M(r, c) = (R_T(r, 0) R_O(c, 0) + R_T(r, 1) R_O(c, 1)) +
+ *     R_T(r, 2) R_O(c, 2), t_M(r) = t_T(r) - ((R_M(r, 0) t_O(0) + R_M(r, 1) t_O(1)) + R_M(r, 2) t_O(2)); inliers and rmse
+ *     as in the submap verification; fitness = the mean over every query row of min(d2 of its final match,
+ *     corr_dist_coarse^2) (a row without a match counts corr_dist_coarse^2); accepted = converged && fitness <= max_fitness.
+ *     An empty query or an empty map: EMPTY, T = G, fitness +inf, not accepted.
+ *   - Device.  A load is k_loc_bounds (one read-back), k_loc_keys, the radix sort of the merged map (k_gmm_hist /
+ *     k_gmm_offsets / k_gmm_scatter per 8-bit digit, k_gmm_head_count / k_gmm_head_scatter), k_loc_cells and
+ *     k_loc_normals, then one synchronisation.  A frame is the query's down-sample (one read-back of its size), then
+ *     k_loc_predict, the rounds of k_loc_match / k_loc_reduce / k_loc_step, the final pass and k_loc_final, with one copy
+ *     home.  Memory: 93 B per map row for the map and its index plus 24 B per row of sort scratch; the kernels live in
+ *     libtloam_b200_loc.so, loaded from this library's directory by the enable call (ERR_CUDA if it is missing). */
+typedef struct tloam_localize_config {
+  double voxel;                        /* query down-sample, m */
+  double cell;                         /* grid cell edge, m */
+  double normal_radius;                /* m, <= 3 cell */
+  int min_normal_neighbours;           /* >= 3 */
+  double max_planarity;                /* a normal is valid iff l0 <= max_planarity * l1 */
+  double corr_dist_coarse;             /* first correspondence radius, m, <= 3 cell */
+  double corr_dist_fine;               /* last correspondence radius, m (<= corr_dist_coarse) */
+  int max_iterations;                  /* Gauss-Newton steps, 1 .. 200 */
+  double eps_translation;              /* m */
+  double eps_rotation;                 /* rad */
+  double max_fitness;                  /* m^2 */
+} tloam_localize_config;
+typedef struct tloam_localize_result {
+  double T[16];                        /* map <- sensor, column-major */
+  double T_map_odom[16];               /* T . O_now^-1 */
+  double guess[16];                    /* the G the run started from */
+  int iterations;
+  int termination;                     /* TLOAM_LOOP_VERIFY_* */
+  int accepted;
+  long long inliers;
+  double rmse, fitness;
+  long long n_query_points, n_map_points;
+} tloam_localize_result;
+/* voxel 0.5 m, cell 1 m, normal_radius 1 m, min_normal_neighbours 5, max_planarity 0.1, corr_dist_coarse 2 m,
+ * corr_dist_fine 0.5 m, max_iterations 30, eps_translation 1e-4 m, eps_rotation 1e-5 rad, max_fitness 0.5 m^2 */
+void tloam_b200_localize_default_config(tloam_localize_config* c);
+/* turns localization on (or re-configures it) and drops any loaded map.  INVALID_ARG: cfg null; a value not finite or
+ * not > 0; min_normal_neighbours < 3; corr_dist_fine > corr_dist_coarse; max_iterations outside [1, 200];
+ * corr_dist_coarse or normal_radius > 3 cell. */
+int tloam_b200_localize_enable(tloam_b200_handle* h, const tloam_localize_config* cfg);
+/* loads a HOST map (n x 3) and builds its index and normals; synchronises.  NOT_READY: localization off.  INVALID_ARG:
+ * xyz null with n > 0, n >= 2^32, a non-finite row.  VOXEL_RANGE: an extent of 2^21 cells.  A refused load leaves no map. */
+int tloam_b200_localize_set_map(tloam_b200_handle* h, const double* xyz, size_t n);
+/* the same with the handle's last tloam_b200_global_map_merge, copied on the device.  NOT_READY: localization off or no
+ * merge. */
+int tloam_b200_localize_set_map_merged(tloam_b200_handle* h);
+/* localizes the scan the last tloam_b200_process_raw_scan* left on the device from guess (NULL: the prediction) and
+ * returns once the result is home.  NOT_READY: localization off, no map, no such scan, or guess NULL on the first
+ * localization after a load.  BAD_POSE: guess not rigid.  VOXEL_RANGE: the query's extent. */
+int tloam_b200_localize_frame(tloam_b200_handle* h, const double guess[16], tloam_localize_result* out);
+/* the same for a HOST cloud (n x 3) */
+int tloam_b200_localize(tloam_b200_handle* h, const double* xyz, size_t n, const double guess[16], tloam_localize_result* out);
+/* the last localization's matches at pass k (0 .. iterations): per query row the map row (-1: none) and its d2 */
+int tloam_b200_localize_matches(tloam_b200_handle* h, int pass, int* index, double* d2, size_t capacity, size_t* n);
+/* the last localization's query (n x 3) */
+int tloam_b200_localize_query(tloam_b200_handle* h, double* xyz, size_t capacity, size_t* n);
+/* the loaded map's normals, validity and neighbour counts, per map row (any output may be null) */
+int tloam_b200_localize_map_normals(tloam_b200_handle* h, double* normal, unsigned char* valid, int* neighbours, size_t capacity,
+                                    size_t* n);
+/* the loaded map's cell table: the map row at each sorted position (n), the *n_cells occupied cells' keys and their
+ * starts (*n_cells + 1); capacity is that of sorted_rows and must be >= the map's rows (keys and starts need as many) */
+int tloam_b200_localize_cells(tloam_b200_handle* h, unsigned* sorted_rows, unsigned long long* keys, unsigned* starts,
+                              size_t capacity, size_t* n_cells);
+
 /* Pinned host memory helpers (optional; pinned inputs make set_* a direct DMA, no staging threads). */
 int tloam_b200_host_alloc(void** p, size_t bytes);
 int tloam_b200_host_free(void* p);

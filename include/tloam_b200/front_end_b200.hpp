@@ -316,6 +316,30 @@ class FrontEndB200 {
                                                         has ? intensity.data() : nullptr), "mergedGlobalMap");
   }
 
+  // Localization in a prior map (include/tloam_b200.h "Localization in a prior map"): a map from an earlier session (for
+  // example its mergedGlobalMap, saved by the caller) is loaded once; each frame is then registered against it and comes
+  // out in the map's frame, with the map <- odom correction.  The odometry and the maps above are not touched.
+  bool enableLocalization(const tloam_localize_config& cfg) { return report(tloam_b200_localize_enable(h_, &cfg), "enableLocalization"); }
+  bool enableLocalization() {
+    tloam_localize_config c;
+    tloam_b200_localize_default_config(&c);
+    return enableLocalization(c);
+  }
+  bool setPriorMap(const std::vector<Eigen::Vector3d>& map) {
+    return report(tloam_b200_localize_set_map(h_, map.empty() ? nullptr : reinterpret_cast<const double*>(map.data()), map.size()),
+                  "setPriorMap");
+  }
+  // the handle's last mergedGlobalMap, on the device
+  bool setPriorMapMerged() { return report(tloam_b200_localize_set_map_merged(h_), "setPriorMapMerged"); }
+  // the scan the handle processed last; guess null: the prediction from the previous localization and the odometry
+  bool localizeFrame(tloam_localize_result& out, const Eigen::Isometry3d* guess = nullptr) {
+    return report(tloam_b200_localize_frame(h_, guess ? guess->matrix().data() : nullptr, &out), "localizeFrame");
+  }
+  // a host cloud
+  bool localize(const CloudData& scan, tloam_localize_result& out, const Eigen::Isometry3d* guess = nullptr) {
+    return report(tloam_b200_localize(h_, data(scan), size(scan), guess ? guess->matrix().data() : nullptr, &out), "localize");
+  }
+
   // processCloud + setInputSource (ref: front_end.cpp:181-199, :313): the three clouds the segmentation nodelet publishes
   bool processCloud(CloudData& ground, CloudData& edge, CloudData& general) {
     return report(tloam_b200_process_cloud(h_, &fcfg_, ground_down_sample_, edge_down_sample_, data(ground), size(ground), data(edge),

@@ -96,6 +96,22 @@ class LoopVerifyResult(C.Structure):
                 ("n_candidate_points", C.c_longlong), ("iterations", C.c_int), ("termination", C.c_int), ("accepted", C.c_int)]
 
 
+class LocalizeConfig(C.Structure):
+    """tloam_localize_config (include/tloam_b200.h "Localization in a prior map")."""
+    _fields_ = [("voxel", C.c_double), ("cell", C.c_double), ("normal_radius", C.c_double),
+                ("min_normal_neighbours", C.c_int), ("max_planarity", C.c_double), ("corr_dist_coarse", C.c_double),
+                ("corr_dist_fine", C.c_double), ("max_iterations", C.c_int), ("eps_translation", C.c_double),
+                ("eps_rotation", C.c_double), ("max_fitness", C.c_double)]
+
+
+class LocalizeResult(C.Structure):
+    """tloam_localize_result: T (map <- sensor), T_map_odom and the guess (column-major), and the ICP's verdict."""
+    _fields_ = [("T", C.c_double * 16), ("T_map_odom", C.c_double * 16), ("guess", C.c_double * 16),
+                ("iterations", C.c_int), ("termination", C.c_int), ("accepted", C.c_int), ("inliers", C.c_longlong),
+                ("rmse", C.c_double), ("fitness", C.c_double), ("n_query_points", C.c_longlong),
+                ("n_map_points", C.c_longlong)]
+
+
 class PoseGraphConfig(C.Structure):
     """tloam_pose_graph_config (include/tloam_b200.h "Pose graph"): the edges' sigmas and the Gauss-Newton schedule."""
     _fields_ = [("sigma_odom_translation", C.c_double), ("sigma_odom_rotation", C.c_double),
@@ -233,6 +249,9 @@ EXPORTS = [
     "tloam_b200_global_map_dynamic_default_config", "tloam_b200_global_map_dynamic_enable",
     "tloam_b200_global_map_votes_download", "tloam_b200_global_map_static_download",
     "tloam_b200_global_map_merge", "tloam_b200_global_map_merged_download",
+    "tloam_b200_localize_default_config", "tloam_b200_localize_enable", "tloam_b200_localize_set_map",
+    "tloam_b200_localize_set_map_merged", "tloam_b200_localize_frame", "tloam_b200_localize", "tloam_b200_localize_matches",
+    "tloam_b200_localize_query", "tloam_b200_localize_map_normals", "tloam_b200_localize_cells",
 ]
 
 _lib = None
@@ -435,5 +454,16 @@ def load():
     L.tloam_b200_global_map_static_download.argtypes = [vp, dp, dp, C.c_size_t, szp]
     L.tloam_b200_global_map_merge.argtypes = [vp, C.c_double, C.c_int, szp]
     L.tloam_b200_global_map_merged_download.argtypes = [vp, C.c_size_t, C.c_size_t, dp, dp]
+    L.tloam_b200_localize_default_config.argtypes = [C.POINTER(LocalizeConfig)]
+    L.tloam_b200_localize_default_config.restype = None
+    L.tloam_b200_localize_enable.argtypes = [vp, C.POINTER(LocalizeConfig)]
+    L.tloam_b200_localize_set_map.argtypes = [vp, dp, C.c_size_t]
+    L.tloam_b200_localize_set_map_merged.argtypes = [vp]
+    L.tloam_b200_localize_frame.argtypes = [vp, dp, C.POINTER(LocalizeResult)]
+    L.tloam_b200_localize.argtypes = [vp, dp, C.c_size_t, dp, C.POINTER(LocalizeResult)]
+    L.tloam_b200_localize_matches.argtypes = [vp, C.c_int, C.POINTER(C.c_int), dp, C.c_size_t, szp]
+    L.tloam_b200_localize_query.argtypes = [vp, dp, C.c_size_t, szp]
+    L.tloam_b200_localize_map_normals.argtypes = [vp, dp, C.POINTER(C.c_ubyte), C.POINTER(C.c_int), C.c_size_t, szp]
+    L.tloam_b200_localize_cells.argtypes = [vp, up, C.POINTER(C.c_ulonglong), up, C.c_size_t, szp]
     _lib = L
     return L

@@ -15,6 +15,7 @@
 
 #include "ldlt6.cuh"
 #include "loop_verify_submap.h"
+#include "normal_fit.cuh"
 #include "se3.cuh"
 
 namespace tloam {
@@ -83,60 +84,6 @@ __global__ void __launch_bounds__(kLvsT) k_lvs_assemble(tloam_lvs_args a) {
   for (int r = 0; r < 3; ++r) o[r] = __dadd_rn(lvs_dot3(A[r], x, A[4 + r], y, A[8 + r], z), A[12 + r]);
 }
 
-// cyclic Jacobi of the symmetric c (xx, xy, xz, yy, yz, zz): at most 32 sweeps over (0,1), (0,2), (1,2), a rotation
-// skipped when its entry is 0, done once off <= 1e-32 diag; eigenvalues ascending by three compare-exchanges (ties keep
-// the lower axis first), nvec the eigenvector of the least.  Every operation separately rounded.
-__device__ __forceinline__ void lvs_jacobi3(const double c[6], double eig[3], double nvec[3]) {
-  double a[3][3] = {{c[0], c[1], c[2]}, {c[1], c[3], c[4]}, {c[2], c[4], c[5]}};
-  double v[3][3] = {{1, 0, 0}, {0, 1, 0}, {0, 0, 1}};
-#pragma unroll 1
-  for (int sweep = 0; sweep < 32; ++sweep) {
-    const double off = lvs_dot3(a[0][1], a[0][1], a[0][2], a[0][2], a[1][2], a[1][2]);
-    const double diag = lvs_dot3(a[0][0], a[0][0], a[1][1], a[1][1], a[2][2], a[2][2]);
-    if (off <= __dmul_rn(1e-32, diag) || off == 0.0) break;
-#pragma unroll
-    for (int p = 0; p < 2; ++p)
-#pragma unroll
-      for (int q = p + 1; q < 3; ++q) {
-        if (a[p][q] == 0.0) continue;
-        const double theta = __ddiv_rn(__dsub_rn(a[q][q], a[p][p]), __dmul_rn(2.0, a[p][q]));
-        const double t = __ddiv_rn(theta >= 0 ? 1.0 : -1.0, __dadd_rn(fabs(theta), __dsqrt_rn(__dadd_rn(__dmul_rn(theta, theta), 1.0))));
-        const double cs = __ddiv_rn(1.0, __dsqrt_rn(__dadd_rn(__dmul_rn(t, t), 1.0))), sn = __dmul_rn(t, cs);
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-          const double akp = a[k][p], akq = a[k][q];
-          a[k][p] = __dsub_rn(__dmul_rn(cs, akp), __dmul_rn(sn, akq));
-          a[k][q] = __dadd_rn(__dmul_rn(sn, akp), __dmul_rn(cs, akq));
-        }
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-          const double apk = a[p][k], aqk = a[q][k];
-          a[p][k] = __dsub_rn(__dmul_rn(cs, apk), __dmul_rn(sn, aqk));
-          a[q][k] = __dadd_rn(__dmul_rn(sn, apk), __dmul_rn(cs, aqk));
-        }
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-          const double vkp = v[k][p], vkq = v[k][q];
-          v[k][p] = __dsub_rn(__dmul_rn(cs, vkp), __dmul_rn(sn, vkq));
-          v[k][q] = __dadd_rn(__dmul_rn(sn, vkp), __dmul_rn(cs, vkq));
-        }
-      }
-  }
-  double d0 = a[0][0], d1 = a[1][1], d2 = a[2][2];
-  double n0[3] = {v[0][0], v[1][0], v[2][0]}, n1[3] = {v[0][1], v[1][1], v[2][1]}, n2[3] = {v[0][2], v[1][2], v[2][2]};
-  auto cswap = [](double& da, double& db, double* na, double* nb) {
-    if (db < da) {
-      const double t = da; da = db; db = t;
-      for (int r = 0; r < 3; ++r) { const double u = na[r]; na[r] = nb[r]; nb[r] = u; }
-    }
-  };
-  cswap(d0, d1, n0, n1);
-  cswap(d1, d2, n1, n2);
-  cswap(d0, d1, n0, n1);
-  eig[0] = d0; eig[1] = d1; eig[2] = d2;
-  nvec[0] = n0[0]; nvec[1] = n0[1]; nvec[2] = n0[2];
-}
-
 // a thread per target row i; the whole target streamed through shared memory in tiles of kLvsN in ascending row order,
 // twice: the first sweep counts the rows within normal_radius and sums them, the second sums the products of their
 // offsets from the mean.  Each thread adds its neighbours in ascending row order.
@@ -168,12 +115,7 @@ __global__ void __launch_bounds__(kLvsN) k_lvs_normals(tloam_lvs_args a) {
       } else {
         for (int k = 0; k < n; ++k) {
           const double x = sx[k], y = sy[k], z = sz[k];
-          if (lvs_d2(px, py, pz, x, y, z) <= r2) {
-            const double dx = __dsub_rn(x, mx), dy = __dsub_rn(y, my), dz = __dsub_rn(z, mz);
-            c[0] = __dadd_rn(c[0], __dmul_rn(dx, dx)); c[1] = __dadd_rn(c[1], __dmul_rn(dx, dy));
-            c[2] = __dadd_rn(c[2], __dmul_rn(dx, dz)); c[3] = __dadd_rn(c[3], __dmul_rn(dy, dy));
-            c[4] = __dadd_rn(c[4], __dmul_rn(dy, dz)); c[5] = __dadd_rn(c[5], __dmul_rn(dz, dz));
-          }
+          if (lvs_d2(px, py, pz, x, y, z) <= r2) nf_cov_add(c, x, y, z, mx, my, mz);
         }
       }
     }
@@ -183,14 +125,11 @@ __global__ void __launch_bounds__(kLvsN) k_lvs_normals(tloam_lvs_args a) {
     }
   }
   if (!have) return;
-  const double n = (double)cnt;
-#pragma unroll
-  for (int k = 0; k < 6; ++k) c[k] = __ddiv_rn(c[k], n);
-  double eig[3], nv[3];
-  lvs_jacobi3(c, eig, nv);
+  double nv[3];
+  const unsigned char ok = nf_finish(cnt, c, a.min_normal_neighbours, a.max_planarity, nv);
   a.normal[3 * i] = nv[0]; a.normal[3 * i + 1] = nv[1]; a.normal[3 * i + 2] = nv[2];
   a.neighbours[i] = cnt;
-  a.valid[i] = cnt >= a.min_normal_neighbours && eig[0] <= __dmul_rn(a.max_planarity, eig[1]) ? 1 : 0;
+  a.valid[i] = ok;
 }
 
 // grid (query blocks, splits): thread i of block (x, y) takes query row x * kLvsT + i and the rows of slice y of the

@@ -37,6 +37,7 @@
 #include "map_correct.h"
 #include "map_dynamic.h"
 #include "map_merge.h"
+#include "localize.h"
 
 
 
@@ -277,6 +278,22 @@ struct tloam_b200_handle {
   unsigned char* d_lvs_scratch = nullptr;  size_t cap_lvs_scratch = 0;
   bool lvs_ran = false;                    int lvs_passes = 0;   unsigned long long lvs_nq = 0, lvs_nm = 0;   // the last run
   tloam_lvs_args lvs_last;                 // its buffers (target, normals, matches)
+  // ---- localization in a prior map (tloam_b200_localize*, libtloam_b200_loc.so): the map and its index (one buffer,
+  //      grown by a load), the query's ordered down-sample and the run's scratch; nothing is allocated or launched until
+  //      it is enabled ----
+  bool loc_on = false;
+  tloam_localize_config loc_cfg;
+  unsigned char* d_loc_map = nullptr;      size_t cap_loc_map = 0;     // map, sorted map, rows, cells, normals
+  unsigned char* d_loc_scratch = nullptr;  size_t cap_loc_scratch = 0; // the index build's radix sort
+  bool loc_loaded = false;                 size_t loc_n = 0;           tloam_loc_index_args loc_index;
+  GMapState* d_loc_qst = nullptr;
+  double* d_loc_reg = nullptr;             size_t cap_loc_reg = 0;
+  double* d_loc_fin = nullptr;             size_t cap_loc_fin = 0;
+  double* d_loc_q = nullptr;               size_t cap_loc_q = 0;       // the query (ordered down-sample)
+  double* d_loc_in = nullptr;              size_t cap_loc_in = 0;      // a host cloud
+  unsigned char* d_loc_run = nullptr;      size_t cap_loc_run = 0;     // state, memory, partials, matches
+  bool loc_have_prev = false;              // a localization since the load: the prediction has its memory
+  bool loc_ran = false;                    int loc_passes = 0;  size_t loc_nq = 0;   tloam_loc_args loc_last;
   // ---- pose graph (tloam_b200_pose_graph*, libtloam_b200_pg.so): the node store on the device, the loop edges on the
   //      host until an optimisation uploads them; nothing is allocated or launched until it is enabled ----
   bool pg_on = false;
@@ -494,6 +511,8 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   cudaFree(h->d_gmd_through); cudaFree(h->d_gmd_hits); cudaFree(h->d_gmd_image); cudaFree(h->d_gmd_window);
   cudaFree(h->d_gmd_bounds); cudaFree(h->d_gmd_scratch);
   cudaFree(h->d_gmm_scratch); cudaFree(h->d_gmm_out);
+  cudaFree(h->d_loc_map); cudaFree(h->d_loc_scratch); cudaFree(h->d_loc_qst); cudaFree(h->d_loc_reg); cudaFree(h->d_loc_fin);
+  cudaFree(h->d_loc_q); cudaFree(h->d_loc_in); cudaFree(h->d_loc_run);
   for (int i = 0; i < 2; ++i) if (h->ev_stage_free[i]) cudaEventDestroy(h->ev_stage_free[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_fit[i]) cudaEventDestroy(h->ev_fit[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_res[i]) cudaEventDestroy(h->ev_res[i]);
@@ -5421,6 +5440,370 @@ int tloam_b200_loop_verify_submap_matches(tloam_b200_handle* h, int pass, int* i
   CU_TRY(cudaStreamSynchronize(h->stream));
   if (index) CU_TRY(cudaMemcpyAsync(index, a.match_index + (size_t)pass * nq, nq * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   if (d2) CU_TRY(cudaMemcpyAsync(d2, a.match_d2 + (size_t)pass * nq, nq * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Localization in a prior map (the checks, the query's down-sample and the buffers here; the kernels in localize.cu,
+// loaded from libtloam_b200_loc.so by the enable call).
+// ---------------------------------------------------------------------------------------------
+struct LocLib {
+  tloam_loc_scratch_bytes_fn scratch_bytes = nullptr;
+  tloam_loc_index_fn bounds = nullptr, index = nullptr;
+  tloam_loc_run_fn run = nullptr;
+};
+static std::mutex g_loc_mu;
+static LocLib g_loc;
+
+static int loc_load(tloam_b200_handle* h, LocLib* out) {
+  std::lock_guard<std::mutex> lk(g_loc_mu);
+  if (!g_loc.run) {
+    const std::string path = sibling_path("libtloam_b200_loc.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    LocLib l;
+    if (so) {
+      l.scratch_bytes = reinterpret_cast<tloam_loc_scratch_bytes_fn>(dlsym(so, "tloam_loc_scratch_bytes"));
+      l.bounds = reinterpret_cast<tloam_loc_index_fn>(dlsym(so, "tloam_loc_bounds"));
+      l.index = reinterpret_cast<tloam_loc_index_fn>(dlsym(so, "tloam_loc_index"));
+      l.run = reinterpret_cast<tloam_loc_run_fn>(dlsym(so, "tloam_loc_run"));
+    }
+    if (!l.scratch_bytes || !l.bounds || !l.index || !l.run) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "localization: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_loc = l;
+  }
+  *out = g_loc;
+  return TLOAM_B200_OK;
+}
+
+static int loc_status(tloam_b200_handle* h, int e, const char* where) {
+  if (e == cudaSuccess) return TLOAM_B200_OK;
+  snprintf(h->last_error, sizeof(h->last_error), "localization: %s: %s", where, cudaGetErrorString((cudaError_t)e));
+  return TLOAM_B200_ERR_CUDA;
+}
+
+// the small block: the query's GMapState at 0, the identity pose at 256, the prediction's memory at 512
+static GMapState* loc_qst(tloam_b200_handle* h) { return h->d_loc_qst; }
+static double* loc_eye(tloam_b200_handle* h) { return reinterpret_cast<double*>(reinterpret_cast<char*>(h->d_loc_qst) + 256); }
+static tloam_loc_memory* loc_memory(tloam_b200_handle* h) {
+  return reinterpret_cast<tloam_loc_memory*>(reinterpret_cast<char*>(h->d_loc_qst) + 512);
+}
+
+void tloam_b200_localize_default_config(tloam_localize_config* c) {
+  c->voxel = 0.5; c->cell = 1.0;
+  c->normal_radius = 1.0; c->min_normal_neighbours = 5; c->max_planarity = 0.1;
+  c->corr_dist_coarse = 2.0; c->corr_dist_fine = 0.5;
+  c->max_iterations = 30;
+  c->eps_translation = 1e-4; c->eps_rotation = 1e-5;
+  c->max_fitness = 0.5;
+}
+
+int tloam_b200_localize_enable(tloam_b200_handle* h, const tloam_localize_config* c) {
+  if (!h || !c) return TLOAM_B200_ERR_INVALID_ARG;
+  const double v[9] = {c->voxel, c->cell, c->normal_radius, c->max_planarity, c->corr_dist_coarse, c->corr_dist_fine,
+                       c->eps_translation, c->eps_rotation, c->max_fitness};
+  for (double x : v)
+    if (!std::isfinite(x) || !(x > 0.0)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (c->min_normal_neighbours < 3 || c->corr_dist_fine > c->corr_dist_coarse || c->max_iterations < 1 || c->max_iterations > 200 ||
+      c->corr_dist_coarse > 3.0 * c->cell || c->normal_radius > 3.0 * c->cell)
+    return TLOAM_B200_ERR_INVALID_ARG;
+  LocLib lib;
+  int rc = loc_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (!h->d_loc_qst) {
+    CU_TRY(cudaMalloc(&h->d_loc_qst, 512 + sizeof(tloam_loc_memory)));
+    const double eye[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+    CU_TRY(cudaMemcpy(loc_eye(h), eye, sizeof(eye), cudaMemcpyHostToDevice));
+  }
+  h->loc_cfg = *c;
+  h->loc_on = true;
+  h->loc_loaded = false; h->loc_n = 0; h->loc_have_prev = false;
+  h->loc_ran = false; h->loc_passes = 0; h->loc_nq = 0;
+  return TLOAM_B200_OK;
+}
+
+// the map (already at the start of d_loc_map) indexed: bounds, key range, sort, cells, normals; synchronises
+static int loc_build(tloam_b200_handle* h, size_t n) {
+  LocLib lib;
+  int rc = loc_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  unsigned char* b = h->d_loc_map;
+  tloam_loc_index_args a;
+  memset(&a, 0, sizeof(a));
+  size_t o = 0;
+  a.map = reinterpret_cast<const double*>(b + o);   o += round_up(n * 24, 256);
+  a.sxyz = reinterpret_cast<double*>(b + o);        o += round_up(n * 24, 256);
+  a.normal = reinterpret_cast<double*>(b + o);      o += round_up(n * 24, 256);
+  a.ckey = reinterpret_cast<unsigned long long*>(b + o); o += round_up(n * 8, 256);
+  a.srow = reinterpret_cast<unsigned*>(b + o);      o += round_up(n * 4, 256);
+  a.cstart = reinterpret_cast<unsigned*>(b + o);    o += round_up((n + 1) * 4, 256);
+  a.neighbours = reinterpret_cast<int*>(b + o);     o += round_up(n * 4, 256);
+  a.valid = b + o;                                  o += round_up(n, 256);
+  a.st = reinterpret_cast<tloam_gmm_state*>(b + o);
+  a.n = n;
+  a.normal_radius = h->loc_cfg.normal_radius; a.max_planarity = h->loc_cfg.max_planarity;
+  a.min_normal_neighbours = h->loc_cfg.min_normal_neighbours;
+  a.grid.sxyz = a.sxyz; a.grid.srow = a.srow; a.grid.ckey = a.ckey; a.grid.cstart = a.cstart; a.grid.st = a.st;
+  a.grid.cell = h->loc_cfg.cell;
+  a.device = h->device; a.stream = h->stream;
+  const size_t bytes = lib.scratch_bytes(n ? n : 1);
+  if (bytes > h->cap_loc_scratch) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_loc_scratch); h->d_loc_scratch = nullptr; h->cap_loc_scratch = 0;
+    CU_TRY(cudaMalloc(&h->d_loc_scratch, bytes));
+    h->cap_loc_scratch = bytes;
+  }
+  a.scratch = h->d_loc_scratch;
+  int e = 0, launches = 0;
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.bounds(&a, &launches)));
+  h->launches += launches > 0 ? launches - 1 : 0;
+  if ((rc = loc_status(h, e, "k_loc_bounds")) != TLOAM_B200_OK) return rc;
+  tloam_gmm_state gs;
+  CU_TRY(cudaMemcpyAsync(&gs, a.st, sizeof(gs), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (gs.nonfinite) return TLOAM_B200_ERR_INVALID_ARG;
+  if (n) {
+    for (int d = 0; d < 3; ++d) {                // cell index floor((x - min) / cell), monotone in x: the max row has the top
+      a.grid.mb[d] = dec_ordered(~gs.lo[d]);
+      const double ref = std::floor((dec_ordered(gs.hi[d]) - a.grid.mb[d]) / a.grid.cell);
+      if (!(ref < (double)(1u << kGMapKeyBits))) return TLOAM_B200_ERR_VOXEL_RANGE;
+      // the search's cell ranges (k_loc_normals keeps at most TLOAM_LOC_MAX_SPAN per axis) assume that a coordinate's
+      // rounding is far below a cell: radius <= 3 cells spans at most 6 (1 + 1e-7) cells plus that rounding
+      const double big = std::fmax(std::fabs(dec_ordered(~gs.lo[d])), std::fabs(dec_ordered(gs.hi[d])));
+      if (!(big * 0x1p-52 < 1e-6 * a.grid.cell)) return TLOAM_B200_ERR_VOXEL_RANGE;
+      a.grid.top[d] = (long long)ref;
+      int bits = 0;
+      while (bits < 64 && ((unsigned long long)a.grid.top[d] >> bits)) ++bits;
+      a.grid.bits[d] = bits;
+    }
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.index(&a, &launches)));
+    h->launches += launches > 0 ? launches - 1 : 0;
+    if ((rc = loc_status(h, e, "k_loc_keys / k_gmm_* / k_loc_cells / k_loc_normals")) != TLOAM_B200_OK) return rc;
+    CU_TRY(cudaStreamSynchronize(h->stream));
+  }
+  h->loc_index = a;
+  h->loc_n = n; h->loc_loaded = true;
+  return TLOAM_B200_OK;
+}
+
+// room for an n-row map and its index at the start of d_loc_map (the old map is dropped)
+static int loc_reserve_map(tloam_b200_handle* h, size_t n) {
+  const size_t need = 3 * round_up(n * 24, 256) + round_up(n * 8, 256) + round_up(n * 4, 256) + round_up((n + 1) * 4, 256) +
+                      round_up(n * 4, 256) + round_up(n, 256) + round_up(sizeof(tloam_gmm_state), 256);
+  if (need > h->cap_loc_map) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_loc_map); h->d_loc_map = nullptr; h->cap_loc_map = 0;
+    CU_TRY(cudaMalloc(&h->d_loc_map, need));
+    h->cap_loc_map = need;
+  }
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_localize_set_map(tloam_b200_handle* h, const double* xyz, size_t n) {
+  if (!h || (!xyz && n)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loc_on) return TLOAM_B200_ERR_NOT_READY;
+  if (n >> 32) return TLOAM_B200_ERR_INVALID_ARG;             // the sort's row payload is a u32
+  CU_TRY(cudaSetDevice(h->device));
+  h->loc_loaded = false; h->loc_have_prev = false; h->loc_ran = false; h->loc_passes = 0;
+  int rc;
+  if ((rc = loc_reserve_map(h, n)) != TLOAM_B200_OK) return rc;
+  if (n && (rc = upload_host(h, h->d_loc_map, xyz, n * 24)) != TLOAM_B200_OK) return rc;
+  return loc_build(h, n);
+}
+
+int tloam_b200_localize_set_map_merged(tloam_b200_handle* h) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loc_on || !h->gmm_valid) return TLOAM_B200_ERR_NOT_READY;
+  CU_TRY(cudaSetDevice(h->device));
+  const size_t n = h->gmm_n;
+  h->loc_loaded = false; h->loc_have_prev = false; h->loc_ran = false; h->loc_passes = 0;
+  int rc;
+  if ((rc = loc_reserve_map(h, n)) != TLOAM_B200_OK) return rc;
+  if (n) CU_TRY(cudaMemcpyAsync(h->d_loc_map, h->d_gmm_out, n * 24, cudaMemcpyDeviceToDevice, h->stream));
+  return loc_build(h, n);
+}
+
+// the query: VoxelDownSample(voxel) of the finite rows of the n rows at d_in by the global map's ordered path at pose I
+// (the keyframe path of loop verification, in buffers of its own); synchronises and returns its row count
+static int loc_query(tloam_b200_handle* h, const double* d_in, size_t n, size_t* nq) {
+  int rc;
+  if ((rc = ensure_dev(h, &h->d_loc_reg, &h->cap_loc_reg, n, false)) != TLOAM_B200_OK) return rc;
+  if ((rc = ensure_dev(h, &h->d_loc_fin, &h->cap_loc_fin, n, false)) != TLOAM_B200_OK) return rc;
+  if ((rc = ensure_dev(h, &h->d_loc_q, &h->cap_loc_q, n, false)) != TLOAM_B200_OK) return rc;
+  GMapState* st = loc_qst(h);
+  const double voxel = h->loc_cfg.voxel;
+  CU_TRY(cudaMemsetAsync(st, 0, sizeof(GMapState), h->stream));
+  const unsigned tb = 256, gb = (unsigned)((n + tb - 1) / tb);
+  if (n) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_transform<<<gb, tb, 0, h->stream>>>(d_in, (unsigned)n, loc_eye(h), h->d_loc_reg, h->d_loc_fin, st)));
+  if (n) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_guard<<<1, 32, 0, h->stream>>>(st, voxel)));
+  VoxSorted vs;
+  if ((rc = voxel_pipeline(h, h->d_loc_fin, n, &st->n_fin, 0u, nullptr, nullptr, nullptr, 0.0, voxel, nullptr, &st->n_vox,
+                           h->stream, 0, &vs)) != TLOAM_B200_OK) return rc;
+  if (n) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_emit<<<gb, tb, 0, h->stream>>>(vs.a, vs.slots, h->d_loc_q, st, h->cap_loc_q)));
+  CU_TRY(cudaGetLastError());
+  GMapState s;
+  CU_TRY(cudaMemcpyAsync(&s, st, sizeof(s), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (s.refused) return TLOAM_B200_ERR_VOXEL_RANGE;
+  *nq = s.refused ? 0 : s.n_vox;
+  return TLOAM_B200_OK;
+}
+
+static int loc_run(tloam_b200_handle* h, const double* d_in, size_t n, const double* guess, tloam_localize_result* out) {
+  if (!h->loc_loaded) return TLOAM_B200_ERR_NOT_READY;
+  if (!guess && !h->loc_have_prev) return TLOAM_B200_ERR_NOT_READY;
+  if (guess && !pg_rigid(guess)) return TLOAM_B200_ERR_BAD_POSE;
+  LocLib lib;
+  int rc = loc_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  size_t nq = 0;
+  if ((rc = loc_query(h, d_in, n, &nq)) != TLOAM_B200_OK) return rc;
+  const tloam_localize_config& c = h->loc_cfg;
+  const size_t nr = h->loc_n ? nq : 0;                          // an empty map: nothing to match (EMPTY)
+  const size_t passes = (size_t)c.max_iterations + 1, qb = (nr + TLOAM_LOC_THREADS - 1) / TLOAM_LOC_THREADS;
+  size_t o = round_up(sizeof(tloam_loc_state), 256);
+  const size_t o_sums = o;  o += round_up(qb * TLOAM_LOC_SUMS * sizeof(double), 256);
+  const size_t o_idx = o;   o += round_up(passes * nr * sizeof(int), 256);
+  const size_t o_d2 = o;    o += passes * nr * sizeof(double);
+  if (o > h->cap_loc_run) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_loc_run); h->d_loc_run = nullptr; h->cap_loc_run = 0;
+    CU_TRY(cudaMalloc(&h->d_loc_run, o + o / 2));
+    h->cap_loc_run = o + o / 2;
+  }
+  unsigned char* base = h->d_loc_run;
+  tloam_loc_state s;
+  memset(&s, 0, sizeof(s));
+  s.r = c.corr_dist_coarse;
+  s.term = nr ? TLOAM_LOOP_VERIFY_ITERATION_LIMIT : TLOAM_LOOP_VERIFY_EMPTY;
+  s.done = nr ? 0 : 1;
+  if (guess) memcpy(s.guess, guess, sizeof(s.guess));
+  CU_TRY(cudaMemcpyAsync(base, &s, sizeof(s), cudaMemcpyHostToDevice, h->stream));   // pageable: staged before return
+  tloam_loc_args a;
+  memset(&a, 0, sizeof(a));
+  a.grid = h->loc_index.grid;
+  a.map = h->loc_index.map; a.normal = h->loc_index.normal; a.valid = h->loc_index.valid;
+  a.query = h->d_loc_q; a.nq = nr;
+  a.odom = reinterpret_cast<const double*>(reinterpret_cast<const char*>(h->d_state) + offsetof(FrameState, result));
+  a.predict = guess ? 0 : 1;
+  a.memory = loc_memory(h);
+  a.corr_dist_coarse = c.corr_dist_coarse; a.corr_dist_fine = c.corr_dist_fine;
+  a.eps_translation = c.eps_translation; a.eps_rotation = c.eps_rotation; a.max_fitness = c.max_fitness;
+  a.max_iterations = c.max_iterations;
+  a.state = reinterpret_cast<tloam_loc_state*>(base);
+  a.sums = reinterpret_cast<double*>(base + o_sums);
+  a.match_index = reinterpret_cast<int*>(base + o_idx);
+  a.match_d2 = reinterpret_cast<double*>(base + o_d2);
+  a.device = h->device; a.stream = h->stream;
+  int e = 0, launches = 0;
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.run(&a, &launches)));
+  h->launches += launches > 0 ? launches - 1 : 0;
+  if ((rc = loc_status(h, e, "k_loc_*")) != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaMemcpyAsync(&s, a.state, sizeof(s), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  memset(out, 0, sizeof(*out));
+  for (int r = 0; r < 3; ++r) {
+    for (int j = 0; j < 3; ++j) out->T[4 * j + r] = s.R[3 * r + j];
+    out->T[12 + r] = s.t[r];
+  }
+  out->T[15] = 1.0;
+  memcpy(out->T_map_odom, s.map_odom, sizeof(out->T_map_odom));
+  memcpy(out->guess, s.guess, sizeof(out->guess));
+  out->iterations = s.iter; out->termination = s.term; out->accepted = s.accepted;
+  out->inliers = (long long)s.inliers; out->rmse = s.rmse; out->fitness = s.fitness;
+  out->n_query_points = (long long)nq; out->n_map_points = (long long)h->loc_n;
+  h->loc_have_prev = true;
+  h->loc_ran = true; h->loc_passes = nr ? s.iter + 1 : 0; h->loc_nq = nr; h->loc_last = a;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_localize_frame(tloam_b200_handle* h, const double guess[16], tloam_localize_result* out) {
+  if (!h || !out) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loc_on || h->raw_gen != h->seg_gen) return TLOAM_B200_ERR_NOT_READY;
+  CU_TRY(cudaSetDevice(h->device));
+  return loc_run(h, h->raw_scan, h->raw_n, guess, out);
+}
+
+int tloam_b200_localize(tloam_b200_handle* h, const double* xyz, size_t n, const double guess[16], tloam_localize_result* out) {
+  if (!h || !out || (!xyz && n) || n > ((size_t)1 << 30)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loc_on) return TLOAM_B200_ERR_NOT_READY;
+  CU_TRY(cudaSetDevice(h->device));
+  int rc;
+  if ((rc = ensure_dev(h, &h->d_loc_in, &h->cap_loc_in, n, false)) != TLOAM_B200_OK) return rc;
+  if (n && (rc = upload_host(h, h->d_loc_in, xyz, n * 24)) != TLOAM_B200_OK) return rc;
+  return loc_run(h, h->d_loc_in, n, guess, out);
+}
+
+int tloam_b200_localize_matches(tloam_b200_handle* h, int pass, int* index, double* d2, size_t capacity, size_t* n) {
+  if (!h || !n) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loc_on || !h->loc_ran) return TLOAM_B200_ERR_NOT_READY;
+  *n = h->loc_nq;
+  if (pass < 0 || pass >= h->loc_passes || capacity < h->loc_nq) return TLOAM_B200_ERR_INVALID_ARG;
+  const size_t nq = h->loc_nq;
+  const tloam_loc_args& a = h->loc_last;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (index) CU_TRY(cudaMemcpyAsync(index, a.match_index + (size_t)pass * nq, nq * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  if (d2) CU_TRY(cudaMemcpyAsync(d2, a.match_d2 + (size_t)pass * nq, nq * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_localize_query(tloam_b200_handle* h, double* xyz, size_t capacity, size_t* n) {
+  if (!h || !n) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loc_on || !h->loc_ran) return TLOAM_B200_ERR_NOT_READY;
+  CU_TRY(cudaSetDevice(h->device));
+  GMapState s;
+  CU_TRY(cudaMemcpyAsync(&s, loc_qst(h), sizeof(s), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  *n = s.n_vox;
+  if (capacity < *n || (!xyz && *n)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (*n) CU_TRY(cudaMemcpyAsync(xyz, h->d_loc_q, *n * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_localize_map_normals(tloam_b200_handle* h, double* normal, unsigned char* valid, int* neighbours, size_t capacity,
+                                    size_t* n) {
+  if (!h || !n) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loc_on || !h->loc_loaded) return TLOAM_B200_ERR_NOT_READY;
+  const size_t m = h->loc_n;
+  *n = m;
+  if (capacity < m) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!m) return TLOAM_B200_OK;
+  const tloam_loc_index_args& a = h->loc_index;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (normal) CU_TRY(cudaMemcpyAsync(normal, a.normal, m * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (valid) CU_TRY(cudaMemcpyAsync(valid, a.valid, m, cudaMemcpyDeviceToHost, h->stream));
+  if (neighbours) CU_TRY(cudaMemcpyAsync(neighbours, a.neighbours, m * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_localize_cells(tloam_b200_handle* h, unsigned* sorted_rows, unsigned long long* keys, unsigned* starts,
+                              size_t capacity, size_t* n_cells) {
+  if (!h || !n_cells) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loc_on || !h->loc_loaded) return TLOAM_B200_ERR_NOT_READY;
+  const tloam_loc_index_args& a = h->loc_index;
+  CU_TRY(cudaSetDevice(h->device));
+  unsigned long long nc = 0;
+  if (h->loc_n) {
+    CU_TRY(cudaMemcpyAsync(&nc, &a.st->n_vox, sizeof(nc), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+  }
+  *n_cells = nc;
+  if (capacity < h->loc_n) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loc_n) return TLOAM_B200_OK;
+  if (sorted_rows) CU_TRY(cudaMemcpyAsync(sorted_rows, a.srow, h->loc_n * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+  if (keys) CU_TRY(cudaMemcpyAsync(keys, a.ckey, nc * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+  if (starts) CU_TRY(cudaMemcpyAsync(starts, a.cstart, (nc + 1) * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
   CU_TRY(cudaStreamSynchronize(h->stream));
   return TLOAM_B200_OK;
 }

@@ -140,6 +140,23 @@ class LoopVerifyResult:
 
 
 @dataclasses.dataclass(frozen=True)
+class LocalizeResult:
+    """tloam_localize_result: T (4 x 4) = map <- sensor, T_map_odom = T . O_now^-1, guess = the G the run started from;
+    termination is one of LoopVerifyResult.CONVERGED .. EMPTY; accepted = converged and fitness <= max_fitness."""
+    T: np.ndarray
+    T_map_odom: np.ndarray
+    guess: np.ndarray
+    iterations: int
+    termination: int
+    accepted: bool
+    inliers: int
+    rmse: float
+    fitness: float
+    n_query_points: int
+    n_map_points: int
+
+
+@dataclasses.dataclass(frozen=True)
 class PoseGraphResult:
     """tloam_pose_graph_result: termination is one of PoseGraphResult.CONVERGED .. NO_LOOPS; the costs are sum r^T Omega r
     at the odometry poses and at the returned poses; step_* are the last step's largest |upsilon| / |omega| component."""
@@ -1120,6 +1137,95 @@ class LocalRegistration:
         self._check(self._L.tloam_b200_global_map_merged_download(self._h, 0, n.value, _dp(xyz), _dp(inten) if has else None),
                     "global_map_merged_download")
         return xyz, inten
+
+    # ---- localization in a prior map (include/tloam_b200.h "Localization in a prior map") ----
+    def localize_enable(self, **overrides):
+        """turn localization on and drop any loaded map; overrides: fields of tloam_localize_config (voxel, cell,
+        normal_radius, min_normal_neighbours, max_planarity, corr_dist_coarse, corr_dist_fine, max_iterations,
+        eps_translation, eps_rotation, max_fitness)"""
+        cfg = _lib.LocalizeConfig()
+        self._L.tloam_b200_localize_default_config(C.byref(cfg))
+        for k, v in overrides.items():
+            if not hasattr(cfg, k):
+                raise KeyError(k)
+            setattr(cfg, k, v)
+        self._check(self._L.tloam_b200_localize_enable(self._h, C.byref(cfg)), "localize_enable")
+
+    def localize_set_map(self, xyz):
+        """load a prior map (n x 3) and build its grid index and normals"""
+        p = np.ascontiguousarray(np.asarray(xyz, dtype=np.float64).reshape(-1, 3))
+        self._check(self._L.tloam_b200_localize_set_map(self._h, _dp(p) if len(p) else None, len(p)), "localize_set_map")
+
+    def localize_set_map_merged(self):
+        """load the last global_map_merged on the device as the prior map"""
+        self._check(self._L.tloam_b200_localize_set_map_merged(self._h), "localize_set_map_merged")
+
+    @staticmethod
+    def _localize_out(r):
+        f = lambda a: np.array(a[:]).reshape(4, 4, order="F")                                    # noqa: E731
+        return LocalizeResult(f(r.T), f(r.T_map_odom), f(r.guess), r.iterations, r.termination, bool(r.accepted), r.inliers,
+                              r.rmse, r.fitness, r.n_query_points, r.n_map_points)
+
+    def localize_frame(self, guess=None):
+        """localize the scan the last process_raw_scan left on the device, from guess (4 x 4, map <- sensor) or, with None,
+        from the prediction L_prev . O_prev^-1 . O_now.  Returns a LocalizeResult"""
+        g = None if guess is None else np.asarray(guess, dtype=np.float64).reshape(4, 4).ravel(order="F").copy()
+        r = _lib.LocalizeResult()
+        self._check(self._L.tloam_b200_localize_frame(self._h, None if g is None else _dp(g), C.byref(r)), "localize_frame")
+        return self._localize_out(r)
+
+    def localize(self, xyz, guess=None):
+        """localize a host cloud (n x 3); as localize_frame"""
+        p = np.ascontiguousarray(np.asarray(xyz, dtype=np.float64).reshape(-1, 3))
+        g = None if guess is None else np.asarray(guess, dtype=np.float64).reshape(4, 4).ravel(order="F").copy()
+        r = _lib.LocalizeResult()
+        self._check(self._L.tloam_b200_localize(self._h, _dp(p) if len(p) else None, len(p), None if g is None else _dp(g),
+                                                C.byref(r)), "localize")
+        return self._localize_out(r)
+
+    def localize_matches(self, k):
+        """the last localization's matches at pass k (k = iterations: the final pass): per query row the map row (-1:
+        none) and its d2"""
+        n = C.c_size_t(0)
+        rc = self._L.tloam_b200_localize_matches(self._h, int(k), None, None, 0, C.byref(n))
+        if rc != _lib.ERR_INVALID_ARG or n.value == 0:
+            self._check(rc, "localize_matches")
+        idx, d2 = np.zeros(n.value, dtype=np.int32), np.zeros(n.value)
+        self._check(self._L.tloam_b200_localize_matches(self._h, int(k), idx.ctypes.data_as(C.POINTER(C.c_int)), _dp(d2),
+                                                        n.value, C.byref(n)), "localize_matches")
+        return idx, d2
+
+    def localize_query(self):
+        """the last localization's query: the down-sampled scan (n x 3)"""
+        n = C.c_size_t(0)
+        rc = self._L.tloam_b200_localize_query(self._h, None, 0, C.byref(n))
+        if rc != _lib.ERR_INVALID_ARG or n.value == 0:
+            self._check(rc, "localize_query")
+        xyz = np.zeros((n.value, 3))
+        self._check(self._L.tloam_b200_localize_query(self._h, _dp(xyz), n.value, C.byref(n)), "localize_query")
+        return xyz
+
+    def localize_map_normals(self):
+        """the loaded map's (normal (n x 3), valid (n,) bool, neighbours (n,))"""
+        n = C.c_size_t(0)
+        rc = self._L.tloam_b200_localize_map_normals(self._h, None, None, None, 0, C.byref(n))
+        if rc != _lib.ERR_INVALID_ARG or n.value == 0:
+            self._check(rc, "localize_map_normals")
+        nrm, valid, cnt = np.zeros((n.value, 3)), np.zeros(n.value, dtype=np.uint8), np.zeros(n.value, dtype=np.int32)
+        self._check(self._L.tloam_b200_localize_map_normals(self._h, _dp(nrm), valid.ctypes.data_as(C.POINTER(C.c_ubyte)),
+                                                            cnt.ctypes.data_as(C.POINTER(C.c_int)), n.value, C.byref(n)),
+                    "localize_map_normals")
+        return nrm, valid.astype(bool), cnt
+
+    def localize_cells(self, n_rows):
+        """the loaded map's cell table: (sorted rows (n_rows,), cell keys (n_cells,), cell starts (n_cells + 1,))"""
+        nc = C.c_size_t(0)
+        rows, keys = np.zeros(n_rows, dtype=np.uint32), np.zeros(n_rows, dtype=np.uint64)
+        starts = np.zeros(n_rows + 1, dtype=np.uint32)
+        up = C.POINTER(C.c_uint)
+        self._check(self._L.tloam_b200_localize_cells(self._h, rows.ctypes.data_as(up), keys.ctypes.data_as(C.POINTER(C.c_ulonglong)),
+                                                      starts.ctypes.data_as(up), n_rows, C.byref(nc)), "localize_cells")
+        return rows, keys[:nc.value], starts[:nc.value + 1]
 
     # ---- shared map (multi-GPU) ----
     def map_blob_size(self):
