@@ -654,6 +654,9 @@ int tloam_b200_loop_size(tloam_b200_handle* h, size_t* n_frames);
 /* frame's descriptor to out: n_ring * n_sector bins (row-major), n_ring ring key values, n_sector column norms
  * (synchronises).  INVALID_ARG past the last frame. */
 int tloam_b200_loop_descriptor_download(tloam_b200_handle* h, size_t frame, double* out);
+/* the descriptors of frames [first, first + count), one slot after another, in one copy (synchronises): what
+ * tloam_b200_relocalize_set_places takes.  INVALID_ARG past the last frame. */
+int tloam_b200_loop_descriptors_download(tloam_b200_handle* h, size_t first, size_t count, double* out);
 
 /* ---- Loop verification (opt-in, on top of loop closure): a geometric check of a candidate that also gives the relative
  * pose a pose-graph edge needs.  Scan Context's yaw is one sector coarse and it gives no translation; a descriptor match
@@ -1199,6 +1202,94 @@ int tloam_b200_localize_map_normals(tloam_b200_handle* h, double* normal, unsign
  * starts (*n_cells + 1); capacity is that of sorted_rows and must be >= the map's rows (keys and starts need as many) */
 int tloam_b200_localize_cells(tloam_b200_handle* h, unsigned* sorted_rows, unsigned long long* keys, unsigned* starts,
                               size_t capacity, size_t* n_cells);
+
+/* ---- Relocalization in a prior map (opt-in, on top of localization): the pose of a scan in the map's frame without a
+ * guess -- the first frame after a load, or after tracking is lost -- from the places of a recorded session.
+ *   - Places.  Place j is a Scan Context descriptor (one slot of tloam_b200_loop_descriptor_download's layout: bins, ring
+ *     key, column norms) and a pose P_j (map <- sensor, column-major, rigid): in the mapping session the loop frames'
+ *     descriptors and their corrected poses (the pose graph's, or tloam_b200_global_map_frame_poses).  Loaded once, fixed
+ *     after the load; place j's identity is its index.
+ *   - Query descriptor.  The descriptor of the raw scan by the rule of "Loop closure", with this configuration's
+ *     lidar_height, n_ring, n_sector and max_radius (they must be the ones the places were made with; only the slot size
+ *     is checked).
+ *   - Candidates.  Per place its best shift, the minimum of (distance, shift) over every shift, the distance exactly
+ *     Scan Context's.  The places whose best distance is < max_distance, ordered by (distance, place); the first top_k are
+ *     the hypotheses, rank 0 .. n_hypotheses - 1.  There is no exclude_recent.
+ *   - Guess of hypothesis k (place j, shift s): G_k = P_j . Rz(yaw_s) with tloam_loop_result's yaw convention
+ *     (p_place ~ Rz(yaw) p_query).  cos and sin are the sector boundary table's: direction m = (-s) mod n_sector, direction 0
+ *     is (1, 0), direction m > 0 is (cos, sin)(2 pi m / n_sector) by the C library.  R_G(r, c) = (R_P(r, 0) Rz(0, c) +
+ *     R_P(r, 1) Rz(1, c)) + R_P(r, 2) Rz(2, c), each product and sum rounded on its own; t_G = t_P.
+ *   - Refinement.  Each hypothesis is exactly the run of "Localization in a prior map" from G_k: the same query, passes,
+ *     radius schedule, termination, fitness and accepted; hypothesis k's result is tloam_b200_localize(scan, G_k) on the
+ *     same map.
+ *   - Selection.  The winner is the accepted hypothesis minimal by (fitness, rank); without one, the hypothesis minimal by
+ *     (fitness, rank), reported but not accepted.  ambiguous: another accepted hypothesis has fitness <= ambiguity_ratio *
+ *     the winner's (rounded) and a pose distinct from the winner's: |t_a - t_b| (d2 as in "Loop verification", then sqrt)
+ *     > distinct_translation, or angle > distinct_rotation with angle = acos(clamp((tr - 1) * 0.5, -1, 1)), tr = the sum
+ *     over the 9 entries in row-major order of R_a(i, j) R_b(i, j) (= trace(R_a^T R_b)), evaluated as clamp(...) <
+ *     cos(distinct_rotation).  accepted = the winner is accepted and the result is not ambiguous.  T_map_odom = T . O_now^-1
+ *     by the localization's rule.
+ *   - Effect.  An accepted relocalization writes the localization's prediction memory as an accepted localization does
+ *     (L = T, O = O_now), so the next tloam_b200_localize_frame(NULL) predicts from it.  A rejected one changes no
+ *     localization state.  tloam_b200_localize_query / _matches keep describing the last tloam_b200_localize*.  Nothing
+ *     else is written: odometry, pose history, submap, global map, loop database, pose graph, and every other call's
+ *     launch counts.  No candidate: OK, n_hypotheses 0, place -1, T identity, not accepted.
+ *   - Device.  k_sc_bin / k_sc_finish (libtloam_b200_loop.so) into a slot of its own, the query's down-sample (one
+ *     read-back of its size), then k_rl_search, k_rl_topk, k_rl_guess and the K hypotheses' ICP in one launch sequence
+ *     (k_rl_match / k_rl_reduce over query blocks x top_k, k_rl_step and k_rl_final one warp per hypothesis), k_rl_select,
+ *     and one copy home.  The kernels live in libtloam_b200_reloc.so, loaded from this library's directory by the enable
+ *     call (ERR_CUDA if it is missing). */
+typedef struct tloam_relocalize_config {
+  double lidar_height;                 /* the descriptor's, as tloam_loop_config */
+  int n_ring, n_sector;
+  double max_radius;                   /* m */
+  int top_k;                           /* hypotheses, 1 .. 64 */
+  double max_distance;                 /* a place is a candidate below this Scan Context distance */
+  double distinct_translation;         /* m */
+  double distinct_rotation;            /* rad */
+  double ambiguity_ratio;              /* >= 1 */
+} tloam_relocalize_config;
+typedef struct tloam_relocalize_hypothesis {
+  long long place;
+  int shift;
+  double distance;                     /* the place's Scan Context distance at that shift */
+  tloam_localize_result result;        /* its run from G_k (result.guess) */
+} tloam_relocalize_hypothesis;
+typedef struct tloam_relocalize_result {
+  tloam_localize_result result;        /* the winner's run */
+  long long place;                     /* the winner's place, -1 without hypotheses */
+  int shift;
+  double distance;
+  int n_hypotheses;
+  int winner;                          /* its rank, -1 without hypotheses */
+  int ambiguous;
+  int accepted;
+} tloam_relocalize_result;
+/* the loop closure's descriptor shape, top_k 8, max_distance 0.4, distinct_translation 2 m, distinct_rotation 10 deg,
+ * ambiguity_ratio 1.5 (DESIGN.md section 4c has how they were checked) */
+void tloam_b200_relocalize_default_config(tloam_relocalize_config* c);
+/* turns relocalization on (or re-configures it) and drops the places.  NOT_READY: localization off.  INVALID_ARG: cfg
+ * null, the descriptor shape as tloam_b200_loop_enable refuses it, top_k outside [1, 64], a value not finite,
+ * distinct_translation or distinct_rotation < 0, ambiguity_ratio < 1. */
+int tloam_b200_relocalize_enable(tloam_b200_handle* h, const tloam_relocalize_config* cfg);
+/* loads n places from HOST arrays: n descriptor slots and n poses (16 each, column-major).  NOT_READY: relocalization
+ * off.  INVALID_ARG: a null array with n > 0, a non-finite value.  BAD_POSE: a pose not rigid.  A refused load leaves
+ * no places. */
+int tloam_b200_relocalize_set_places(tloam_b200_handle* h, const double* descriptors, const double* poses, size_t n);
+/* the same with the handle's own loop database as the descriptors, copied on the device.  NOT_READY: relocalization or
+ * loop closure off.  INVALID_ARG: n != tloam_b200_loop_size, or a descriptor shape other than the loop closure's. */
+int tloam_b200_relocalize_set_places_loop(tloam_b200_handle* h, const double* poses, size_t n);
+/* relocalizes the scan the last tloam_b200_process_raw_scan* left on the device and returns once the result is home.
+ * NOT_READY: relocalization off, no map, no places, or no such scan (tloam_b200_localize_frame's rule).  VOXEL_RANGE: the
+ * query's extent. */
+int tloam_b200_relocalize_frame(tloam_b200_handle* h, tloam_relocalize_result* out);
+/* the same for a HOST cloud (n x 3) */
+int tloam_b200_relocalize(tloam_b200_handle* h, const double* xyz, size_t n, tloam_relocalize_result* out);
+/* the last relocalization's hypotheses in rank order (*n = n_hypotheses; INVALID_ARG if capacity < *n) */
+int tloam_b200_relocalize_hypotheses(tloam_b200_handle* h, tloam_relocalize_hypothesis* out, size_t capacity, size_t* n);
+/* the last relocalization's matches of hypothesis k at pass p (0 .. its iterations), as tloam_b200_localize_matches */
+int tloam_b200_relocalize_matches(tloam_b200_handle* h, int hypothesis, int pass, int* index, double* d2, size_t capacity,
+                                  size_t* n);
 
 /* Pinned host memory helpers (optional; pinned inputs make set_* a direct DMA, no staging threads). */
 int tloam_b200_host_alloc(void** p, size_t bytes);

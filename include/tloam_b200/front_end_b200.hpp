@@ -18,6 +18,8 @@
 // Context descriptor per frame and an exact search over every earlier frame, on the GPU; enableLoopVerification / verifyLoop
 // check a candidate by a scan-to-scan ICP of down-sampled keyframes kept on the GPU and give the relative pose;
 // enableSubmapVerification / verifyLoopSubmap check it against the keyframes around the candidate, point to plane.
+// enableLocalization / localizeFrame register each frame against a prior map; enableRelocalization / setPlaces /
+// relocalizeFrame find the first pose in that map (or the pose after tracking is lost) from a recorded session's places.
 // Without the reference headers (this repository's tests) define TLOAM_B200_MOCK_HOST_TYPES and provide the host types
 // (tests/mock/mock_tloam.hpp).
 #ifndef TLOAM_B200_FRONT_END_B200_HPP
@@ -340,6 +342,49 @@ class FrontEndB200 {
     return report(tloam_b200_localize(h_, data(scan), size(scan), guess ? guess->matrix().data() : nullptr, &out), "localize");
   }
 
+  // Relocalization in a prior map (include/tloam_b200.h "Relocalization in a prior map"): the places of a recorded session
+  // (its loop frames' descriptors, as loopDescriptors returns them, and their poses) are loaded once; relocalizeFrame then
+  // finds the pose of the processed scan in the map without a guess, and an accepted result seeds the next
+  // localizeFrame(out, nullptr).  Needs enableLocalization and a prior map.
+  bool enableRelocalization(const tloam_relocalize_config& cfg) {
+    const bool ok = report(tloam_b200_relocalize_enable(h_, &cfg), "enableRelocalization");
+    if (ok) place_slot_ = (size_t)cfg.n_ring * cfg.n_sector + cfg.n_ring + cfg.n_sector;
+    return ok;
+  }
+  bool enableRelocalization() {
+    tloam_relocalize_config c;
+    tloam_b200_relocalize_default_config(&c);
+    return enableRelocalization(c);
+  }
+  // the loop database's descriptors, one slot after another (what setPlaces takes); the slot is enableRelocalization's,
+  // which must have the loop detection's shape
+  bool loopDescriptors(std::vector<double>& out) {
+    if (!place_slot_) return report(TLOAM_B200_ERR_NOT_READY, "loopDescriptors");
+    size_t n = 0;
+    if (!report(tloam_b200_loop_size(h_, &n), "loopDescriptors")) return false;
+    out.resize(n * place_slot_);
+    return report(tloam_b200_loop_descriptors_download(h_, 0, n, n ? out.data() : nullptr), "loopDescriptors");
+  }
+  // descriptors: poses.size() slots of enableRelocalization's shape; poses: map <- sensor
+  bool setPlaces(const std::vector<double>& descriptors, const std::vector<Eigen::Isometry3d>& poses) {
+    if (descriptors.size() != poses.size() * place_slot_) return report(TLOAM_B200_ERR_INVALID_ARG, "setPlaces");
+    const std::vector<double> p = columnMajor(poses);
+    return report(tloam_b200_relocalize_set_places(h_, descriptors.empty() ? nullptr : descriptors.data(), p.empty() ? nullptr : p.data(),
+                                                    poses.size()),
+                  "setPlaces");
+  }
+  // the handle's own loop database as the descriptors, one pose per loop frame
+  bool setPlacesFromLoop(const std::vector<Eigen::Isometry3d>& poses) {
+    const std::vector<double> p = columnMajor(poses);
+    return report(tloam_b200_relocalize_set_places_loop(h_, p.empty() ? nullptr : p.data(), poses.size()), "setPlacesFromLoop");
+  }
+  // the scan the handle processed last
+  bool relocalizeFrame(tloam_relocalize_result& out) { return report(tloam_b200_relocalize_frame(h_, &out), "relocalizeFrame"); }
+  // a host cloud
+  bool relocalize(const CloudData& scan, tloam_relocalize_result& out) {
+    return report(tloam_b200_relocalize(h_, data(scan), size(scan), &out), "relocalize");
+  }
+
   // processCloud + setInputSource (ref: front_end.cpp:181-199, :313): the three clouds the segmentation nodelet publishes
   bool processCloud(CloudData& ground, CloudData& edge, CloudData& general) {
     return report(tloam_b200_process_cloud(h_, &fcfg_, ground_down_sample_, edge_down_sample_, data(ground), size(ground), data(edge),
@@ -369,6 +414,12 @@ class FrontEndB200 {
     return c.cloud_ptr->points_.empty() ? nullptr : reinterpret_cast<const double*>(c.cloud_ptr->points_.data());
   }
   static size_t size(const CloudData& c) { return c.cloud_ptr->points_.size(); }
+  static std::vector<double> columnMajor(const std::vector<Eigen::Isometry3d>& poses) {
+    std::vector<double> out(16 * poses.size());
+    for (size_t j = 0; j < poses.size(); ++j)
+      for (int i = 0; i < 16; ++i) out[16 * j + i] = poses[j].matrix().data()[i];
+    return out;
+  }
   static bool hasIntensity(const CloudData& c) {                     // PointCloud2::HasIntensity (PointCloud2.hpp:108-110)
     return !c.cloud_ptr->intensity_.empty() && c.cloud_ptr->intensity_.size() == c.cloud_ptr->points_.size();
   }
@@ -386,6 +437,7 @@ class FrontEndB200 {
   size_t n_source_[4] = {0, 0, 0, 0};
   bool mapping_ = false;
   bool loop_ = false;
+  size_t place_slot_ = 0;               // descriptor slot of enableRelocalization's shape
   int last_status_ = TLOAM_B200_OK;
 };
 

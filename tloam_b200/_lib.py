@@ -112,6 +112,24 @@ class LocalizeResult(C.Structure):
                 ("n_map_points", C.c_longlong)]
 
 
+class RelocalizeConfig(C.Structure):
+    """tloam_relocalize_config (include/tloam_b200.h "Relocalization in a prior map")."""
+    _fields_ = [("lidar_height", C.c_double), ("n_ring", C.c_int), ("n_sector", C.c_int), ("max_radius", C.c_double),
+                ("top_k", C.c_int), ("max_distance", C.c_double), ("distinct_translation", C.c_double),
+                ("distinct_rotation", C.c_double), ("ambiguity_ratio", C.c_double)]
+
+
+class RelocalizeHypothesis(C.Structure):
+    """tloam_relocalize_hypothesis: a candidate place, its shift and distance, and its run."""
+    _fields_ = [("place", C.c_longlong), ("shift", C.c_int), ("distance", C.c_double), ("result", LocalizeResult)]
+
+
+class RelocalizeResult(C.Structure):
+    """tloam_relocalize_result: the winner's run, its place, and the selection."""
+    _fields_ = [("result", LocalizeResult), ("place", C.c_longlong), ("shift", C.c_int), ("distance", C.c_double),
+                ("n_hypotheses", C.c_int), ("winner", C.c_int), ("ambiguous", C.c_int), ("accepted", C.c_int)]
+
+
 class PoseGraphConfig(C.Structure):
     """tloam_pose_graph_config (include/tloam_b200.h "Pose graph"): the edges' sigmas and the Gauss-Newton schedule."""
     _fields_ = [("sigma_odom_translation", C.c_double), ("sigma_odom_rotation", C.c_double),
@@ -252,6 +270,9 @@ EXPORTS = [
     "tloam_b200_localize_default_config", "tloam_b200_localize_enable", "tloam_b200_localize_set_map",
     "tloam_b200_localize_set_map_merged", "tloam_b200_localize_frame", "tloam_b200_localize", "tloam_b200_localize_matches",
     "tloam_b200_localize_query", "tloam_b200_localize_map_normals", "tloam_b200_localize_cells",
+    "tloam_b200_loop_descriptors_download", "tloam_b200_relocalize_default_config", "tloam_b200_relocalize_enable",
+    "tloam_b200_relocalize_set_places", "tloam_b200_relocalize_set_places_loop", "tloam_b200_relocalize_frame",
+    "tloam_b200_relocalize", "tloam_b200_relocalize_hypotheses", "tloam_b200_relocalize_matches",
 ]
 
 _lib = None
@@ -465,5 +486,15 @@ def load():
     L.tloam_b200_localize_query.argtypes = [vp, dp, C.c_size_t, szp]
     L.tloam_b200_localize_map_normals.argtypes = [vp, dp, C.POINTER(C.c_ubyte), C.POINTER(C.c_int), C.c_size_t, szp]
     L.tloam_b200_localize_cells.argtypes = [vp, up, C.POINTER(C.c_ulonglong), up, C.c_size_t, szp]
+    L.tloam_b200_loop_descriptors_download.argtypes = [vp, C.c_size_t, C.c_size_t, dp]
+    L.tloam_b200_relocalize_default_config.argtypes = [C.POINTER(RelocalizeConfig)]
+    L.tloam_b200_relocalize_default_config.restype = None
+    L.tloam_b200_relocalize_enable.argtypes = [vp, C.POINTER(RelocalizeConfig)]
+    L.tloam_b200_relocalize_set_places.argtypes = [vp, dp, dp, C.c_size_t]
+    L.tloam_b200_relocalize_set_places_loop.argtypes = [vp, dp, C.c_size_t]
+    L.tloam_b200_relocalize_frame.argtypes = [vp, C.POINTER(RelocalizeResult)]
+    L.tloam_b200_relocalize.argtypes = [vp, dp, C.c_size_t, C.POINTER(RelocalizeResult)]
+    L.tloam_b200_relocalize_hypotheses.argtypes = [vp, C.POINTER(RelocalizeHypothesis), C.c_size_t, szp]
+    L.tloam_b200_relocalize_matches.argtypes = [vp, C.c_int, C.c_int, C.POINTER(C.c_int), dp, C.c_size_t, szp]
     _lib = L
     return L

@@ -1,6 +1,6 @@
 """In-tree build of libtloam_b200.so, libtloam_b200_gmi.so, libtloam_b200_unpack.so, libtloam_b200_deskew.so,
 libtloam_b200_loop.so, libtloam_b200_loopv.so, libtloam_b200_pg.so, libtloam_b200_gmc.so, libtloam_b200_pgr.so,
-libtloam_b200_loopvs.so, libtloam_b200_gmd.so, libtloam_b200_gmm.so and libtloam_b200_loc.so
+libtloam_b200_loopvs.so, libtloam_b200_gmd.so, libtloam_b200_gmm.so, libtloam_b200_loc.so and libtloam_b200_reloc.so
 (hand-written CUDA for sm_90a; no torch, no CPU fallback).
 
     python -m tloam_b200.build [--force]
@@ -13,7 +13,8 @@ libtloam_b200_pg.so the pose-graph kernels (csrc/pose_graph.cu), libtloam_b200_g
 loop-closure correction (csrc/map_correct.cu), libtloam_b200_pgr.so the robust pose graph's loop-edge weights
 (csrc/pose_graph_robust.cu), libtloam_b200_loopvs.so the loop verification against a submap (csrc/loop_verify_submap.cu), libtloam_b200_gmd.so the
 global map's dynamic-point removal (csrc/map_dynamic.cu), libtloam_b200_gmm.so the merge of the global map into one voxel
-grid (csrc/map_merge.cu), libtloam_b200_loc.so the localization in a prior map (csrc/localize.cu); libtloam_b200.so loads each from its own directory when first needed.
+grid (csrc/map_merge.cu), libtloam_b200_loc.so the localization in a prior map (csrc/localize.cu), libtloam_b200_reloc.so the relocalization in a
+prior map (csrc/relocalize.cu); libtloam_b200.so loads each from its own directory when first needed.
 """
 import os
 import subprocess
@@ -47,6 +48,8 @@ GMM_LIB = os.path.join(HERE, "libtloam_b200_gmm.so")
 GMM_SOURCES = [os.path.join(CSRC, "map_merge.cu")]
 LOC_LIB = os.path.join(HERE, "libtloam_b200_loc.so")
 LOC_SOURCES = [os.path.join(CSRC, "localize.cu")]
+RELOC_LIB = os.path.join(HERE, "libtloam_b200_reloc.so")
+RELOC_SOURCES = [os.path.join(CSRC, "relocalize.cu")]
 import glob
 # every header the translation unit can include: editing any of them triggers a rebuild
 HEADERS = sorted(glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(CSRC, "*.h")) +
@@ -78,11 +81,11 @@ def _nvcc(lib, sources, verbose, extra):
 
 
 def build(force=False, verbose=False, extra=()):
-    """builds the thirteen libraries (each only when out of date); returns the path of libtloam_b200.so"""
+    """builds the fourteen libraries (each only when out of date); returns the path of libtloam_b200.so"""
     for lib, sources in ((LIB, SOURCES), (GMI_LIB, GMI_SOURCES), (UNPACK_LIB, UNPACK_SOURCES), (DESKEW_LIB, DESKEW_SOURCES),
                          (LOOP_LIB, LOOP_SOURCES), (LOOPV_LIB, LOOPV_SOURCES), (PG_LIB, PG_SOURCES), (GMC_LIB, GMC_SOURCES),
                          (PGR_LIB, PGR_SOURCES), (LOOPVS_LIB, LOOPVS_SOURCES), (GMD_LIB, GMD_SOURCES),
-                         (GMM_LIB, GMM_SOURCES), (LOC_LIB, LOC_SOURCES)):
+                         (GMM_LIB, GMM_SOURCES), (LOC_LIB, LOC_SOURCES), (RELOC_LIB, RELOC_SOURCES)):
         if force or needs_build(lib, sources):
             _nvcc(lib, sources, verbose, extra)
     return LIB

@@ -14,6 +14,7 @@
 #include <cuda_runtime.h>
 #include <math.h>
 
+#include "scan_context.cuh"
 #include "scan_context.h"
 
 namespace tloam {
@@ -87,10 +88,6 @@ __global__ void __launch_bounds__(kScThreads) k_sc_finish(tloam_sc_args a) {
   }
 }
 
-__device__ __forceinline__ bool sc_less(double d1, long long j1, long long s1, double d2, long long j2, long long s2) {
-  return d1 < d2 || (d1 == d2 && (j1 < j2 || (j1 == j2 && s1 < s2)));
-}
-
 // the block's minimum of (d, j, s) into *out (thread 0)
 __device__ void sc_block_min(double d, long long j, long long s, tloam_sc_best* out) {
   __shared__ tloam_sc_best wb[kScThreads / 32];
@@ -110,9 +107,7 @@ __device__ void sc_block_min(double d, long long j, long long s, tloam_sc_best* 
 }
 
 // Each block holds the query in shared memory and streams groups of `per_block` candidates through it; thread p of a group
-// takes candidate p / S at shift s = p % S.  For shift s candidate column (c - s) mod S meets query column c; a column pair
-// counts when both norms are non-zero, and its cosine is (sum over rings of a * b) / (|a| * |b|).  The distance is
-// 1 - (sum of the cosines in ascending c) / count, or 1 when no column counts.  Each block's minimum goes to a.partial.
+// takes candidate p / S at shift s = p % S, at sc_distance (scan_context.cuh).  Each block's minimum goes to a.partial.
 __global__ void __launch_bounds__(kScThreads) k_sc_search(tloam_sc_args a, int per_block) {
   extern __shared__ double sm[];
   const int R = a.n_ring, S = a.n_sector;
@@ -138,21 +133,7 @@ __global__ void __launch_bounds__(kScThreads) k_sc_search(tloam_sc_args a, int p
       const unsigned long long j = g * per_block + m;
       if (j >= M) continue;
       const double* cb = sm + desc + (size_t)m * desc;
-      const double* cn = cb + bins;
-      double sum = 0.0;
-      int count = 0;
-      int cc = s == 0 ? 0 : S - s;                         // (c - s) mod S at c = 0
-      for (int c = 0; c < S; ++c) {
-        const double na = qn[c], nb = cn[cc];
-        if (na != 0.0 && nb != 0.0) {
-          double dot = 0.0;
-          for (int r = 0; r < R; ++r) dot = __dadd_rn(dot, __dmul_rn(qb[r * S + c], cb[r * S + cc]));
-          sum = __dadd_rn(sum, __ddiv_rn(dot, __dmul_rn(na, nb)));
-          ++count;
-        }
-        if (++cc == S) cc = 0;
-      }
-      const double dist = count ? __dsub_rn(1.0, __ddiv_rn(sum, (double)count)) : 1.0;
+      const double dist = sc_distance(qb, qn, cb, cb + bins, R, S, s);
       if (sc_less(dist, (long long)j, s, bd, bj, bs)) { bd = dist; bj = (long long)j; bs = s; }
     }
   }

@@ -38,6 +38,7 @@
 #include "map_dynamic.h"
 #include "map_merge.h"
 #include "localize.h"
+#include "relocalize.h"
 
 
 
@@ -294,6 +295,16 @@ struct tloam_b200_handle {
   unsigned char* d_loc_run = nullptr;      size_t cap_loc_run = 0;     // state, memory, partials, matches
   bool loc_have_prev = false;              // a localization since the load: the prediction has its memory
   bool loc_ran = false;                    int loc_passes = 0;  size_t loc_nq = 0;   tloam_loc_args loc_last;
+  // ---- relocalization in a prior map (tloam_b200_relocalize*, libtloam_b200_reloc.so): the places (descriptor slots,
+  //      poses, per-place best distance and shift in one buffer), the query's descriptor and down-sample, the batch ----
+  bool rl_on = false;                      tloam_relocalize_config rl_cfg;
+  double* d_rl_dirs = nullptr;             // sector boundary directions of rl_cfg.n_sector
+  unsigned char* d_rl_places = nullptr;    size_t cap_rl_places = 0;  size_t rl_n = 0;  bool rl_loaded = false;
+  unsigned char* d_rl_small = nullptr;     // the query's GMapState at 0, its descriptor slot at 256
+  double* d_rl_q = nullptr;                size_t cap_rl_q = 0;
+  unsigned char* d_rl_run = nullptr;       size_t cap_rl_run = 0;     // states, candidates, partials, matches
+  bool rl_ran = false;                     size_t rl_nq = 0, rl_qn = 0;  tloam_rl_args rl_last;   // rl_qn: query rows
+  std::vector<tloam_loc_state> rl_states;  tloam_rl_top rl_top;
   // ---- pose graph (tloam_b200_pose_graph*, libtloam_b200_pg.so): the node store on the device, the loop edges on the
   //      host until an optimisation uploads them; nothing is allocated or launched until it is enabled ----
   bool pg_on = false;
@@ -513,6 +524,7 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   cudaFree(h->d_gmm_scratch); cudaFree(h->d_gmm_out);
   cudaFree(h->d_loc_map); cudaFree(h->d_loc_scratch); cudaFree(h->d_loc_qst); cudaFree(h->d_loc_reg); cudaFree(h->d_loc_fin);
   cudaFree(h->d_loc_q); cudaFree(h->d_loc_in); cudaFree(h->d_loc_run);
+  cudaFree(h->d_rl_dirs); cudaFree(h->d_rl_places); cudaFree(h->d_rl_small); cudaFree(h->d_rl_q); cudaFree(h->d_rl_run);
   for (int i = 0; i < 2; ++i) if (h->ev_stage_free[i]) cudaEventDestroy(h->ev_stage_free[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_fit[i]) cudaEventDestroy(h->ev_fit[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_res[i]) cudaEventDestroy(h->ev_res[i]);
@@ -4149,6 +4161,18 @@ int tloam_b200_loop_descriptor_download(tloam_b200_handle* h, size_t frame, doub
   return TLOAM_B200_OK;
 }
 
+int tloam_b200_loop_descriptors_download(tloam_b200_handle* h, size_t first, size_t count, double* out) {
+  if (!h || (!out && count)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loop_on) return TLOAM_B200_ERR_NOT_READY;
+  if (first > h->loop_frames || count > h->loop_frames - first) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!count) return TLOAM_B200_OK;
+  const size_t slot = TLOAM_SC_SLOT_DOUBLES(h->loop_cfg.n_ring, h->loop_cfg.n_sector);
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaMemcpyAsync(out, h->d_loop_db + first * slot, count * slot * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
 // ---------------------------------------------------------------------------------------------
 // Loop verification (a keyframe per loop frame, by the global map's ordered path into buffers of its own; the commit and
 // the ICP kernels in loop_verify.cu, loaded from libtloam_b200_loopv.so on the first verification call).
@@ -5630,13 +5654,13 @@ int tloam_b200_localize_set_map_merged(tloam_b200_handle* h) {
 }
 
 // the query: VoxelDownSample(voxel) of the finite rows of the n rows at d_in by the global map's ordered path at pose I
-// (the keyframe path of loop verification, in buffers of its own); synchronises and returns its row count
-static int loc_query(tloam_b200_handle* h, const double* d_in, size_t n, size_t* nq) {
+// (the keyframe path of loop verification, in buffers of its own) into *q with its state at st (the localization's, or
+// relocalization's own); synchronises and returns its row count
+static int loc_query(tloam_b200_handle* h, const double* d_in, size_t n, size_t* nq, GMapState* st, double** q, size_t* cap_q) {
   int rc;
   if ((rc = ensure_dev(h, &h->d_loc_reg, &h->cap_loc_reg, n, false)) != TLOAM_B200_OK) return rc;
   if ((rc = ensure_dev(h, &h->d_loc_fin, &h->cap_loc_fin, n, false)) != TLOAM_B200_OK) return rc;
-  if ((rc = ensure_dev(h, &h->d_loc_q, &h->cap_loc_q, n, false)) != TLOAM_B200_OK) return rc;
-  GMapState* st = loc_qst(h);
+  if ((rc = ensure_dev(h, q, cap_q, n, false)) != TLOAM_B200_OK) return rc;
   const double voxel = h->loc_cfg.voxel;
   CU_TRY(cudaMemsetAsync(st, 0, sizeof(GMapState), h->stream));
   const unsigned tb = 256, gb = (unsigned)((n + tb - 1) / tb);
@@ -5645,7 +5669,7 @@ static int loc_query(tloam_b200_handle* h, const double* d_in, size_t n, size_t*
   VoxSorted vs;
   if ((rc = voxel_pipeline(h, h->d_loc_fin, n, &st->n_fin, 0u, nullptr, nullptr, nullptr, 0.0, voxel, nullptr, &st->n_vox,
                            h->stream, 0, &vs)) != TLOAM_B200_OK) return rc;
-  if (n) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_emit<<<gb, tb, 0, h->stream>>>(vs.a, vs.slots, h->d_loc_q, st, h->cap_loc_q)));
+  if (n) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_emit<<<gb, tb, 0, h->stream>>>(vs.a, vs.slots, *q, st, *cap_q)));
   CU_TRY(cudaGetLastError());
   GMapState s;
   CU_TRY(cudaMemcpyAsync(&s, st, sizeof(s), cudaMemcpyDeviceToHost, h->stream));
@@ -5663,7 +5687,7 @@ static int loc_run(tloam_b200_handle* h, const double* d_in, size_t n, const dou
   int rc = loc_load(h, &lib);
   if (rc != TLOAM_B200_OK) return rc;
   size_t nq = 0;
-  if ((rc = loc_query(h, d_in, n, &nq)) != TLOAM_B200_OK) return rc;
+  if ((rc = loc_query(h, d_in, n, &nq, loc_qst(h), &h->d_loc_q, &h->cap_loc_q)) != TLOAM_B200_OK) return rc;
   const tloam_localize_config& c = h->loc_cfg;
   const size_t nr = h->loc_n ? nq : 0;                          // an empty map: nothing to match (EMPTY)
   const size_t passes = (size_t)c.max_iterations + 1, qb = (nr + TLOAM_LOC_THREADS - 1) / TLOAM_LOC_THREADS;
@@ -5804,6 +5828,310 @@ int tloam_b200_localize_cells(tloam_b200_handle* h, unsigned* sorted_rows, unsig
   if (sorted_rows) CU_TRY(cudaMemcpyAsync(sorted_rows, a.srow, h->loc_n * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
   if (keys) CU_TRY(cudaMemcpyAsync(keys, a.ckey, nc * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
   if (starts) CU_TRY(cudaMemcpyAsync(starts, a.cstart, (nc + 1) * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Relocalization in a prior map (the checks, the places, the query's descriptor and down-sample and the buffers here; the
+// kernels in relocalize.cu, loaded from libtloam_b200_reloc.so by the enable call, and the descriptor's in scan_context.cu).
+// ---------------------------------------------------------------------------------------------
+static std::mutex g_rl_mu;
+static tloam_rl_run_fn g_rl_run = nullptr;
+
+static int rl_load(tloam_b200_handle* h, tloam_rl_run_fn* out) {
+  std::lock_guard<std::mutex> lk(g_rl_mu);
+  if (!g_rl_run) {
+    const std::string path = sibling_path("libtloam_b200_reloc.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    tloam_rl_run_fn f = so ? reinterpret_cast<tloam_rl_run_fn>(dlsym(so, "tloam_rl_run")) : nullptr;
+    if (!f) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "relocalization: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_rl_run = f;
+  }
+  *out = g_rl_run;
+  return TLOAM_B200_OK;
+}
+
+// d_rl_small: the query's GMapState at 0, its descriptor slot at 256
+static_assert(sizeof(GMapState) <= 256, "the query's GMapState must fit below its descriptor slot");
+
+static size_t rl_slot(const tloam_relocalize_config& c) { return TLOAM_SC_SLOT_DOUBLES(c.n_ring, c.n_sector); }
+
+void tloam_b200_relocalize_default_config(tloam_relocalize_config* c) {
+  tloam_loop_config l;
+  tloam_b200_loop_default_config(&l);
+  c->lidar_height = l.lidar_height; c->n_ring = l.n_ring; c->n_sector = l.n_sector; c->max_radius = l.max_radius;
+  c->top_k = 8; c->max_distance = 0.4;
+  c->distinct_translation = 2.0; c->distinct_rotation = 10.0 * M_PI / 180.0; c->ambiguity_ratio = 1.5;
+}
+
+int tloam_b200_relocalize_enable(tloam_b200_handle* h, const tloam_relocalize_config* c) {
+  if (!h || !c || c->n_ring < 1 || c->n_sector < 1 || (long long)c->n_ring * c->n_sector > 4096 || !std::isfinite(c->max_radius) ||
+      !(c->max_radius > 0.0) || !std::isfinite(c->lidar_height) || c->top_k < 1 || c->top_k > TLOAM_RL_MAX_K ||
+      !std::isfinite(c->max_distance) || !std::isfinite(c->distinct_translation) || !(c->distinct_translation >= 0.0) ||
+      !std::isfinite(c->distinct_rotation) || !(c->distinct_rotation >= 0.0) || !std::isfinite(c->ambiguity_ratio) ||
+      !(c->ambiguity_ratio >= 1.0))
+    return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loc_on) return TLOAM_B200_ERR_NOT_READY;
+  tloam_rl_run_fn run;
+  int rc = rl_load(h, &run);
+  if (rc != TLOAM_B200_OK) return rc;
+  LoopLib lib;
+  if ((rc = loop_load(h, &lib)) != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  h->rl_on = false; h->rl_loaded = false; h->rl_ran = false;   // until the new configuration is in place
+  if (!h->d_rl_small) CU_TRY(cudaMalloc(&h->d_rl_small, 256 + 4096 * 3 * sizeof(double)));
+  cudaFree(h->d_rl_dirs); h->d_rl_dirs = nullptr;
+  std::vector<double> dirs(2 * (size_t)c->n_sector);           // the loop closure's table: the same bits
+  for (int k = 1; k < c->n_sector; ++k) {
+    const double t = 2.0 * M_PI * k / c->n_sector;
+    dirs[2 * (k - 1)] = std::cos(t);
+    dirs[2 * (k - 1) + 1] = std::sin(t);
+  }
+  CU_TRY(cudaMalloc(&h->d_rl_dirs, dirs.size() * sizeof(double)));
+  CU_TRY(cudaMemcpy(h->d_rl_dirs, dirs.data(), dirs.size() * sizeof(double), cudaMemcpyHostToDevice));
+  h->rl_cfg = *c;
+  h->rl_on = true;
+  h->rl_loaded = false; h->rl_n = 0; h->rl_ran = false;
+  return TLOAM_B200_OK;
+}
+
+// room for n places: slots, poses, each place's best distance and shift
+static int rl_reserve(tloam_b200_handle* h, size_t n, size_t* o_pose, size_t* o_dist, size_t* o_shift) {
+  const size_t slot = rl_slot(h->rl_cfg);
+  size_t o = round_up(n * slot * sizeof(double), 256);
+  *o_pose = o;  o += round_up(n * 16 * sizeof(double), 256);
+  *o_dist = o;  o += round_up(n * sizeof(double), 256);
+  *o_shift = o; o += n * sizeof(long long);
+  if (o > h->cap_rl_places) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_rl_places); h->d_rl_places = nullptr; h->cap_rl_places = 0;
+    CU_TRY(cudaMalloc(&h->d_rl_places, o ? o : 256));
+    h->cap_rl_places = o ? o : 256;
+  }
+  return TLOAM_B200_OK;
+}
+
+static int rl_check_poses(const double* poses, size_t n) {
+  for (size_t j = 0; j < 16 * n; ++j)
+    if (!std::isfinite(poses[j])) return TLOAM_B200_ERR_INVALID_ARG;
+  for (size_t j = 0; j < n; ++j)
+    if (!pg_rigid(poses + 16 * j)) return TLOAM_B200_ERR_BAD_POSE;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_relocalize_set_places(tloam_b200_handle* h, const double* descriptors, const double* poses, size_t n) {
+  if (!h || (n && (!descriptors || !poses))) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->rl_on) return TLOAM_B200_ERR_NOT_READY;
+  const size_t slot = rl_slot(h->rl_cfg);
+  for (size_t j = 0; j < n * slot; ++j)
+    if (!std::isfinite(descriptors[j])) return TLOAM_B200_ERR_INVALID_ARG;
+  int rc = rl_check_poses(poses, n);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  h->rl_loaded = false;
+  size_t op, od, os;
+  if ((rc = rl_reserve(h, n, &op, &od, &os)) != TLOAM_B200_OK) return rc;
+  if (n && (rc = upload_host(h, h->d_rl_places, descriptors, n * slot * sizeof(double))) != TLOAM_B200_OK) return rc;
+  if (n && (rc = upload_host(h, h->d_rl_places + op, poses, n * 16 * sizeof(double))) != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  h->rl_n = n; h->rl_loaded = true;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_relocalize_set_places_loop(tloam_b200_handle* h, const double* poses, size_t n) {
+  if (!h || (n && !poses)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->rl_on || !h->loop_on) return TLOAM_B200_ERR_NOT_READY;
+  if (n != h->loop_frames || h->loop_cfg.n_ring != h->rl_cfg.n_ring || h->loop_cfg.n_sector != h->rl_cfg.n_sector)
+    return TLOAM_B200_ERR_INVALID_ARG;
+  int rc = rl_check_poses(poses, n);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  h->rl_loaded = false;
+  size_t op, od, os;
+  if ((rc = rl_reserve(h, n, &op, &od, &os)) != TLOAM_B200_OK) return rc;
+  if (n) CU_TRY(cudaMemcpyAsync(h->d_rl_places, h->d_loop_db, n * rl_slot(h->rl_cfg) * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
+  if (n && (rc = upload_host(h, h->d_rl_places + op, poses, n * 16 * sizeof(double))) != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  h->rl_n = n; h->rl_loaded = true;
+  return TLOAM_B200_OK;
+}
+
+// a run's state as a tloam_localize_result (loc_run's copy home)
+static void rl_result(const tloam_loc_state& s, size_t nq, size_t n_map, tloam_localize_result* out) {
+  memset(out, 0, sizeof(*out));
+  for (int r = 0; r < 3; ++r) {
+    for (int j = 0; j < 3; ++j) out->T[4 * j + r] = s.R[3 * r + j];
+    out->T[12 + r] = s.t[r];
+  }
+  out->T[15] = 1.0;
+  memcpy(out->T_map_odom, s.map_odom, sizeof(out->T_map_odom));
+  memcpy(out->guess, s.guess, sizeof(out->guess));
+  out->iterations = s.iter; out->termination = s.term; out->accepted = s.accepted;
+  out->inliers = (long long)s.inliers; out->rmse = s.rmse; out->fitness = s.fitness;
+  out->n_query_points = (long long)nq; out->n_map_points = (long long)n_map;
+}
+
+// the query's descriptor and down-sample, the search, the guesses and the batched ICP, with one read-back of the query's
+// size and one copy home
+static int rl_run(tloam_b200_handle* h, const double* d_in, size_t n, tloam_relocalize_result* out) {
+  if (!h->loc_loaded || !h->rl_loaded) return TLOAM_B200_ERR_NOT_READY;
+  tloam_rl_run_fn run;
+  int rc = rl_load(h, &run);
+  if (rc != TLOAM_B200_OK) return rc;
+  LoopLib lib;
+  if ((rc = loop_load(h, &lib)) != TLOAM_B200_OK) return rc;
+  const tloam_relocalize_config& rc_ = h->rl_cfg;
+  double* qdesc = reinterpret_cast<double*>(h->d_rl_small + 256);
+  tloam_sc_args sa;
+  memset(&sa, 0, sizeof(sa));
+  sa.n_ring = rc_.n_ring; sa.n_sector = rc_.n_sector; sa.lidar_height = rc_.lidar_height; sa.max_radius = rc_.max_radius;
+  sa.dirs = h->d_rl_dirs; sa.xyz = d_in; sa.n = n; sa.db = qdesc; sa.frame = 0;
+  sa.device = h->device; sa.stream = h->stream;
+  int e = 0;
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.bin(&sa)));
+  if (e == cudaSuccess) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.finish(&sa)));
+  if (e != cudaSuccess) {
+    snprintf(h->last_error, sizeof(h->last_error), "relocalization: k_sc_bin / k_sc_finish: %s", cudaGetErrorString((cudaError_t)e));
+    return TLOAM_B200_ERR_CUDA;
+  }
+  size_t nq = 0;
+  if ((rc = loc_query(h, d_in, n, &nq, reinterpret_cast<GMapState*>(h->d_rl_small), &h->d_rl_q, &h->cap_rl_q)) != TLOAM_B200_OK)
+    return rc;
+  const tloam_localize_config& c = h->loc_cfg;
+  const size_t nr = h->loc_n ? nq : 0;
+  const size_t K = (size_t)rc_.top_k, passes = (size_t)c.max_iterations + 1, qb = (nr + TLOAM_LOC_THREADS - 1) / TLOAM_LOC_THREADS;
+  const size_t home = K * sizeof(tloam_loc_state) + sizeof(tloam_rl_top);
+  size_t o = round_up(home, 256);
+  const size_t o_sums = o;  o += round_up(K * qb * TLOAM_LOC_SUMS * sizeof(double), 256);
+  const size_t o_idx = o;   o += round_up(K * passes * nr * sizeof(int), 256);
+  const size_t o_d2 = o;    o += K * passes * nr * sizeof(double);
+  if (o > h->cap_rl_run) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_rl_run); h->d_rl_run = nullptr; h->cap_rl_run = 0;
+    CU_TRY(cudaMalloc(&h->d_rl_run, o + o / 2));
+    h->cap_rl_run = o + o / 2;
+  }
+  unsigned char* base = h->d_rl_run;
+  std::vector<tloam_loc_state> st(K);
+  for (auto& s : st) {
+    memset(&s, 0, sizeof(s));
+    s.r = c.corr_dist_coarse;
+    s.term = nr ? TLOAM_LOOP_VERIFY_ITERATION_LIMIT : TLOAM_LOOP_VERIFY_EMPTY;
+    s.done = nr ? 0 : 1;
+  }
+  CU_TRY(cudaMemcpyAsync(base, st.data(), K * sizeof(tloam_loc_state), cudaMemcpyHostToDevice, h->stream));   // pageable: staged
+  size_t op, od, os;
+  if ((rc = rl_reserve(h, h->rl_n, &op, &od, &os)) != TLOAM_B200_OK) return rc;   // the places' offsets (no growth)
+  tloam_rl_args a;
+  memset(&a, 0, sizeof(a));
+  a.loc.grid = h->loc_index.grid;
+  a.loc.map = h->loc_index.map; a.loc.normal = h->loc_index.normal; a.loc.valid = h->loc_index.valid;
+  a.loc.query = h->d_rl_q; a.loc.nq = nr;
+  a.loc.odom = reinterpret_cast<const double*>(reinterpret_cast<const char*>(h->d_state) + offsetof(FrameState, result));
+  a.loc.memory = loc_memory(h);
+  a.loc.corr_dist_coarse = c.corr_dist_coarse; a.loc.corr_dist_fine = c.corr_dist_fine;
+  a.loc.eps_translation = c.eps_translation; a.loc.eps_rotation = c.eps_rotation; a.loc.max_fitness = c.max_fitness;
+  a.loc.max_iterations = c.max_iterations;
+  a.loc.device = h->device; a.loc.stream = h->stream;
+  a.qdesc = qdesc;
+  a.places = reinterpret_cast<const double*>(h->d_rl_places);
+  a.poses = reinterpret_cast<const double*>(h->d_rl_places + op);
+  a.n_places = h->rl_n;
+  a.n_ring = rc_.n_ring; a.n_sector = rc_.n_sector; a.dirs = h->d_rl_dirs;
+  a.place_distance = reinterpret_cast<double*>(h->d_rl_places + od);
+  a.place_shift = reinterpret_cast<long long*>(h->d_rl_places + os);
+  a.top_k = rc_.top_k; a.max_distance = rc_.max_distance; a.distinct_translation = rc_.distinct_translation;
+  a.cos_distinct_rotation = std::cos(rc_.distinct_rotation); a.ambiguity_ratio = rc_.ambiguity_ratio;
+  a.states = reinterpret_cast<tloam_loc_state*>(base);
+  a.top = reinterpret_cast<tloam_rl_top*>(base + K * sizeof(tloam_loc_state));
+  a.sums = reinterpret_cast<double*>(base + o_sums);
+  a.match_index = reinterpret_cast<int*>(base + o_idx);
+  a.match_d2 = reinterpret_cast<double*>(base + o_d2);
+  a.device = h->device; a.stream = h->stream;
+  int launches = 0;
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = run(&a, &launches)));
+  h->launches += launches > 0 ? launches - 1 : 0;
+  if (e != cudaSuccess) {
+    snprintf(h->last_error, sizeof(h->last_error), "relocalization: k_rl_*: %s", cudaGetErrorString((cudaError_t)e));
+    return TLOAM_B200_ERR_CUDA;
+  }
+  std::vector<unsigned char> back(home);
+  CU_TRY(cudaMemcpyAsync(back.data(), base, home, cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  h->rl_states.assign(reinterpret_cast<const tloam_loc_state*>(back.data()), reinterpret_cast<const tloam_loc_state*>(back.data()) + K);
+  memcpy(&h->rl_top, back.data() + K * sizeof(tloam_loc_state), sizeof(tloam_rl_top));
+  const tloam_rl_top& t = h->rl_top;
+  memset(out, 0, sizeof(*out));
+  out->n_hypotheses = t.n;
+  out->winner = t.winner;
+  if (t.n > 0 && t.winner >= 0) {
+    rl_result(h->rl_states[t.winner], nq, h->loc_n, &out->result);
+    out->place = t.place[t.winner]; out->shift = (int)t.shift[t.winner]; out->distance = t.distance[t.winner];
+  } else {
+    tloam_loc_state none;
+    memset(&none, 0, sizeof(none));
+    none.term = TLOAM_LOOP_VERIFY_EMPTY; none.fitness = INFINITY;
+    for (int k = 0; k < 3; ++k) none.R[4 * k] = 1.0;
+    for (int k = 0; k < 4; ++k) { none.guess[5 * k] = 1.0; none.odom[5 * k] = 1.0; none.map_odom[5 * k] = 1.0; }
+    rl_result(none, nq, h->loc_n, &out->result);
+    out->place = -1; out->shift = 0; out->distance = INFINITY; out->winner = -1;
+  }
+  out->ambiguous = t.ambiguous; out->accepted = t.accepted;
+  if (t.accepted) h->loc_have_prev = true;                      // k_rl_select wrote the prediction's memory
+  h->rl_ran = true; h->rl_nq = nr; h->rl_qn = nq; h->rl_last = a;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_relocalize_frame(tloam_b200_handle* h, tloam_relocalize_result* out) {
+  if (!h || !out) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->rl_on || h->raw_gen != h->seg_gen) return TLOAM_B200_ERR_NOT_READY;
+  CU_TRY(cudaSetDevice(h->device));
+  return rl_run(h, h->raw_scan, h->raw_n, out);
+}
+
+int tloam_b200_relocalize(tloam_b200_handle* h, const double* xyz, size_t n, tloam_relocalize_result* out) {
+  if (!h || !out || (!xyz && n) || n > ((size_t)1 << 30)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->rl_on) return TLOAM_B200_ERR_NOT_READY;
+  CU_TRY(cudaSetDevice(h->device));
+  int rc;
+  if ((rc = ensure_dev(h, &h->d_loc_in, &h->cap_loc_in, n, false)) != TLOAM_B200_OK) return rc;
+  if (n && (rc = upload_host(h, h->d_loc_in, xyz, n * 24)) != TLOAM_B200_OK) return rc;
+  return rl_run(h, h->d_loc_in, n, out);
+}
+
+int tloam_b200_relocalize_hypotheses(tloam_b200_handle* h, tloam_relocalize_hypothesis* out, size_t capacity, size_t* n) {
+  if (!h || !n) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->rl_on || !h->rl_ran) return TLOAM_B200_ERR_NOT_READY;
+  *n = (size_t)h->rl_top.n;
+  if (capacity < *n || (!out && *n)) return TLOAM_B200_ERR_INVALID_ARG;
+  for (size_t k = 0; k < *n; ++k) {
+    out[k].place = h->rl_top.place[k]; out[k].shift = (int)h->rl_top.shift[k]; out[k].distance = h->rl_top.distance[k];
+    rl_result(h->rl_states[k], h->rl_qn, h->loc_n, &out[k].result);
+  }
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_relocalize_matches(tloam_b200_handle* h, int hypothesis, int pass, int* index, double* d2, size_t capacity, size_t* n) {
+  if (!h || !n) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->rl_on || !h->rl_ran) return TLOAM_B200_ERR_NOT_READY;
+  *n = h->rl_nq;
+  if (hypothesis < 0 || hypothesis >= h->rl_top.n || capacity < h->rl_nq) return TLOAM_B200_ERR_INVALID_ARG;
+  const int passes = h->rl_nq ? h->rl_states[hypothesis].iter + 1 : 0;
+  if (pass < 0 || pass >= passes) return TLOAM_B200_ERR_INVALID_ARG;
+  const size_t nq = h->rl_nq, stride = (size_t)(h->rl_last.loc.max_iterations + 1) * nq;
+  const tloam_rl_args& a = h->rl_last;
+  const size_t off = (size_t)hypothesis * stride + (size_t)pass * nq;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (index) CU_TRY(cudaMemcpyAsync(index, a.match_index + off, nq * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  if (d2) CU_TRY(cudaMemcpyAsync(d2, a.match_d2 + off, nq * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   CU_TRY(cudaStreamSynchronize(h->stream));
   return TLOAM_B200_OK;
 }

@@ -157,6 +157,21 @@ class LocalizeResult:
 
 
 @dataclasses.dataclass(frozen=True)
+class RelocalizeResult:
+    """tloam_relocalize_result: result = the winner's LocalizeResult; place / shift / distance its candidate (place -1
+    without hypotheses); winner = its rank; accepted = the winner is accepted and no distinct hypothesis fits about as
+    well (ambiguous)."""
+    result: LocalizeResult
+    place: int
+    shift: int
+    distance: float
+    n_hypotheses: int
+    winner: int
+    ambiguous: bool
+    accepted: bool
+
+
+@dataclasses.dataclass(frozen=True)
 class PoseGraphResult:
     """tloam_pose_graph_result: termination is one of PoseGraphResult.CONVERGED .. NO_LOOPS; the costs are sum r^T Omega r
     at the odometry poses and at the returned poses; step_* are the last step's largest |upsilon| / |omega| component."""
@@ -1226,6 +1241,87 @@ class LocalRegistration:
         self._check(self._L.tloam_b200_localize_cells(self._h, rows.ctypes.data_as(up), keys.ctypes.data_as(C.POINTER(C.c_ulonglong)),
                                                       starts.ctypes.data_as(up), n_rows, C.byref(nc)), "localize_cells")
         return rows, keys[:nc.value], starts[:nc.value + 1]
+
+    # ---- relocalization in a prior map (include/tloam_b200.h "Relocalization in a prior map") ----
+    def relocalize_enable(self, **overrides):
+        """turn relocalization on (localization must be on) and drop the places; overrides: fields of
+        tloam_relocalize_config (lidar_height, n_ring, n_sector, max_radius, top_k, max_distance, distinct_translation,
+        distinct_rotation, ambiguity_ratio)"""
+        cfg = _lib.RelocalizeConfig()
+        self._L.tloam_b200_relocalize_default_config(C.byref(cfg))
+        for k, v in overrides.items():
+            if not hasattr(cfg, k):
+                raise KeyError(k)
+            setattr(cfg, k, v)
+        self._check(self._L.tloam_b200_relocalize_enable(self._h, C.byref(cfg)), "relocalize_enable")
+        self._reloc_slot = cfg.n_ring * cfg.n_sector + cfg.n_ring + cfg.n_sector
+
+    def relocalize_set_places(self, descriptors, poses):
+        """load the places: descriptor slots (n x slot, as loop_descriptors returns them) and poses (n x 4 x 4, map <- sensor)"""
+        P = np.asarray(poses, dtype=np.float64).reshape(-1, 4, 4)
+        p = np.ascontiguousarray(P.transpose(0, 2, 1))                            # column-major per pose
+        n = len(P)
+        d = np.ascontiguousarray(np.asarray(descriptors, dtype=np.float64))
+        slot = getattr(self, "_reloc_slot", None)
+        if slot is None:
+            raise RuntimeError("relocalize_set_places: relocalize_enable first")
+        if d.shape != (n, slot):
+            raise ValueError(f"relocalize_set_places: descriptors of shape {d.shape}, want ({n}, {slot}) for {n} poses")
+        self._check(self._L.tloam_b200_relocalize_set_places(self._h, _dp(d) if n else None, _dp(p) if n else None, n),
+                    "relocalize_set_places")
+
+    def relocalize_set_places_loop(self, poses):
+        """load the places from the handle's own loop database, with one pose per loop frame (n x 4 x 4)"""
+        P = np.asarray(poses, dtype=np.float64).reshape(-1, 4, 4)
+        p = np.ascontiguousarray(P.transpose(0, 2, 1))
+        self._check(self._L.tloam_b200_relocalize_set_places_loop(self._h, _dp(p) if len(P) else None, len(P)),
+                    "relocalize_set_places_loop")
+
+    def _relocalize_out(self, r):
+        return RelocalizeResult(self._localize_out(r.result), r.place, r.shift, r.distance, r.n_hypotheses, r.winner,
+                                bool(r.ambiguous), bool(r.accepted))
+
+    def relocalize_frame(self):
+        """relocalize the scan the last process_raw_scan left on the device; returns a RelocalizeResult"""
+        r = _lib.RelocalizeResult()
+        self._check(self._L.tloam_b200_relocalize_frame(self._h, C.byref(r)), "relocalize_frame")
+        return self._relocalize_out(r)
+
+    def relocalize(self, xyz):
+        """relocalize a host cloud (n x 3); as relocalize_frame"""
+        p = np.ascontiguousarray(np.asarray(xyz, dtype=np.float64).reshape(-1, 3))
+        r = _lib.RelocalizeResult()
+        self._check(self._L.tloam_b200_relocalize(self._h, _dp(p) if len(p) else None, len(p), C.byref(r)), "relocalize")
+        return self._relocalize_out(r)
+
+    def relocalize_hypotheses(self):
+        """the last relocalization's hypotheses in rank order: [(place, shift, distance, LocalizeResult)]"""
+        n = C.c_size_t(0)
+        buf = (_lib.RelocalizeHypothesis * 64)()
+        self._check(self._L.tloam_b200_relocalize_hypotheses(self._h, buf, 64, C.byref(n)), "relocalize_hypotheses")
+        return [(buf[k].place, buf[k].shift, buf[k].distance, self._localize_out(buf[k].result)) for k in range(n.value)]
+
+    def relocalize_matches(self, hypothesis, k):
+        """hypothesis's matches at pass k, as localize_matches"""
+        n = C.c_size_t(0)
+        rc = self._L.tloam_b200_relocalize_matches(self._h, int(hypothesis), int(k), None, None, 0, C.byref(n))
+        if rc != _lib.ERR_INVALID_ARG or n.value == 0:
+            self._check(rc, "relocalize_matches")
+        idx, d2 = np.zeros(n.value, dtype=np.int32), np.zeros(n.value)
+        self._check(self._L.tloam_b200_relocalize_matches(self._h, int(hypothesis), int(k), idx.ctypes.data_as(C.POINTER(C.c_int)),
+                                                          _dp(d2), n.value, C.byref(n)), "relocalize_matches")
+        return idx, d2
+
+    def loop_descriptors(self, first=0, count=None):
+        """the descriptor slots of loop frames [first, first + count) in one copy (count None: to the last), count x slot:
+        what relocalize_set_places takes"""
+        R, S = self._loop_shape
+        if count is None:
+            count = self.loop_size() - first
+        out = np.zeros((count, R * S + R + S))
+        self._check(self._L.tloam_b200_loop_descriptors_download(self._h, int(first), int(count), _dp(out) if count else None),
+                    "loop_descriptors_download")
+        return out
 
     # ---- shared map (multi-GPU) ----
     def map_blob_size(self):
