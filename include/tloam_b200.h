@@ -1291,6 +1291,101 @@ int tloam_b200_relocalize_hypotheses(tloam_b200_handle* h, tloam_relocalize_hypo
 int tloam_b200_relocalize_matches(tloam_b200_handle* h, int hypothesis, int pass, int* index, double* d2, size_t capacity,
                                   size_t* n);
 
+/* ---- Updating a prior map (opt-in, on top of localization): the prior map of "Localization in a prior map" is kept as it
+ * was loaded, and each localized frame votes on it and proposes what is new; one build gives the updated map, which
+ * tloam_b200_localize_set_map_updated loads in its place.  A car parked when the map was made and gone now is seen
+ * through; a wall or a street that is new finds no prior row near it.
+ *   - State.  Two counters (through, hits) per prior row; the additions: rows in the map's frame, each with its frame
+ *     number and its own (through, hits).  tloam_b200_map_update_enable and every map load (tloam_b200_localize_set_map,
+ *     _set_map_merged, _set_map_updated) empty it; tloam_b200_localize_enable turns updating off.  While it is off nothing
+ *     is allocated or launched.
+ *   - Add.  tloam_b200_map_update_add uses the last tloam_b200_localize_frame or tloam_b200_localize (relocalization runs
+ *     do not count).  NOT_READY when there was none since the load or the enable, when the add was already made for it, or
+ *     when the scan it read has been replaced since: for _frame the raw scan under tloam_b200_global_map_append_frame's
+ *     rule, for a host cloud the next tloam_b200_localize or tloam_b200_relocalize with a host cloud.  A localization that
+ *     was not accepted gives OK with used = 0 and changes nothing, so a caller may add after every frame.
+ *   - Votes of an add.  The scan rows the localization's query came from (the raw scan or the host cloud, sensor frame)
+ *     at T = the result's T vote, by the rule of "Dynamic-point removal" with this configuration's image (range image,
+ *     window image, through and hits), first on every prior row, then on every addition of the earlier adds.  The rows this
+ *     add appends start at (0, 0).
+ *   - Novelty of an add.  For each query row q in query order, p = T q by the localization's final pass:
+ *     p_r = ((R(r, 0) q0 + R(r, 1) q1) + R(r, 2) q2) + t_r, each product and sum rounded on its own.  p is new iff no prior
+ *     row (removed or not) has d2(p, m) <= novel_radius * novel_radius (d2 as in "Loop verification", the square rounded);
+ *     the cells visited are those of the localization's grid search, so the answer is the exhaustive scan's.  The new p
+ *     are appended to the additions in query order with frame number f = the number of used adds before this one since
+ *     the state was emptied.
+ *   - Removed.  A row (prior or addition) is removed iff through >= image.min_through and through > hits.
+ *   - Build.  One cloud: the prior rows that are not removed, in row order (tloam_gmd_static: the rows
+ *     tloam_b200_global_map_static_download's rule keeps, bit for bit), then the supported voxels.  The voxels are
+ *     VoxelDownSample(voxel) of the additions that are not removed, by the rules of "Merged global map": bounds, index,
+ *     VOXEL_RANGE at 2^21 voxels, sums in row order from +0.0 then / count, ascending key order.  A voxel is supported
+ *     iff its rows come from at least min_frames distinct adds: the frame numbers never decrease along the additions, so
+ *     within a voxel (rows in row order) the distinct count is 1 + the number of increases.  A session with no removal and
+ *     no supported voxel builds the prior map bit for bit.  The cloud stays on the device until the next build, enable, or
+ *     tloam_b200_localize_enable; a refused build leaves none.
+ *   - Rounding.  Every product, sum, quotient and square root is rounded on its own, left to right as written, so
+ *     tests/map_update_oracle.py reproduces every counter, addition and row bit for bit.
+ *   - Nothing else moves.  The localization results and its prediction memory, the odometry, the pose history, the
+ *     submap, the global map and its tables, the loop database and the pose graph keep their bits, and every other call
+ *     its launch counts.
+ *   - Device.  An add is k_mu_pose, tloam_gmd_vote twice (k_gmd_clear, k_gmd_bin, k_gmd_window, k_gmd_vote: the prior rows
+ *     with a device word holding their count, then the additions with the device-side count), then k_mu_novel, k_mu_count
+ *     and k_mu_scatter.  The host bounds the additions' count by the count at its last read-back plus the query rows of
+ *     every add since; an add synchronises once, to read the count back, only when that bound passes the buffer's
+ *     capacity, and when fewer rows than 16 adds of its size are left then, the buffer grows in the same add without a
+ *     further synchronisation (the rows copied on the stream, the old buffer freed at a later synchronisation), so a
+ *     read-back comes at most once per 16 adds of one size.  Every other add, the first after an enable or a load among
+ *     them, enqueues its work and returns.  The prior rows' counters are allocated by the enable and by the loads.  A build is k_gmd_count / k_gmd_scatter over the prior rows, k_mu_bounds,
+ *     k_mu_keys, the shared radix sort (k_gmm_hist / k_gmm_offsets / k_gmm_scatter per 8-bit digit, k_gmm_head_count /
+ *     k_gmm_head_scatter), k_mu_average, k_mu_count and k_mu_scatter, with four synchronisations.
+ *   - Memory.  8 B per prior row (the counters); 36 B per addition row (xyz, frame, counters); per build 24 B per row of
+ *     the cloud plus 49 B per addition row of sort scratch and voxels; 25 B per query row; two range images of the
+ *     configuration's size.  The kernels live in libtloam_b200_mapu.so and libtloam_b200_gmd.so, loaded from this
+ *     library's directory by the enable call (ERR_CUDA if one is missing). */
+typedef struct tloam_map_update_config {
+  tloam_global_map_dynamic_config image;   /* the votes' range image and removal rule, as "Dynamic-point removal" */
+  double novel_radius;                 /* m, > 0, <= 3 localization cells */
+  double voxel;                        /* the additions' voxel, m, > 0 */
+  int min_frames;                      /* distinct adds a voxel needs, >= 1 */
+} tloam_map_update_config;
+typedef struct tloam_map_update_add_result {
+  int used;                            /* 0: the localization was not accepted, nothing changed */
+  long long frame;                     /* this add's frame number, -1 when not used */
+  long long n_scan_points;             /* the scan rows that voted */
+  long long n_query_points;            /* the query rows tested for novelty */
+} tloam_map_update_add_result;
+typedef struct tloam_map_update_result {
+  long long n_prior, n_prior_removed;          /* prior rows, and those removed */
+  long long n_additions, n_additions_removed;  /* addition rows, and those removed */
+  long long n_voxels, n_voxels_kept;           /* the additions' voxels before and after the min_frames test */
+  long long n_total;                           /* the cloud's rows: n_prior - n_prior_removed + n_voxels_kept */
+} tloam_map_update_result;
+/* image: the dynamic removal's defaults; novel_radius 0.5 m, voxel 0.5 m, min_frames 3 (DESIGN.md section 4c has how they
+ * were checked) */
+void tloam_b200_map_update_default_config(tloam_map_update_config* c);
+/* turns updating on (or re-configures it) and empties its state.  INVALID_ARG: cfg null, an image that
+ * tloam_b200_global_map_dynamic_enable refuses, novel_radius or voxel not finite or not > 0, min_frames < 1, or (with
+ * localization on) novel_radius > 3 cell.  NOT_READY: localization off. */
+int tloam_b200_map_update_enable(tloam_b200_handle* h, const tloam_map_update_config* cfg);
+/* votes and appends for the last localization (see Add above).  NOT_READY: updating off, no map, or the rules above. */
+int tloam_b200_map_update_add(tloam_b200_handle* h, tloam_map_update_add_result* out);
+/* builds the updated cloud; synchronises.  NOT_READY: updating off or no map.  VOXEL_RANGE: the kept additions' extent
+ * reaches 2^21 voxels on an axis (no cloud). */
+int tloam_b200_map_update_build(tloam_b200_handle* h, tloam_map_update_result* out);
+/* the prior rows, the additions and the built cloud's rows (0 without a cloud); any output may be null; synchronises.
+ * NOT_READY: updating off or no map. */
+int tloam_b200_map_update_size(tloam_b200_handle* h, size_t* n_prior, size_t* n_additions, size_t* n_built);
+/* rows [first, first + count) of the built cloud (count x 3).  NOT_READY: no cloud.  INVALID_ARG past the end. */
+int tloam_b200_map_update_download(tloam_b200_handle* h, size_t first, size_t count, double* xyz);
+/* the counters of rows [first, first + count) of the prior map (which 0) or of the additions (which 1); either output may
+ * be null; synchronises.  NOT_READY: updating off or no map.  INVALID_ARG: which not 0 or 1, or past the end. */
+int tloam_b200_map_update_votes(tloam_b200_handle* h, int which, size_t first, size_t count, unsigned* through, unsigned* hits);
+/* additions [first, first + count): xyz (count x 3) and frame numbers (either may be null); as _votes */
+int tloam_b200_map_update_additions(tloam_b200_handle* h, size_t first, size_t count, double* xyz, unsigned* frame);
+/* tloam_b200_localize_set_map of the built cloud, copied on the device.  NOT_READY: localization or updating off, or no
+ * built cloud.  Like every load it empties the update's state. */
+int tloam_b200_localize_set_map_updated(tloam_b200_handle* h);
+
 /* Pinned host memory helpers (optional; pinned inputs make set_* a direct DMA, no staging threads). */
 int tloam_b200_host_alloc(void** p, size_t bytes);
 int tloam_b200_host_free(void* p);

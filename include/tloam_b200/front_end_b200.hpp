@@ -19,7 +19,8 @@
 // check a candidate by a scan-to-scan ICP of down-sampled keyframes kept on the GPU and give the relative pose;
 // enableSubmapVerification / verifyLoopSubmap check it against the keyframes around the candidate, point to plane.
 // enableLocalization / localizeFrame register each frame against a prior map; enableRelocalization / setPlaces /
-// relocalizeFrame find the first pose in that map (or the pose after tracking is lost) from a recorded session's places.
+// relocalizeFrame find the first pose in that map (or the pose after tracking is lost) from a recorded session's places;
+// enableMapUpdate / addMapUpdateFrame / buildUpdatedMap keep that map up to date from the localized frames.
 // Without the reference headers (this repository's tests) define TLOAM_B200_MOCK_HOST_TYPES and provide the host types
 // (tests/mock/mock_tloam.hpp).
 #ifndef TLOAM_B200_FRONT_END_B200_HPP
@@ -384,6 +385,32 @@ class FrontEndB200 {
   bool relocalize(const CloudData& scan, tloam_relocalize_result& out) {
     return report(tloam_b200_relocalize(h_, data(scan), size(scan), &out), "relocalize");
   }
+
+  // Updating a prior map (include/tloam_b200.h "Updating a prior map"): after each localizeFrame / localize,
+  // addMapUpdateFrame lets that frame's scan vote on the prior map's points and keeps its points no prior point is near
+  // (out.used = 0 when the localization was not accepted, and nothing changes); buildUpdatedMap gives the prior points not
+  // seen through, then the new voxels enough frames agree on; updatedMap reads it back and setPriorMapUpdated loads it in
+  // place of the prior map.  Needs enableLocalization and a prior map; enableLocalization turns it off.
+  bool enableMapUpdate(const tloam_map_update_config& cfg) { return report(tloam_b200_map_update_enable(h_, &cfg), "enableMapUpdate"); }
+  bool enableMapUpdate() {
+    tloam_map_update_config c;
+    tloam_b200_map_update_default_config(&c);
+    return enableMapUpdate(c);
+  }
+  bool addMapUpdateFrame(tloam_map_update_add_result& out) { return report(tloam_b200_map_update_add(h_, &out), "addMapUpdateFrame"); }
+  bool addMapUpdateFrame() {
+    tloam_map_update_add_result r;
+    return addMapUpdateFrame(r);
+  }
+  bool buildUpdatedMap(tloam_map_update_result& out) { return report(tloam_b200_map_update_build(h_, &out), "buildUpdatedMap"); }
+  // the last buildUpdatedMap's points
+  bool updatedMap(std::vector<Eigen::Vector3d>& out) {
+    size_t n = 0;
+    if (!report(tloam_b200_map_update_size(h_, nullptr, nullptr, &n), "updatedMap")) return false;
+    out.resize(n);
+    return report(tloam_b200_map_update_download(h_, 0, n, n ? reinterpret_cast<double*>(out.data()) : nullptr), "updatedMap");
+  }
+  bool setPriorMapUpdated() { return report(tloam_b200_localize_set_map_updated(h_), "setPriorMapUpdated"); }
 
   // processCloud + setInputSource (ref: front_end.cpp:181-199, :313): the three clouds the segmentation nodelet publishes
   bool processCloud(CloudData& ground, CloudData& edge, CloudData& general) {

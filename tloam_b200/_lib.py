@@ -130,6 +130,23 @@ class RelocalizeResult(C.Structure):
                 ("n_hypotheses", C.c_int), ("winner", C.c_int), ("ambiguous", C.c_int), ("accepted", C.c_int)]
 
 
+class MapUpdateConfig(C.Structure):
+    """tloam_map_update_config (include/tloam_b200.h "Updating a prior map"): the votes' image and the additions' rules."""
+    _fields_ = [("image", GlobalMapDynamicConfig), ("novel_radius", C.c_double), ("voxel", C.c_double), ("min_frames", C.c_int)]
+
+
+class MapUpdateAddResult(C.Structure):
+    """tloam_map_update_add_result: whether the add was used, its frame number and the rows it read."""
+    _fields_ = [("used", C.c_int), ("frame", C.c_longlong), ("n_scan_points", C.c_longlong), ("n_query_points", C.c_longlong)]
+
+
+class MapUpdateResult(C.Structure):
+    """tloam_map_update_result: the counts of a build."""
+    _fields_ = [("n_prior", C.c_longlong), ("n_prior_removed", C.c_longlong), ("n_additions", C.c_longlong),
+                ("n_additions_removed", C.c_longlong), ("n_voxels", C.c_longlong), ("n_voxels_kept", C.c_longlong),
+                ("n_total", C.c_longlong)]
+
+
 class PoseGraphConfig(C.Structure):
     """tloam_pose_graph_config (include/tloam_b200.h "Pose graph"): the edges' sigmas and the Gauss-Newton schedule."""
     _fields_ = [("sigma_odom_translation", C.c_double), ("sigma_odom_rotation", C.c_double),
@@ -273,6 +290,9 @@ EXPORTS = [
     "tloam_b200_loop_descriptors_download", "tloam_b200_relocalize_default_config", "tloam_b200_relocalize_enable",
     "tloam_b200_relocalize_set_places", "tloam_b200_relocalize_set_places_loop", "tloam_b200_relocalize_frame",
     "tloam_b200_relocalize", "tloam_b200_relocalize_hypotheses", "tloam_b200_relocalize_matches",
+    "tloam_b200_map_update_default_config", "tloam_b200_map_update_enable", "tloam_b200_map_update_add",
+    "tloam_b200_map_update_build", "tloam_b200_map_update_size", "tloam_b200_map_update_download",
+    "tloam_b200_map_update_votes", "tloam_b200_map_update_additions", "tloam_b200_localize_set_map_updated",
 ]
 
 _lib = None
@@ -496,5 +516,15 @@ def load():
     L.tloam_b200_relocalize.argtypes = [vp, dp, C.c_size_t, C.POINTER(RelocalizeResult)]
     L.tloam_b200_relocalize_hypotheses.argtypes = [vp, C.POINTER(RelocalizeHypothesis), C.c_size_t, szp]
     L.tloam_b200_relocalize_matches.argtypes = [vp, C.c_int, C.c_int, C.POINTER(C.c_int), dp, C.c_size_t, szp]
+    L.tloam_b200_map_update_default_config.argtypes = [C.POINTER(MapUpdateConfig)]
+    L.tloam_b200_map_update_default_config.restype = None
+    L.tloam_b200_map_update_enable.argtypes = [vp, C.POINTER(MapUpdateConfig)]
+    L.tloam_b200_map_update_add.argtypes = [vp, C.POINTER(MapUpdateAddResult)]
+    L.tloam_b200_map_update_build.argtypes = [vp, C.POINTER(MapUpdateResult)]
+    L.tloam_b200_map_update_size.argtypes = [vp, szp, szp, szp]
+    L.tloam_b200_map_update_download.argtypes = [vp, C.c_size_t, C.c_size_t, dp]
+    L.tloam_b200_map_update_votes.argtypes = [vp, C.c_int, C.c_size_t, C.c_size_t, up, up]
+    L.tloam_b200_map_update_additions.argtypes = [vp, C.c_size_t, C.c_size_t, dp, up]
+    L.tloam_b200_localize_set_map_updated.argtypes = [vp]
     _lib = L
     return L

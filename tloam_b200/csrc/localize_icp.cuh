@@ -71,7 +71,8 @@ __device__ __forceinline__ void loc_column(const tloam_loc_grid& g, unsigned n_c
 
 // one thread per query row (blockIdx.x: the query block): p = R q + t and its nearest map row within the pass's radius
 // (s->r, corr_dist_coarse for the final pass) by (d2, row index), recorded at slot `pass` (the final pass: s->iter) of
-// match_index / match_d2
+// match_index / match_d2.  k_mu_novel (map_update.cu) walks the same cells and columns for an existence test: a change to
+// the cell rule here changes it there too.
 template <class Run>
 __device__ __forceinline__ void loc_match_run(const tloam_loc_args& a, const Run& run, int pass, int final_pass) {
   const tloam_loc_state* s = run.state();

@@ -39,6 +39,7 @@
 #include "map_merge.h"
 #include "localize.h"
 #include "relocalize.h"
+#include "map_update.h"
 
 
 
@@ -295,6 +296,26 @@ struct tloam_b200_handle {
   unsigned char* d_loc_run = nullptr;      size_t cap_loc_run = 0;     // state, memory, partials, matches
   bool loc_have_prev = false;              // a localization since the load: the prediction has its memory
   bool loc_ran = false;                    int loc_passes = 0;  size_t loc_nq = 0;   tloam_loc_args loc_last;
+  // what the last tloam_b200_localize* read, for tloam_b200_map_update_add: its serial number, the scan rows (the raw scan
+  // or d_loc_in) with the generation they must still have, and the verdict
+  unsigned long long loc_serial = 0;       const double* loc_src = nullptr;  size_t loc_src_n = 0;
+  bool loc_src_raw = false;                unsigned long long loc_src_gen = 0, loc_in_gen = 0;  bool loc_accepted = false;
+  // ---- updating a prior map (tloam_b200_map_update*, libtloam_b200_mapu.so and libtloam_b200_gmd.so): the prior rows'
+  //      counters, the additions (xyz, frame, counters in one buffer), the range image and the built cloud; nothing is
+  //      allocated or launched until it is enabled ----
+  bool mu_on = false;                      tloam_map_update_config mu_cfg;
+  bool mu_fresh = true;                    // the state is empty: the next add or build clears the counters
+  unsigned long long mu_min_serial = 0, mu_added_serial = 0;  unsigned mu_frames = 0;
+  size_t mu_known = 0, mu_pending = 0;     // the additions' count at the last read-back, and the query rows added since
+  double* d_mu_tables = nullptr;           size_t cap_mu_tables = 0;
+  unsigned long long* d_mu_image = nullptr; double* d_mu_window = nullptr;  size_t cap_mu_image = 0;
+  unsigned* d_mu_prior = nullptr;          size_t cap_mu_prior = 0;   // through [0, cap), hits [cap, 2 cap)
+  unsigned char* d_mu_add = nullptr;       size_t cap_mu_add = 0;     // xyz, frame, through, hits of cap rows each
+  unsigned char* d_mu_small = nullptr;     // the pose at 0, counts at 128, the static part's block counts at 1024
+  unsigned char* d_mu_q = nullptr;         size_t cap_mu_q = 0;       // per query row: the flag and T q
+  std::vector<void*> mu_retired;           // buffers an add replaced, freed at the next point that synchronises anyway
+  unsigned char* d_mu_build = nullptr;     size_t cap_mu_build = 0;
+  double* d_mu_out = nullptr;              size_t cap_mu_out = 0;     bool mu_built = false;  size_t mu_built_n = 0;
   // ---- relocalization in a prior map (tloam_b200_relocalize*, libtloam_b200_reloc.so): the places (descriptor slots,
   //      poses, per-place best distance and shift in one buffer), the query's descriptor and down-sample, the batch ----
   bool rl_on = false;                      tloam_relocalize_config rl_cfg;
@@ -525,6 +546,9 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   cudaFree(h->d_loc_map); cudaFree(h->d_loc_scratch); cudaFree(h->d_loc_qst); cudaFree(h->d_loc_reg); cudaFree(h->d_loc_fin);
   cudaFree(h->d_loc_q); cudaFree(h->d_loc_in); cudaFree(h->d_loc_run);
   cudaFree(h->d_rl_dirs); cudaFree(h->d_rl_places); cudaFree(h->d_rl_small); cudaFree(h->d_rl_q); cudaFree(h->d_rl_run);
+  cudaFree(h->d_mu_tables); cudaFree(h->d_mu_image); cudaFree(h->d_mu_window); cudaFree(h->d_mu_prior); cudaFree(h->d_mu_add);
+  cudaFree(h->d_mu_small); cudaFree(h->d_mu_q); cudaFree(h->d_mu_build); cudaFree(h->d_mu_out);
+  for (void* p : h->mu_retired) cudaFree(p);
   for (int i = 0; i < 2; ++i) if (h->ev_stage_free[i]) cudaEventDestroy(h->ev_stage_free[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_fit[i]) cudaEventDestroy(h->ev_fit[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_res[i]) cudaEventDestroy(h->ev_res[i]);
@@ -5013,6 +5037,24 @@ static bool gmd_config_valid(const tloam_global_map_dynamic_config* c) {
   return c->min_through >= 1;
 }
 
+// the host tables: b_k = sin(lo + k (hi - lo) / n_rows) and Scan Context's sector boundaries (cos, sin of 2 pi k / n_cols);
+// false when the row table is not non-decreasing (the row search needs it so)
+static bool gmd_tables(const tloam_global_map_dynamic_config* cfg, std::vector<double>* out) {
+  std::vector<double>& tab = *out;
+  tab.assign((size_t)(cfg->n_rows + 1) + 2 * (size_t)(cfg->n_cols - 1), 0.0);
+  const double lo = cfg->fov_down * (M_PI / 180.0), hi = cfg->fov_up * (M_PI / 180.0);
+  for (int k = 0; k <= cfg->n_rows; ++k) tab[k] = std::sin(lo + k * (hi - lo) / cfg->n_rows);
+  for (int k = 1; k <= cfg->n_rows; ++k)
+    if (!(tab[k] >= tab[k - 1])) return false;
+  double* dirs = tab.data() + (cfg->n_rows + 1);
+  for (int k = 1; k < cfg->n_cols; ++k) {
+    const double t = 2.0 * M_PI * k / cfg->n_cols;
+    dirs[2 * (k - 1)] = std::cos(t);
+    dirs[2 * (k - 1) + 1] = std::sin(t);
+  }
+  return true;
+}
+
 int tloam_b200_global_map_dynamic_enable(tloam_b200_handle* h, const tloam_global_map_dynamic_config* cfg) {
   if (!h || !cfg) return TLOAM_B200_ERR_INVALID_ARG;
   if (!gmd_config_valid(cfg)) return TLOAM_B200_ERR_INVALID_ARG;
@@ -5022,18 +5064,8 @@ int tloam_b200_global_map_dynamic_enable(tloam_b200_handle* h, const tloam_globa
   if (rc != TLOAM_B200_OK) return rc;
   CU_TRY(cudaSetDevice(h->device));
   CU_TRY(cudaStreamSynchronize(h->stream));
-  // the host tables: b_k = sin(lo + k (hi - lo) / n_rows) and Scan Context's sector boundaries (cos, sin of 2 pi k / n_cols)
-  std::vector<double> tab((size_t)(cfg->n_rows + 1) + 2 * (size_t)(cfg->n_cols - 1));
-  const double lo = cfg->fov_down * (M_PI / 180.0), hi = cfg->fov_up * (M_PI / 180.0);
-  for (int k = 0; k <= cfg->n_rows; ++k) tab[k] = std::sin(lo + k * (hi - lo) / cfg->n_rows);
-  for (int k = 1; k <= cfg->n_rows; ++k)
-    if (!(tab[k] >= tab[k - 1])) return TLOAM_B200_ERR_INVALID_ARG;     // the row search needs a non-decreasing table
-  double* dirs = tab.data() + (cfg->n_rows + 1);
-  for (int k = 1; k < cfg->n_cols; ++k) {
-    const double t = 2.0 * M_PI * k / cfg->n_cols;
-    dirs[2 * (k - 1)] = std::cos(t);
-    dirs[2 * (k - 1) + 1] = std::sin(t);
-  }
+  std::vector<double> tab;
+  if (!gmd_tables(cfg, &tab)) return TLOAM_B200_ERR_INVALID_ARG;
   if (tab.size() > h->cap_gmd_bounds) {
     cudaFree(h->d_gmd_bounds); h->d_gmd_bounds = nullptr; h->cap_gmd_bounds = 0;
     CU_TRY(cudaMalloc(&h->d_gmd_bounds, tab.size() * sizeof(double)));
@@ -5547,6 +5579,7 @@ int tloam_b200_localize_enable(tloam_b200_handle* h, const tloam_localize_config
   }
   h->loc_cfg = *c;
   h->loc_on = true;
+  h->mu_on = false;                                             // updating a prior map is off until enabled again
   h->loc_loaded = false; h->loc_n = 0; h->loc_have_prev = false;
   h->loc_ran = false; h->loc_passes = 0; h->loc_nq = 0;
   return TLOAM_B200_OK;
@@ -5629,16 +5662,19 @@ static int loc_reserve_map(tloam_b200_handle* h, size_t n) {
   return TLOAM_B200_OK;
 }
 
+static int mu_after_load(tloam_b200_handle* h, int rc);   // updating a prior map: its counters sized to the new map
+
 int tloam_b200_localize_set_map(tloam_b200_handle* h, const double* xyz, size_t n) {
   if (!h || (!xyz && n)) return TLOAM_B200_ERR_INVALID_ARG;
   if (!h->loc_on) return TLOAM_B200_ERR_NOT_READY;
   if (n >> 32) return TLOAM_B200_ERR_INVALID_ARG;             // the sort's row payload is a u32
   CU_TRY(cudaSetDevice(h->device));
   h->loc_loaded = false; h->loc_have_prev = false; h->loc_ran = false; h->loc_passes = 0;
+  h->mu_fresh = true; h->mu_frames = 0;                         // an update belongs to the map it was made on
   int rc;
   if ((rc = loc_reserve_map(h, n)) != TLOAM_B200_OK) return rc;
   if (n && (rc = upload_host(h, h->d_loc_map, xyz, n * 24)) != TLOAM_B200_OK) return rc;
-  return loc_build(h, n);
+  return mu_after_load(h, loc_build(h, n));
 }
 
 int tloam_b200_localize_set_map_merged(tloam_b200_handle* h) {
@@ -5647,10 +5683,11 @@ int tloam_b200_localize_set_map_merged(tloam_b200_handle* h) {
   CU_TRY(cudaSetDevice(h->device));
   const size_t n = h->gmm_n;
   h->loc_loaded = false; h->loc_have_prev = false; h->loc_ran = false; h->loc_passes = 0;
+  h->mu_fresh = true; h->mu_frames = 0;                         // an update belongs to the map it was made on
   int rc;
   if ((rc = loc_reserve_map(h, n)) != TLOAM_B200_OK) return rc;
   if (n) CU_TRY(cudaMemcpyAsync(h->d_loc_map, h->d_gmm_out, n * 24, cudaMemcpyDeviceToDevice, h->stream));
-  return loc_build(h, n);
+  return mu_after_load(h, loc_build(h, n));
 }
 
 // the query: VoxelDownSample(voxel) of the finite rows of the n rows at d_in by the global map's ordered path at pose I
@@ -5686,6 +5723,7 @@ static int loc_run(tloam_b200_handle* h, const double* d_in, size_t n, const dou
   LocLib lib;
   int rc = loc_load(h, &lib);
   if (rc != TLOAM_B200_OK) return rc;
+  h->loc_src = nullptr;                                         // the last query is rewritten: no add until this run ends
   size_t nq = 0;
   if ((rc = loc_query(h, d_in, n, &nq, loc_qst(h), &h->d_loc_q, &h->cap_loc_q)) != TLOAM_B200_OK) return rc;
   const tloam_localize_config& c = h->loc_cfg;
@@ -5744,6 +5782,9 @@ static int loc_run(tloam_b200_handle* h, const double* d_in, size_t n, const dou
   out->n_query_points = (long long)nq; out->n_map_points = (long long)h->loc_n;
   h->loc_have_prev = true;
   h->loc_ran = true; h->loc_passes = nr ? s.iter + 1 : 0; h->loc_nq = nr; h->loc_last = a;
+  h->loc_serial++; h->loc_accepted = s.accepted != 0;
+  h->loc_src = d_in; h->loc_src_n = n; h->loc_src_raw = d_in == h->raw_scan;
+  h->loc_src_gen = h->loc_src_raw ? h->raw_gen : h->loc_in_gen;
   return TLOAM_B200_OK;
 }
 
@@ -5760,6 +5801,7 @@ int tloam_b200_localize(tloam_b200_handle* h, const double* xyz, size_t n, const
   CU_TRY(cudaSetDevice(h->device));
   int rc;
   if ((rc = ensure_dev(h, &h->d_loc_in, &h->cap_loc_in, n, false)) != TLOAM_B200_OK) return rc;
+  h->loc_in_gen++;                                              // the host cloud of an earlier localization is replaced
   if (n && (rc = upload_host(h, h->d_loc_in, xyz, n * 24)) != TLOAM_B200_OK) return rc;
   return loc_run(h, h->d_loc_in, n, guess, out);
 }
@@ -6102,6 +6144,7 @@ int tloam_b200_relocalize(tloam_b200_handle* h, const double* xyz, size_t n, tlo
   CU_TRY(cudaSetDevice(h->device));
   int rc;
   if ((rc = ensure_dev(h, &h->d_loc_in, &h->cap_loc_in, n, false)) != TLOAM_B200_OK) return rc;
+  h->loc_in_gen++;                                              // the host cloud of an earlier localization is replaced
   if (n && (rc = upload_host(h, h->d_loc_in, xyz, n * 24)) != TLOAM_B200_OK) return rc;
   return rl_run(h, h->d_loc_in, n, out);
 }
@@ -6134,6 +6177,453 @@ int tloam_b200_relocalize_matches(tloam_b200_handle* h, int hypothesis, int pass
   if (d2) CU_TRY(cudaMemcpyAsync(d2, a.match_d2 + off, nq * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   CU_TRY(cudaStreamSynchronize(h->stream));
   return TLOAM_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Updating a prior map (the checks, the state and the buffers here; the votes and the prior rows' compaction in
+// map_dynamic.cu, the novelty and the additions' voxels in map_update.cu, loaded from libtloam_b200_gmd.so and
+// libtloam_b200_mapu.so by the enable call).
+// ---------------------------------------------------------------------------------------------
+struct MuLib {
+  tloam_mu_add_fn pose = nullptr, novel = nullptr;
+  tloam_mu_scratch_bytes_fn scratch_bytes = nullptr;
+  tloam_mu_state_of_fn state_of = nullptr;
+  tloam_mu_build_fn bounds = nullptr, sort = nullptr, average = nullptr;
+};
+static std::mutex g_mu_mu;
+static MuLib g_mu;
+
+static int mu_load(tloam_b200_handle* h, MuLib* out) {
+  std::lock_guard<std::mutex> lk(g_mu_mu);
+  if (!g_mu.average) {
+    const std::string path = sibling_path("libtloam_b200_mapu.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    MuLib l;
+    if (so) {
+      l.pose = reinterpret_cast<tloam_mu_add_fn>(dlsym(so, "tloam_mu_pose"));
+      l.novel = reinterpret_cast<tloam_mu_add_fn>(dlsym(so, "tloam_mu_novel"));
+      l.scratch_bytes = reinterpret_cast<tloam_mu_scratch_bytes_fn>(dlsym(so, "tloam_mu_scratch_bytes"));
+      l.state_of = reinterpret_cast<tloam_mu_state_of_fn>(dlsym(so, "tloam_mu_state_of"));
+      l.bounds = reinterpret_cast<tloam_mu_build_fn>(dlsym(so, "tloam_mu_bounds"));
+      l.sort = reinterpret_cast<tloam_mu_build_fn>(dlsym(so, "tloam_mu_sort"));
+      l.average = reinterpret_cast<tloam_mu_build_fn>(dlsym(so, "tloam_mu_average"));
+    }
+    if (!l.pose || !l.novel || !l.scratch_bytes || !l.state_of || !l.bounds || !l.sort || !l.average) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "map update: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_mu = l;
+  }
+  *out = g_mu;
+  return TLOAM_B200_OK;
+}
+
+static int mu_status(tloam_b200_handle* h, int e, const char* where) {
+  if (e == cudaSuccess) return TLOAM_B200_OK;
+  snprintf(h->last_error, sizeof(h->last_error), "map update: %s: %s", where, cudaGetErrorString((cudaError_t)e));
+  return TLOAM_B200_ERR_CUDA;
+}
+
+// d_mu_small: the vote pose at 0, the prior rows' count at 128, the additions' count at 136, the compaction base at 144,
+// the built cloud's count at 152, the static part's block counts at 1024
+constexpr size_t kMuSmall = 1024 + 4 * 1024;
+static double* mu_pose(tloam_b200_handle* h) { return reinterpret_cast<double*>(h->d_mu_small); }
+static unsigned long long* mu_word(tloam_b200_handle* h, int k) {
+  return reinterpret_cast<unsigned long long*>(h->d_mu_small + 128 + 8 * k);
+}
+// the additions' arrays in d_mu_add for a capacity of cap rows
+struct MuAdd { double* xyz; unsigned* frame; unsigned* through; unsigned* hits; };
+static MuAdd mu_add_of(unsigned char* base, size_t cap) {
+  MuAdd a;
+  a.xyz = reinterpret_cast<double*>(base);
+  a.frame = reinterpret_cast<unsigned*>(base + round_up(cap * 24, 256));
+  a.through = reinterpret_cast<unsigned*>(base + round_up(cap * 24, 256) + round_up(cap * 4, 256));
+  a.hits = reinterpret_cast<unsigned*>(base + round_up(cap * 24, 256) + 2 * round_up(cap * 4, 256));
+  return a;
+}
+static size_t mu_add_bytes(size_t cap) { return round_up(cap * 24, 256) + 3 * round_up(cap * 4, 256); }
+
+// after a synchronisation: the buffers adds replaced (their last readers have finished)
+static void mu_free_retired(tloam_b200_handle* h) {
+  for (void* p : h->mu_retired) cudaFree(p);
+  h->mu_retired.clear();
+}
+
+// the prior rows' counters for the loaded map, allocated where the caller synchronises anyway (the enable, a load)
+static int mu_prior_alloc(tloam_b200_handle* h) {
+  const size_t n = h->loc_loaded ? h->loc_n : 0;
+  if (n <= h->cap_mu_prior) return TLOAM_B200_OK;
+  cudaFree(h->d_mu_prior); h->d_mu_prior = nullptr; h->cap_mu_prior = 0;
+  CU_TRY(cudaMalloc(&h->d_mu_prior, 2 * n * sizeof(unsigned)));
+  h->cap_mu_prior = n;
+  return TLOAM_B200_OK;
+}
+
+void tloam_b200_map_update_default_config(tloam_map_update_config* c) {
+  tloam_b200_global_map_dynamic_default_config(&c->image);
+  c->novel_radius = 0.5;
+  c->voxel = 0.5;
+  c->min_frames = 3;
+}
+
+int tloam_b200_map_update_enable(tloam_b200_handle* h, const tloam_map_update_config* c) {
+  if (!h || !c) return TLOAM_B200_ERR_INVALID_ARG;
+  std::vector<double> tab;
+  if (!gmd_config_valid(&c->image) || !gmd_tables(&c->image, &tab)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!std::isfinite(c->novel_radius) || !(c->novel_radius > 0.0) || !std::isfinite(c->voxel) || !(c->voxel > 0.0) ||
+      c->min_frames < 1)
+    return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loc_on) return TLOAM_B200_ERR_NOT_READY;
+  if (c->novel_radius > 3.0 * h->loc_cfg.cell) return TLOAM_B200_ERR_INVALID_ARG;   // the grid search's span
+  GmdLib gmd;
+  MuLib lib;
+  int rc;
+  if ((rc = gmd_load(h, &gmd)) != TLOAM_B200_OK || (rc = mu_load(h, &lib)) != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (tab.size() > h->cap_mu_tables) {
+    cudaFree(h->d_mu_tables); h->d_mu_tables = nullptr; h->cap_mu_tables = 0;
+    CU_TRY(cudaMalloc(&h->d_mu_tables, tab.size() * sizeof(double)));
+    h->cap_mu_tables = tab.size();
+  }
+  CU_TRY(cudaMemcpy(h->d_mu_tables, tab.data(), tab.size() * sizeof(double), cudaMemcpyHostToDevice));
+  const size_t pix = (size_t)c->image.n_rows * c->image.n_cols;
+  if (pix > h->cap_mu_image) {
+    cudaFree(h->d_mu_image); cudaFree(h->d_mu_window); h->d_mu_image = nullptr; h->d_mu_window = nullptr;
+    h->cap_mu_image = 0;
+    CU_TRY(cudaMalloc(&h->d_mu_image, pix * sizeof(unsigned long long)));
+    CU_TRY(cudaMalloc(&h->d_mu_window, pix * sizeof(double)));
+    h->cap_mu_image = pix;
+  }
+  if (!h->d_mu_small) CU_TRY(cudaMalloc(&h->d_mu_small, kMuSmall));
+  mu_free_retired(h);                                           // the stream is idle
+  h->mu_cfg = *c;
+  h->mu_on = true;
+  h->mu_fresh = true; h->mu_frames = 0; h->mu_built = false;
+  h->mu_min_serial = h->loc_serial + 1;                         // the next localization is the first an add may use
+  return mu_prior_alloc(h);
+}
+
+static int mu_after_load(tloam_b200_handle* h, int rc) {
+  if (rc != TLOAM_B200_OK || !h->mu_on) return rc;
+  mu_free_retired(h);                                           // the load synchronised
+  return mu_prior_alloc(h);
+}
+
+// an empty state: the prior rows' counters (loc_n of them, sized by the enable or the load) and the additions' count
+// cleared on the stream
+static int mu_reset(tloam_b200_handle* h) {
+  if (!h->mu_fresh) return TLOAM_B200_OK;
+  const size_t n = h->loc_n;
+  int rc;
+  if ((rc = mu_prior_alloc(h)) != TLOAM_B200_OK) return rc;     // sized already by the enable or the load
+  if (n) {
+    CU_TRY(cudaMemsetAsync(h->d_mu_prior, 0, n * sizeof(unsigned), h->stream));
+    CU_TRY(cudaMemsetAsync(h->d_mu_prior + h->cap_mu_prior, 0, n * sizeof(unsigned), h->stream));
+  }
+  CU_TRY(cudaMemsetAsync(mu_word(h, 1), 0, sizeof(unsigned long long), h->stream));
+  h->mu_known = 0; h->mu_pending = 0; h->mu_fresh = false;
+  return TLOAM_B200_OK;
+}
+
+// adds of the current query size the additions keep room for after a read-back of their count
+constexpr size_t kMuHeadroom = 16;
+
+// the additions hold at least `need` more rows.  The host bounds their count by the count at the last read-back plus the
+// query rows of every add since; only when that bound passes the capacity is the count read back (the add's one
+// synchronisation).  If the rows left then are fewer than kMuHeadroom adds of this size, the buffer grows (the rows copied
+// on the stream, the old buffer freed at a later synchronisation), so a read-back comes at most once per kMuHeadroom adds.
+static int mu_reserve(tloam_b200_handle* h, size_t need) {
+  if (h->mu_known + h->mu_pending + need <= h->cap_mu_add) return TLOAM_B200_OK;
+  if (h->mu_pending) {
+    unsigned long long n = 0;
+    CU_TRY(cudaMemcpyAsync(&n, mu_word(h, 1), sizeof(n), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    h->mu_known = (size_t)n; h->mu_pending = 0;
+    mu_free_retired(h);
+  }
+  if (h->cap_mu_add - h->mu_known >= kMuHeadroom * need) return TLOAM_B200_OK;
+  const size_t cap = std::max(2 * h->cap_mu_add, h->mu_known + h->mu_known / 2 + kMuHeadroom * need);
+  unsigned char* p = nullptr;
+  CU_TRY(cudaMalloc(&p, mu_add_bytes(cap)));
+  if (h->mu_known) {
+    const MuAdd o = mu_add_of(h->d_mu_add, h->cap_mu_add), q = mu_add_of(p, cap);
+    const size_t k = h->mu_known;
+    CU_TRY(cudaMemcpyAsync(q.xyz, o.xyz, k * 24, cudaMemcpyDeviceToDevice, h->stream));
+    CU_TRY(cudaMemcpyAsync(q.frame, o.frame, k * 4, cudaMemcpyDeviceToDevice, h->stream));
+    CU_TRY(cudaMemcpyAsync(q.through, o.through, k * 4, cudaMemcpyDeviceToDevice, h->stream));
+    CU_TRY(cudaMemcpyAsync(q.hits, o.hits, k * 4, cudaMemcpyDeviceToDevice, h->stream));
+  }
+  if (h->d_mu_add) h->mu_retired.push_back(h->d_mu_add);
+  h->d_mu_add = p; h->cap_mu_add = cap;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_map_update_add(tloam_b200_handle* h, tloam_map_update_add_result* out) {
+  if (!h || !out) return TLOAM_B200_ERR_INVALID_ARG;
+  memset(out, 0, sizeof(*out));
+  out->frame = -1;
+  if (!h->mu_on || !h->loc_loaded || !h->loc_ran || !h->loc_src || h->loc_serial < h->mu_min_serial ||
+      h->loc_serial == h->mu_added_serial)
+    return TLOAM_B200_ERR_NOT_READY;
+  // the scan the localization read is still in place (tloam_b200_global_map_append_frame's rule for the raw scan)
+  if (h->loc_src_raw ? (h->raw_gen != h->seg_gen || h->raw_gen != h->loc_src_gen) : h->loc_in_gen != h->loc_src_gen)
+    return TLOAM_B200_ERR_NOT_READY;
+  if (!h->loc_accepted) return TLOAM_B200_OK;
+  GmdLib gmd;
+  MuLib lib;
+  int rc;
+  if ((rc = gmd_load(h, &gmd)) != TLOAM_B200_OK || (rc = mu_load(h, &lib)) != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  if ((rc = mu_reset(h)) != TLOAM_B200_OK) return rc;
+  const size_t nq = h->loc_nq;
+  if ((rc = mu_reserve(h, nq)) != TLOAM_B200_OK) return rc;
+  const size_t q_bytes = round_up(nq, 256) + round_up(nq * 24, 256) + TLOAM_MU_MAX_BLOCKS * 4;
+  if (q_bytes > h->cap_mu_q) {                                  // the old buffer may still be read by the last add
+    if (h->d_mu_q) h->mu_retired.push_back(h->d_mu_q);
+    h->d_mu_q = nullptr; h->cap_mu_q = 0;
+    CU_TRY(cudaMalloc(&h->d_mu_q, q_bytes + q_bytes / 2));
+    h->cap_mu_q = q_bytes + q_bytes / 2;
+  }
+  const MuAdd ad = mu_add_of(h->d_mu_add, h->cap_mu_add);
+  tloam_mu_add_args a;
+  memset(&a, 0, sizeof(a));
+  a.grid = h->loc_index.grid;
+  a.query = h->d_loc_q; a.nq = nq;
+  a.state = h->loc_last.state;
+  a.radius = h->mu_cfg.novel_radius;
+  a.n_prior = h->loc_n;
+  a.pose = mu_pose(h); a.prior_count = mu_word(h, 0);
+  a.flag = h->d_mu_q;
+  a.p = reinterpret_cast<double*>(h->d_mu_q + round_up(nq, 256));
+  a.block_counts = reinterpret_cast<unsigned*>(h->d_mu_q + round_up(nq, 256) + round_up(nq * 24, 256));
+  a.base = mu_word(h, 2); a.count = mu_word(h, 1);
+  a.add_xyz = ad.xyz; a.add_frame = ad.frame; a.add_through = ad.through; a.add_hits = ad.hits;
+  a.frame = h->mu_frames;
+  a.device = h->device; a.stream = h->stream;
+  int e = 0, launches = 0;
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.pose(&a, &launches)));
+  h->launches += launches > 0 ? launches - 1 : 0;
+  if ((rc = mu_status(h, e, "k_mu_pose")) != TLOAM_B200_OK) return rc;
+  // the votes: the scan rows at T on the prior rows, then on the additions of the earlier adds
+  const tloam_global_map_dynamic_config& c = h->mu_cfg.image;
+  tloam_gmd_vote_args v;
+  memset(&v, 0, sizeof(v));
+  v.p.n_rows = c.n_rows; v.p.n_cols = c.n_cols; v.p.wr = c.window_rows; v.p.wc = c.window_cols;
+  v.p.margin_abs = c.margin_abs; v.p.margin_rel = c.margin_rel; v.p.min_range = c.min_range; v.p.max_range = c.max_range;
+  v.p.row_bounds = h->d_mu_tables; v.p.col_bounds = h->d_mu_tables + (c.n_rows + 1);
+  v.scan = h->loc_src; v.n = (unsigned)h->loc_src_n; v.pose = mu_pose(h);
+  v.image = h->d_mu_image; v.window = h->d_mu_window;
+  v.device = h->device; v.stream = h->stream;
+  for (int which = 0; which < 2; ++which) {
+    v.map = which ? ad.xyz : h->loc_index.map;
+    v.count = which ? mu_word(h, 1) : mu_word(h, 0);
+    v.through = which ? ad.through : h->d_mu_prior;
+    v.hits = which ? ad.hits : h->d_mu_prior + h->cap_mu_prior;
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = gmd.vote(&v, &launches)));
+    h->launches += launches > 0 ? launches - 1 : 0;
+    if ((rc = gmd_status(h, e, "k_gmd_vote")) != TLOAM_B200_OK) return rc;
+  }
+  if (nq) {
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.novel(&a, &launches)));
+    h->launches += launches > 0 ? launches - 1 : 0;
+    if ((rc = mu_status(h, e, "k_mu_novel / k_mu_count / k_mu_scatter")) != TLOAM_B200_OK) return rc;
+  }
+  out->used = 1;
+  out->frame = (long long)h->mu_frames;
+  out->n_scan_points = (long long)h->loc_src_n;
+  out->n_query_points = (long long)nq;
+  h->mu_frames++;
+  h->mu_pending += nq;
+  h->mu_added_serial = h->loc_serial;
+  return TLOAM_B200_OK;
+}
+
+// the additions' count (synchronises)
+static int mu_count(tloam_b200_handle* h, size_t* n) {
+  *n = 0;
+  if (h->mu_fresh) return TLOAM_B200_OK;
+  unsigned long long c = 0;
+  CU_TRY(cudaMemcpyAsync(&c, mu_word(h, 1), sizeof(c), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  mu_free_retired(h);
+  h->mu_known = (size_t)c; h->mu_pending = 0;
+  *n = (size_t)c;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_map_update_build(tloam_b200_handle* h, tloam_map_update_result* out) {
+  if (!h || !out) return TLOAM_B200_ERR_INVALID_ARG;
+  memset(out, 0, sizeof(*out));
+  if (!h->mu_on || !h->loc_loaded) return TLOAM_B200_ERR_NOT_READY;
+  GmdLib gmd;
+  MuLib lib;
+  int rc;
+  if ((rc = gmd_load(h, &gmd)) != TLOAM_B200_OK || (rc = mu_load(h, &lib)) != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  h->mu_built = false;                                          // a refused build leaves no cloud
+  if ((rc = mu_reset(h)) != TLOAM_B200_OK) return rc;
+  size_t n_add = 0;
+  if ((rc = mu_count(h, &n_add)) != TLOAM_B200_OK) return rc;
+  const size_t n_prior = h->loc_n, rows = n_prior + n_add;
+  if (rows * 3 > h->cap_mu_out) {
+    cudaFree(h->d_mu_out); h->d_mu_out = nullptr; h->cap_mu_out = 0;
+    CU_TRY(cudaMalloc(&h->d_mu_out, (rows + rows / 2 + 1) * 3 * sizeof(double)));
+    h->cap_mu_out = (rows + rows / 2 + 1) * 3;
+  }
+  const size_t bytes = lib.scratch_bytes(n_add);
+  if (bytes > h->cap_mu_build) {
+    cudaFree(h->d_mu_build); h->d_mu_build = nullptr; h->cap_mu_build = 0;
+    CU_TRY(cudaMalloc(&h->d_mu_build, bytes + bytes / 2));
+    h->cap_mu_build = bytes + bytes / 2;
+  }
+  int e = 0, launches = 0;
+  // the prior rows that are not removed, in row order, at the start of the cloud; their count in word 3
+  unsigned long long* total = mu_word(h, 3);
+  if (n_prior) {
+    tloam_gmd_static_args s;
+    memset(&s, 0, sizeof(s));
+    s.map = h->loc_index.map; s.through = h->d_mu_prior; s.hits = h->d_mu_prior + h->cap_mu_prior;
+    s.count = n_prior; s.min_through = (unsigned)h->mu_cfg.image.min_through;
+    s.block_counts = reinterpret_cast<unsigned*>(h->d_mu_small + 1024);
+    s.total = total; s.out_xyz = h->d_mu_out;
+    s.device = h->device; s.stream = h->stream;
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = gmd.compact(&s, &launches)));
+    h->launches += launches > 0 ? launches - 1 : 0;
+    if ((rc = gmd_status(h, e, "k_gmd_count / k_gmd_scatter")) != TLOAM_B200_OK) return rc;
+  } else {
+    CU_TRY(cudaMemsetAsync(total, 0, sizeof(unsigned long long), h->stream));
+  }
+  const MuAdd ad = mu_add_of(h->d_mu_add, h->cap_mu_add);
+  tloam_mu_build_args a;
+  memset(&a, 0, sizeof(a));
+  a.add_xyz = ad.xyz; a.add_frame = ad.frame; a.add_through = ad.through; a.add_hits = ad.hits;
+  a.n_add = n_add;
+  a.min_through = (unsigned)h->mu_cfg.image.min_through; a.min_frames = (unsigned)h->mu_cfg.min_frames;
+  a.voxel = h->mu_cfg.voxel;
+  a.scratch = h->d_mu_build; a.state = lib.state_of(h->d_mu_build, n_add);
+  a.count = total; a.out_xyz = h->d_mu_out;
+  a.device = h->device; a.stream = h->stream;
+  auto run = [&](tloam_mu_build_fn f, const char* where) -> int {
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = f(&a, &launches)));
+    h->launches += launches > 0 ? launches - 1 : 0;
+    return mu_status(h, e, where);
+  };
+  if ((rc = run(lib.bounds, "k_mu_bounds")) != TLOAM_B200_OK) return rc;
+  tloam_gmm_state gs;
+  unsigned long long kept_prior = 0;
+  CU_TRY(cudaMemcpyAsync(&gs, a.state, sizeof(gs), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaMemcpyAsync(&kept_prior, total, sizeof(kept_prior), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (gs.nonfinite) return TLOAM_B200_ERR_VOXEL_RANGE;
+  unsigned long long n_vox = 0, n_total = kept_prior;
+  if (gs.n_sel) {
+    for (int d = 0; d < 3; ++d) {                               // the merge's bounds, key range and bits
+      const double half = a.voxel * 0.5;
+      a.mb[d] = dec_ordered(~gs.lo[d]) - half;
+      const double ref = (dec_ordered(gs.hi[d]) - a.mb[d]) / a.voxel;
+      if (!(ref < (double)(1u << kGMapKeyBits))) return TLOAM_B200_ERR_VOXEL_RANGE;
+      const unsigned long long top = (unsigned long long)std::floor(ref);
+      int bits = 0;
+      while (bits < 64 && (top >> bits)) ++bits;
+      a.bits[d] = bits;
+    }
+    a.n_sel = gs.n_sel;
+    if ((rc = run(lib.sort, "k_mu_keys / k_gmm_*")) != TLOAM_B200_OK) return rc;
+    CU_TRY(cudaMemcpyAsync(&n_vox, &a.state->n_vox, sizeof(n_vox), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    a.n_vox = n_vox;
+    if ((rc = run(lib.average, "k_mu_average / k_mu_count / k_mu_scatter")) != TLOAM_B200_OK) return rc;
+    CU_TRY(cudaMemcpyAsync(&n_total, total, sizeof(n_total), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+  }
+  out->n_prior = (long long)n_prior;
+  out->n_prior_removed = (long long)(n_prior - kept_prior);
+  out->n_additions = (long long)n_add;
+  out->n_additions_removed = (long long)(n_add - gs.n_sel);
+  out->n_voxels = (long long)n_vox;
+  out->n_voxels_kept = (long long)(n_total - kept_prior);
+  out->n_total = (long long)n_total;
+  h->mu_built = true; h->mu_built_n = (size_t)n_total;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_map_update_size(tloam_b200_handle* h, size_t* n_prior, size_t* n_additions, size_t* n_built) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->mu_on || !h->loc_loaded) return TLOAM_B200_ERR_NOT_READY;
+  CU_TRY(cudaSetDevice(h->device));
+  size_t n = 0;
+  int rc;
+  if ((rc = mu_count(h, &n)) != TLOAM_B200_OK) return rc;
+  if (n_prior) *n_prior = h->loc_n;
+  if (n_additions) *n_additions = n;
+  if (n_built) *n_built = h->mu_built ? h->mu_built_n : 0;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_map_update_download(tloam_b200_handle* h, size_t first, size_t count, double* xyz) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->mu_on || !h->mu_built) return TLOAM_B200_ERR_NOT_READY;
+  if (first > h->mu_built_n || count > h->mu_built_n - first || (count && !xyz)) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  if (count) CU_TRY(cudaMemcpyAsync(xyz, h->d_mu_out + 3 * first, count * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_map_update_votes(tloam_b200_handle* h, int which, size_t first, size_t count, unsigned* through, unsigned* hits) {
+  if (!h || (which != 0 && which != 1)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->mu_on || !h->loc_loaded) return TLOAM_B200_ERR_NOT_READY;
+  CU_TRY(cudaSetDevice(h->device));
+  size_t n = 0;
+  int rc;
+  if ((rc = mu_count(h, &n)) != TLOAM_B200_OK) return rc;
+  const size_t rows = which ? n : h->loc_n;
+  if (first > rows || count > rows - first) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!count) return TLOAM_B200_OK;
+  if (h->mu_fresh) {                                            // nothing voted since the state was emptied
+    if (through) memset(through, 0, count * sizeof(unsigned));
+    if (hits) memset(hits, 0, count * sizeof(unsigned));
+    return TLOAM_B200_OK;
+  }
+  const MuAdd ad = mu_add_of(h->d_mu_add, h->cap_mu_add);
+  const unsigned* t = which ? ad.through : h->d_mu_prior;
+  const unsigned* s = which ? ad.hits : h->d_mu_prior + h->cap_mu_prior;
+  if (through) CU_TRY(cudaMemcpyAsync(through, t + first, count * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+  if (hits) CU_TRY(cudaMemcpyAsync(hits, s + first, count * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_map_update_additions(tloam_b200_handle* h, size_t first, size_t count, double* xyz, unsigned* frame) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->mu_on || !h->loc_loaded) return TLOAM_B200_ERR_NOT_READY;
+  CU_TRY(cudaSetDevice(h->device));
+  size_t n = 0;
+  int rc;
+  if ((rc = mu_count(h, &n)) != TLOAM_B200_OK) return rc;
+  if (first > n || count > n - first) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!count) return TLOAM_B200_OK;
+  const MuAdd ad = mu_add_of(h->d_mu_add, h->cap_mu_add);
+  if (xyz) CU_TRY(cudaMemcpyAsync(xyz, ad.xyz + 3 * first, count * 24, cudaMemcpyDeviceToHost, h->stream));
+  if (frame) CU_TRY(cudaMemcpyAsync(frame, ad.frame + first, count * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_localize_set_map_updated(tloam_b200_handle* h) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->loc_on || !h->mu_on || !h->mu_built) return TLOAM_B200_ERR_NOT_READY;
+  CU_TRY(cudaSetDevice(h->device));
+  const size_t n = h->mu_built_n;
+  h->loc_loaded = false; h->loc_have_prev = false; h->loc_ran = false; h->loc_passes = 0;
+  h->mu_fresh = true; h->mu_frames = 0;
+  int rc;
+  if ((rc = loc_reserve_map(h, n)) != TLOAM_B200_OK) return rc;
+  if (n) CU_TRY(cudaMemcpyAsync(h->d_loc_map, h->d_mu_out, n * 24, cudaMemcpyDeviceToDevice, h->stream));
+  return mu_after_load(h, loc_build(h, n));
 }
 
 int tloam_b200_host_alloc(void** p, size_t bytes) {

@@ -172,6 +172,28 @@ class RelocalizeResult:
 
 
 @dataclasses.dataclass(frozen=True)
+class MapUpdateAddResult:
+    """tloam_map_update_add_result: used = the last localization was accepted and voted; frame = this add's frame number
+    (-1 when not used); the scan rows that voted and the query rows tested for novelty."""
+    used: bool
+    frame: int
+    n_scan_points: int
+    n_query_points: int
+
+
+@dataclasses.dataclass(frozen=True)
+class MapUpdateResult:
+    """tloam_map_update_result: the counts of a build; n_total = kept prior rows + supported voxels."""
+    n_prior: int
+    n_prior_removed: int
+    n_additions: int
+    n_additions_removed: int
+    n_voxels: int
+    n_voxels_kept: int
+    n_total: int
+
+
+@dataclasses.dataclass(frozen=True)
 class PoseGraphResult:
     """tloam_pose_graph_result: termination is one of PoseGraphResult.CONVERGED .. NO_LOOPS; the costs are sum r^T Omega r
     at the odometry poses and at the returned poses; step_* are the last step's largest |upsilon| / |omega| component."""
@@ -1311,6 +1333,66 @@ class LocalRegistration:
         self._check(self._L.tloam_b200_relocalize_matches(self._h, int(hypothesis), int(k), idx.ctypes.data_as(C.POINTER(C.c_int)),
                                                           _dp(d2), n.value, C.byref(n)), "relocalize_matches")
         return idx, d2
+
+    # ---- updating a prior map (include/tloam_b200.h "Updating a prior map") ----
+    def map_update_enable(self, image=None, **overrides):
+        """turn updating of the loaded prior map on (localization must be on) and empty its state; image: a dict of
+        tloam_global_map_dynamic_config overrides for the votes' range image; overrides: novel_radius, voxel, min_frames"""
+        cfg = _lib.MapUpdateConfig()
+        self._L.tloam_b200_map_update_default_config(C.byref(cfg))
+        for k, v in (image or {}).items():
+            if not any(f[0] == k for f in cfg.image._fields_):
+                raise TypeError(f"unknown image field {k!r}")
+            setattr(cfg.image, k, v)
+        for k, v in overrides.items():
+            if k == "image" or not any(f[0] == k for f in cfg._fields_):
+                raise TypeError(f"unknown map-update field {k!r}")
+            setattr(cfg, k, v)
+        self._check(self._L.tloam_b200_map_update_enable(self._h, C.byref(cfg)), "map_update_enable")
+
+    def map_update_add(self):
+        """vote with the last localization's scan at its T and append its new query rows; a rejected localization gives
+        used=False and changes nothing.  Returns a MapUpdateAddResult"""
+        r = _lib.MapUpdateAddResult()
+        self._check(self._L.tloam_b200_map_update_add(self._h, C.byref(r)), "map_update_add")
+        return MapUpdateAddResult(bool(r.used), r.frame, r.n_scan_points, r.n_query_points)
+
+    def map_update_build(self):
+        """(xyz (n, 3), MapUpdateResult): the prior rows not removed, in row order, then the additions' voxels that enough
+        adds support"""
+        r = _lib.MapUpdateResult()
+        self._check(self._L.tloam_b200_map_update_build(self._h, C.byref(r)), "map_update_build")
+        xyz = np.zeros((r.n_total, 3))
+        self._check(self._L.tloam_b200_map_update_download(self._h, 0, r.n_total, _dp(xyz)), "map_update_download")
+        return xyz, MapUpdateResult(r.n_prior, r.n_prior_removed, r.n_additions, r.n_additions_removed, r.n_voxels,
+                                    r.n_voxels_kept, r.n_total)
+
+    def map_update_size(self):
+        """(prior rows, addition rows, built rows)"""
+        a, b, c = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+        self._check(self._L.tloam_b200_map_update_size(self._h, C.byref(a), C.byref(b), C.byref(c)), "map_update_size")
+        return a.value, b.value, c.value
+
+    def map_update_votes(self, which):
+        """(through, hits), uint32 each, of every prior row (which=0) or every addition (which=1)"""
+        n = self.map_update_size()[1 if which else 0]
+        t, h = np.zeros(n, dtype=np.uint32), np.zeros(n, dtype=np.uint32)
+        up = C.POINTER(C.c_uint)
+        self._check(self._L.tloam_b200_map_update_votes(self._h, int(which), 0, n, t.ctypes.data_as(up), h.ctypes.data_as(up)),
+                    "map_update_votes")
+        return t, h
+
+    def map_update_additions(self):
+        """(xyz (n, 3), frame (n,) uint32) of every addition, in the order they were appended"""
+        n = self.map_update_size()[1]
+        xyz, f = np.zeros((n, 3)), np.zeros(n, dtype=np.uint32)
+        self._check(self._L.tloam_b200_map_update_additions(self._h, 0, n, _dp(xyz), f.ctypes.data_as(C.POINTER(C.c_uint))),
+                    "map_update_additions")
+        return xyz, f
+
+    def localize_set_map_updated(self):
+        """load the last map_update_build on the device as the prior map"""
+        self._check(self._L.tloam_b200_localize_set_map_updated(self._h), "localize_set_map_updated")
 
     def loop_descriptors(self, first=0, count=None):
         """the descriptor slots of loop frames [first, first + count) in one copy (count None: to the last), count x slot:
