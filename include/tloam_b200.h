@@ -1386,6 +1386,80 @@ int tloam_b200_map_update_additions(tloam_b200_handle* h, size_t first, size_t c
  * built cloud.  Like every load it empties the update's state. */
 int tloam_b200_localize_set_map_updated(tloam_b200_handle* h);
 
+/* ---- Occupancy grid (opt-in): a 2D occupancy grid of the global map, in the layout of nav_msgs/OccupancyGrid, for a
+ * planner.  Every append records a 2D scan of its rows; a build rasterises every map frame's scan at the frame's current
+ * pose, so after tloam_b200_global_map_correct the next build follows the loop-corrected trajectory.  The map itself, its
+ * frame table, the intensity channel, the vote counters, the pose tables, the registered scan and the odometry keep the
+ * bits they have with the grid off.
+ *   - Enable.  tloam_b200_occupancy_enable is allowed only on an empty map (right after tloam_b200_global_map_enable or
+ *     _reset; otherwise NOT_READY).  tloam_b200_global_map_reset empties the captures and keeps the grid on;
+ *     tloam_b200_global_map_enable turns it off.  While it is off nothing is allocated or launched.
+ *   - Capture.  Every tloam_b200_global_map_append* variant (host, chained, _frame, intensity, packed) records, in the map
+ *     frame slot it takes, the pose it places the block at (the host pose, the device pose for _chained appends, or P_f
+ *     with correction tracking on) and the 2D scan of its sensor-frame rows, read before the transform.  A refused append
+ *     takes no slot, so the next append overwrites its record; an append of no rows records an empty scan.  Four launches
+ *     per append with rows, two without, and no synchronisation.  The records grow with the frame table.
+ *   - 2D scan.  A row (x, y, z) is used iff it is finite and min_range <= rho <= max_range, rho = sqrt(x x + y y).  Its
+ *     sector is Scan Context's sector rule on (x, y) with n_cols sectors ("Dynamic-point removal", Pixel of a used row).
+ *     The obstacle of sector j is the used row with z_lo <= z <= z_hi of least rho, the lowest row index on a tie; its
+ *     sensor-frame (x, y, z) is kept.  The floor of sector j is the largest rho of the used rows with z < z_lo.  Either may
+ *     be absent (NaN).
+ *   - Build pose.  P_f with correction tracking on, otherwise the recorded pose (the same bits until a correction).
+ *   - Extent.  W = (max_range + max(|z_lo|, |z_hi|)) + resolution.  origin_x = resolution floor((min_f t_x - W) /
+ *     resolution), width = floor(((max_f t_x + W) - origin_x) / resolution) + 1, likewise for y and height.  More than
+ *     2^28 cells is VOXEL_RANGE; an empty map gives a 0 x 0 grid.
+ *   - Free.  Per frame, every cell whose centre c satisfies |c - t| <= W on both axes, c_x = origin_x + ((double)i + 0.5)
+ *     resolution (likewise y): d = c - t in x and y, q_r = R(0, r) d0 + R(1, r) d1 for r = 0, 1 (R(k, r) = P[4r + k]),
+ *     rho_c = sqrt(q0 q0 + q1 q1), j the sector of (q0, q1).  The sector's extent e_j is its obstacle's rho, else its
+ *     floor's rho.  free += 1 iff e_j exists, rho_c >= min_range and rho_c + free_margin <= e_j.
+ *   - Occupied.  Each obstacle o moves to the world as w = P o with the point order of "Loop-corrected global map" (A
+ *     point); its cell (floor((w_x - origin_x) / resolution), likewise y) gets occupied += 1.  A hit outside the grid is
+ *     counted in dropped instead.  A cell may get both a free and a hit from one frame.
+ *   - Value.  With n = occupied + free: -1 if n = 0, else (100 occupied + n / 2) / n in integer arithmetic.  Cells are
+ *     row-major from cell (0, 0), i along x, with the origin at the corner of cell (0, 0): nav_msgs/OccupancyGrid's layout.
+ *   - Rounding.  Every product, sum, quotient and square root is rounded on its own (no FMA), left to right as written, so
+ *     tests/occupancy_oracle.py reproduces every scan, count and value bit for bit.
+ *   - Device.  A capture is k_occ_clear, k_occ_bin, k_occ_pick (ties by row index) and k_occ_final into the slot the device
+ *     frame count names.  A build is k_occ_extent (one read-back: it synchronises), then k_occ_free (one thread per frame
+ *     and window cell, integer atomicAdd), k_occ_hits (one per frame and sector) and k_occ_value, and a read-back of
+ *     dropped.  Memory: 32 B per sector and 128 B per frame slot; 9 B per cell, allocated by the first build with half as
+ *     much again, grown only and freed by tloam_b200_destroy.
+ *   - The kernels live in libtloam_b200_occ.so, loaded from this library's directory by the enable call; if it is missing
+ *     the calls return ERR_CUDA (tloam_b200_last_error names the file). */
+typedef struct tloam_occupancy_config {
+  double resolution;                   /* m per cell, > 0 */
+  int n_cols;                          /* sectors of the 2D scan, 1 .. 4096 */
+  double z_lo;                         /* the obstacle band in the sensor frame, m, z_lo < z_hi */
+  double z_hi;
+  double min_range;                    /* m, > 0 */
+  double max_range;                    /* m, >= min_range */
+  double free_margin;                  /* m, >= 0 */
+} tloam_occupancy_config;
+typedef struct tloam_occupancy_info {
+  double origin_x, origin_y;           /* the corner of cell (0, 0), m */
+  double resolution;
+  size_t width, height;                /* cells along x and y */
+  size_t frames;                       /* map frames rasterised */
+  unsigned long long dropped;          /* hits outside the grid */
+  unsigned long long cell_tests;       /* window cells the free pass visited (frames x its window's candidates) */
+} tloam_occupancy_info;
+/* an HDL-64E at 1.73 m: resolution 0.1 m, n_cols 1024, z_lo -1.2 m, z_hi 0.5 m, min_range 3 m, max_range 30 m,
+ * free_margin 0.1 m (DESIGN.md section 4c has how they were checked) */
+void tloam_b200_occupancy_default_config(tloam_occupancy_config* c);
+/* NOT_READY: mapping off, or the map is not empty.  INVALID_ARG: cfg null or a value outside its range above. */
+int tloam_b200_occupancy_enable(tloam_b200_handle* h, const tloam_occupancy_config* cfg);
+/* rasterises every map frame; synchronises.  NOT_READY: mapping or the grid off.  VOXEL_RANGE: more than 2^28 cells or a
+ * non-finite extent (no grid).  info may be null. */
+int tloam_b200_occupancy_build(tloam_b200_handle* h, tloam_occupancy_info* info);
+/* the last build's values, occupied and free counts (width x height each; any output may be null); synchronises.
+ * NOT_READY: the grid off, or no build since the enable or the last reset.  INVALID_ARG: capacity < width x height. */
+int tloam_b200_occupancy_download(tloam_b200_handle* h, signed char* cells, unsigned* occupied, unsigned* free_count,
+                                  size_t capacity);
+/* the 2D scans of map frames first .. first + count - 1: scans (count x n_cols x 4: obstacle x, y, z, floor rho; NaN when
+ * absent) and the recorded poses (count x 16, column-major); either may be null; synchronises.  NOT_READY: mapping or the
+ * grid off.  INVALID_ARG past the last frame. */
+int tloam_b200_occupancy_scans_download(tloam_b200_handle* h, size_t first, size_t count, double* scans, double* poses);
+
 /* Pinned host memory helpers (optional; pinned inputs make set_* a direct DMA, no staging threads). */
 int tloam_b200_host_alloc(void** p, size_t bytes);
 int tloam_b200_host_free(void* p);

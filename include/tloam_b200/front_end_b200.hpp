@@ -27,6 +27,7 @@
 #define TLOAM_B200_FRONT_END_B200_HPP
 
 #include <cmath>
+#include <cstdint>
 #include <cstdio>
 #include <string>
 #include <vector>
@@ -295,6 +296,24 @@ class FrontEndB200 {
     if (has) intensity.resize(n);
     return report(tloam_b200_global_map_static_download(h_, reinterpret_cast<double*>(out.data()),
                                                         has ? intensity.data() : nullptr, n, &n), "staticGlobalMap");
+  }
+
+  // The occupancy grid (include/tloam_b200.h "Occupancy grid"): right after enableGlobalMap, every later updateGlobalMap*
+  // records a 2D scan; occupancyGrid rasterises every map frame at its current pose.  cells is nav_msgs/OccupancyGrid's
+  // data (width x height, row-major from the origin's corner), so a node fills the message with one copy.
+  bool enableOccupancy(const tloam_occupancy_config& cfg) {
+    return report(tloam_b200_occupancy_enable(h_, &cfg), "enableOccupancy");
+  }
+  bool enableOccupancy() {
+    tloam_occupancy_config c;
+    tloam_b200_occupancy_default_config(&c);
+    return enableOccupancy(c);
+  }
+  bool occupancyGrid(std::vector<int8_t>& cells, tloam_occupancy_info& info) {
+    if (!report(tloam_b200_occupancy_build(h_, &info), "occupancyGrid")) return false;
+    cells.resize(info.width * info.height);
+    return report(tloam_b200_occupancy_download(h_, reinterpret_cast<signed char*>(cells.data()), nullptr, nullptr,
+                                                cells.size()), "occupancyGrid");
   }
 
   // The merged map (include/tloam_b200.h "Merged global map"): the whole map, or with static_only the points

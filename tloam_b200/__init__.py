@@ -4,6 +4,7 @@ The product is the C-ABI CUDA library `libtloam_b200.so` (sources in tloam_b200/
 include/tloam_b200.h).  This package is only the Python host-side mirror of the reference interface plus the
 synthetic-scene generator used by tests and bench.py.  Importing it never touches oracle/.
 """
+from .occupancy import save_occupancy_map  # noqa: F401
 from .registration import (BatchRegistration, Frame, LocalRegistration, LoopResult, LoopVerifyResult,  # noqa: F401
-                           PoseGraphResult, PoseGraphRobustResult, RegistrationError, default_config, packed_scan,
+                           OccupancyGrid, PoseGraphResult, PoseGraphRobustResult, RegistrationError, default_config, packed_scan,
                            packed_time)

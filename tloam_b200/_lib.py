@@ -147,6 +147,19 @@ class MapUpdateResult(C.Structure):
                 ("n_total", C.c_longlong)]
 
 
+class OccupancyConfig(C.Structure):
+    """tloam_occupancy_config (include/tloam_b200.h "Occupancy grid")."""
+    _fields_ = [("resolution", C.c_double), ("n_cols", C.c_int), ("z_lo", C.c_double), ("z_hi", C.c_double),
+                ("min_range", C.c_double), ("max_range", C.c_double), ("free_margin", C.c_double)]
+
+
+class OccupancyInfo(C.Structure):
+    """tloam_occupancy_info: the grid's origin, resolution and size, the frames rasterised, the dropped hits and the window
+    cells the free pass visited."""
+    _fields_ = [("origin_x", C.c_double), ("origin_y", C.c_double), ("resolution", C.c_double), ("width", C.c_size_t),
+                ("height", C.c_size_t), ("frames", C.c_size_t), ("dropped", C.c_ulonglong), ("cell_tests", C.c_ulonglong)]
+
+
 class PoseGraphConfig(C.Structure):
     """tloam_pose_graph_config (include/tloam_b200.h "Pose graph"): the edges' sigmas and the Gauss-Newton schedule."""
     _fields_ = [("sigma_odom_translation", C.c_double), ("sigma_odom_rotation", C.c_double),
@@ -293,6 +306,8 @@ EXPORTS = [
     "tloam_b200_map_update_default_config", "tloam_b200_map_update_enable", "tloam_b200_map_update_add",
     "tloam_b200_map_update_build", "tloam_b200_map_update_size", "tloam_b200_map_update_download",
     "tloam_b200_map_update_votes", "tloam_b200_map_update_additions", "tloam_b200_localize_set_map_updated",
+    "tloam_b200_occupancy_default_config", "tloam_b200_occupancy_enable", "tloam_b200_occupancy_build",
+    "tloam_b200_occupancy_download", "tloam_b200_occupancy_scans_download",
 ]
 
 _lib = None
@@ -526,5 +541,11 @@ def load():
     L.tloam_b200_map_update_votes.argtypes = [vp, C.c_int, C.c_size_t, C.c_size_t, up, up]
     L.tloam_b200_map_update_additions.argtypes = [vp, C.c_size_t, C.c_size_t, dp, up]
     L.tloam_b200_localize_set_map_updated.argtypes = [vp]
+    L.tloam_b200_occupancy_default_config.argtypes = [C.POINTER(OccupancyConfig)]
+    L.tloam_b200_occupancy_default_config.restype = None
+    L.tloam_b200_occupancy_enable.argtypes = [vp, C.POINTER(OccupancyConfig)]
+    L.tloam_b200_occupancy_build.argtypes = [vp, C.POINTER(OccupancyInfo)]
+    L.tloam_b200_occupancy_download.argtypes = [vp, C.POINTER(C.c_byte), up, up, C.c_size_t]
+    L.tloam_b200_occupancy_scans_download.argtypes = [vp, C.c_size_t, C.c_size_t, dp, dp]
     _lib = L
     return L

@@ -40,6 +40,7 @@
 #include "localize.h"
 #include "relocalize.h"
 #include "map_update.h"
+#include "occupancy.h"
 
 
 
@@ -231,6 +232,15 @@ struct tloam_b200_handle {
   unsigned long long* d_gmd_image = nullptr; double* d_gmd_window = nullptr; double* d_gmd_bounds = nullptr;
   size_t cap_gmd_image = 0, cap_gmd_bounds = 0;
   unsigned char* d_gmd_scratch = nullptr;  size_t cap_gmd_scratch = 0;                         // the static download
+  // ---- the occupancy grid (tloam_b200_occupancy*, libtloam_b200_occ.so): a 2D scan and a pose per frame slot, with the
+  //      capacity of the frame table; the sector boundaries; the last build's grid (occupied, free, values) ----
+  bool occ_on = false;
+  tloam_occupancy_config occ_cfg;
+  double* d_occ_scans = nullptr;           double* d_occ_poses = nullptr;   size_t cap_occ = 0;
+  double* d_occ_dirs = nullptr;            size_t cap_occ_dirs = 0;
+  unsigned char* d_occ_grid = nullptr;     size_t cap_occ_grid = 0;                            // cells of the buffer
+  unsigned char* d_occ_small = nullptr;    // the extent at 0, dropped at 64
+  bool occ_built = false;                  tloam_occupancy_info occ_info;
   // ---- the merged map (tloam_b200_global_map_merge*, libtloam_b200_gmm.so): the radix sort's scratch (24 B per map row)
   //      and the last merge's voxels (32 B each), allocated by the first merge and grown; the snapshot is dropped by
   //      enable / reset and by the next merge ----
@@ -542,6 +552,7 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   cudaFree(h->d_gmc_O); cudaFree(h->d_gmc_P); cudaFree(h->d_gmc_scratch);
   cudaFree(h->d_gmd_through); cudaFree(h->d_gmd_hits); cudaFree(h->d_gmd_image); cudaFree(h->d_gmd_window);
   cudaFree(h->d_gmd_bounds); cudaFree(h->d_gmd_scratch);
+  cudaFree(h->d_occ_scans); cudaFree(h->d_occ_poses); cudaFree(h->d_occ_dirs); cudaFree(h->d_occ_grid); cudaFree(h->d_occ_small);
   cudaFree(h->d_gmm_scratch); cudaFree(h->d_gmm_out);
   cudaFree(h->d_loc_map); cudaFree(h->d_loc_scratch); cudaFree(h->d_loc_qst); cudaFree(h->d_loc_reg); cudaFree(h->d_loc_fin);
   cudaFree(h->d_loc_q); cudaFree(h->d_loc_in); cudaFree(h->d_loc_run);
@@ -3437,6 +3448,7 @@ static int gmap_clear(tloam_b200_handle* h) {
   for (int k = 0; k < 16; ++k) h->gmc_M[k] = k % 5 == 0 ? 1.0 : 0.0;
   h->gmc_M_identity = true;                // the pose tables are empty with the frame table; tracking stays as it is
   h->gmm_valid = false;                    // the merged snapshot belonged to the map before
+  h->occ_built = false;                    // the grid too; the captures are indexed by the frame count, now 0
   if (h->gmd_on) {                         // every row starts at (0, 0); removal stays on
     CU_TRY(cudaMemsetAsync(h->d_gmd_through, 0, h->cap_gmd * sizeof(unsigned), h->stream));
     CU_TRY(cudaMemsetAsync(h->d_gmd_hits, 0, h->cap_gmd * sizeof(unsigned), h->stream));
@@ -3472,6 +3484,7 @@ int tloam_b200_global_map_enable(tloam_b200_handle* h, const tloam_global_map_co
   h->gmap_on = true;
   h->gmc_on = false;
   h->gmd_on = false;
+  h->occ_on = false;
   return gmap_clear(h);
 }
 
@@ -3540,6 +3553,19 @@ static int gmap_grow(tloam_b200_handle* h, size_t n) {
         *t = qt;
       }
       h->cap_gmc = ncap;
+    }
+    if (h->occ_on) {                       // the captures grow with the frame table
+      const size_t per[2] = {(size_t)h->occ_cfg.n_cols * TLOAM_OCC_SLOT, 16};
+      double** tabs[2] = {&h->d_occ_scans, &h->d_occ_poses};
+      for (int k = 0; k < 2; ++k) {
+        double* qt = nullptr;
+        CU_TRY(cudaMalloc(&qt, ncap * per[k] * sizeof(double)));
+        if (st.frames) CU_TRY(cudaMemcpyAsync(qt, *tabs[k], st.frames * per[k] * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
+        CU_TRY(cudaStreamSynchronize(h->stream));
+        cudaFree(*tabs[k]);
+        *tabs[k] = qt;
+      }
+      h->cap_occ = ncap;
     }
   }
   h->gmap_growths++;
@@ -3653,6 +3679,50 @@ static int gmd_status(tloam_b200_handle* h, int e, const char* where) {
   return TLOAM_B200_ERR_CUDA;
 }
 
+// ---- the occupancy grid's kernels live in libtloam_b200_occ.so (occupancy.cu), next to this library: loaded by
+//      tloam_b200_occupancy_enable, so that the kernels of this library keep their SASS and an append with the grid on
+//      cannot meet a missing library ----
+struct OccLib { tloam_occ_capture_fn capture = nullptr; tloam_occ_build_fn extent = nullptr, rasterise = nullptr; };
+static std::mutex g_occ_mu;
+static OccLib g_occ;
+
+static int occ_load(tloam_b200_handle* h, OccLib* out) {
+  std::lock_guard<std::mutex> lk(g_occ_mu);
+  if (!g_occ.capture) {
+    const std::string path = sibling_path("libtloam_b200_occ.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    OccLib l;
+    if (so) {
+      l.capture = reinterpret_cast<tloam_occ_capture_fn>(dlsym(so, "tloam_occ_capture"));
+      l.extent = reinterpret_cast<tloam_occ_build_fn>(dlsym(so, "tloam_occ_extent"));
+      l.rasterise = reinterpret_cast<tloam_occ_build_fn>(dlsym(so, "tloam_occ_rasterise"));
+    }
+    if (!l.capture || !l.extent || !l.rasterise) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "occupancy grid: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_occ = l;
+  }
+  *out = g_occ;
+  return TLOAM_B200_OK;
+}
+
+static int occ_status(tloam_b200_handle* h, int e, const char* where) {
+  if (e == cudaSuccess) return TLOAM_B200_OK;
+  snprintf(h->last_error, sizeof(h->last_error), "occupancy grid: %s: %s", where, cudaGetErrorString((cudaError_t)e));
+  return TLOAM_B200_ERR_CUDA;
+}
+
+static tloam_occ_params occ_params(const tloam_b200_handle* h) {
+  tloam_occ_params p;
+  const tloam_occupancy_config& c = h->occ_cfg;
+  p.n_cols = c.n_cols; p.z_lo = c.z_lo; p.z_hi = c.z_hi; p.min_range = c.min_range; p.max_range = c.max_range;
+  p.dirs = h->d_occ_dirs;
+  return p;
+}
+
 // device buffers of an intensity frame of n rows (after gmap_grow: d_gmi_map takes the map's current capacity)
 static int gmi_prepare(tloam_b200_handle* h, const GmiLib& lib, size_t n) {
   if (!h->d_gmi_st) {
@@ -3734,6 +3804,20 @@ static int gmap_append_impl(tloam_b200_handle* h, const double* pose_host, const
     TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = gmd.vote(&a, &launches)));
     h->launches += launches > 0 ? launches - 1 : 0;
     if ((rc = gmd_status(h, e, "k_gmd_vote")) != TLOAM_B200_OK) return rc;
+  }
+  if (h->occ_on) {                         // the 2D scan of the sensor-frame rows (before the transform below) and the
+    OccLib occ;                            // block's pose, into the slot of the device frame count
+    if ((rc = occ_load(h, &occ)) != TLOAM_B200_OK) return rc;
+    tloam_occ_capture_args a;
+    memset(&a, 0, sizeof(a));
+    a.p = occ_params(h);
+    a.scan = d_in; a.n = (unsigned)n; a.pose = d_pose; a.frames = &st->frames; a.cap = h->cap_occ;
+    a.scans = h->d_occ_scans; a.poses = h->d_occ_poses;
+    a.device = h->device; a.stream = h->stream;
+    int launches = 0, e = 0;
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = occ.capture(&a, &launches)));
+    h->launches += launches > 0 ? launches - 1 : 0;
+    if ((rc = occ_status(h, e, "k_occ_clear / _bin / _pick / _final")) != TLOAM_B200_OK) return rc;
   }
   CU_TRY(cudaMemsetAsync(&st->n_fin, 0, sizeof(GMapState) - offsetof(GMapState, n_fin), h->stream));
   const unsigned tb = 256, gb = (unsigned)((n + tb - 1) / tb);
@@ -5159,6 +5243,159 @@ int tloam_b200_global_map_static_download(tloam_b200_handle* h, double* xyz, dou
   if (*n) CU_TRY(cudaMemcpyAsync(xyz, a.out_xyz, *n * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   if (*n && intensity && has)
     CU_TRY(cudaMemcpyAsync(intensity, a.out_intensity, *n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Occupancy grid (the captures, the build's extent and the grid here and in gmap_append_impl / gmap_grow / gmap_clear; the
+// kernels in occupancy.cu, loaded from libtloam_b200_occ.so when the grid is enabled).
+// ---------------------------------------------------------------------------------------------
+void tloam_b200_occupancy_default_config(tloam_occupancy_config* c) {
+  c->resolution = 0.1; c->n_cols = 1024;   // an HDL-64E at 1.73 m
+  c->z_lo = -1.2; c->z_hi = 0.5;
+  c->min_range = 3.0; c->max_range = 30.0;
+  c->free_margin = 0.1;
+}
+
+static bool occ_config_valid(const tloam_occupancy_config* c) {
+  const auto fin = [](double v) { return std::isfinite(v); };
+  if (!fin(c->resolution) || !(c->resolution > 0.0) || c->n_cols < 1 || c->n_cols > 4096) return false;
+  if (!fin(c->z_lo) || !fin(c->z_hi) || !(c->z_lo < c->z_hi)) return false;
+  if (!fin(c->min_range) || !fin(c->max_range) || !(c->min_range > 0.0) || !(c->min_range <= c->max_range)) return false;
+  return fin(c->free_margin) && c->free_margin >= 0.0;
+}
+
+int tloam_b200_occupancy_enable(tloam_b200_handle* h, const tloam_occupancy_config* cfg) {
+  if (!h || !cfg || !occ_config_valid(cfg)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on || h->gmap_calls != 0) return TLOAM_B200_ERR_NOT_READY;
+  OccLib lib;
+  int rc = occ_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  std::vector<double> dirs(2 * (size_t)(cfg->n_cols - 1) + 1, 0.0);   // Scan Context's boundaries, as gmd_tables
+  for (int k = 1; k < cfg->n_cols; ++k) {
+    const double t = 2.0 * M_PI * k / cfg->n_cols;
+    dirs[2 * (k - 1)] = std::cos(t);
+    dirs[2 * (k - 1) + 1] = std::sin(t);
+  }
+  if (dirs.size() > h->cap_occ_dirs) {
+    cudaFree(h->d_occ_dirs); h->d_occ_dirs = nullptr; h->cap_occ_dirs = 0;
+    CU_TRY(cudaMalloc(&h->d_occ_dirs, dirs.size() * sizeof(double)));
+    h->cap_occ_dirs = dirs.size();
+  }
+  CU_TRY(cudaMemcpy(h->d_occ_dirs, dirs.data(), dirs.size() * sizeof(double), cudaMemcpyHostToDevice));
+  cudaFree(h->d_occ_scans); cudaFree(h->d_occ_poses); h->d_occ_scans = h->d_occ_poses = nullptr; h->cap_occ = 0;
+  CU_TRY(cudaMalloc(&h->d_occ_scans, h->cap_gmap_off * (size_t)cfg->n_cols * TLOAM_OCC_SLOT * sizeof(double)));
+  CU_TRY(cudaMalloc(&h->d_occ_poses, h->cap_gmap_off * 16 * sizeof(double)));
+  h->cap_occ = h->cap_gmap_off;
+  if (!h->d_occ_small) CU_TRY(cudaMalloc(&h->d_occ_small, 128));
+  h->occ_cfg = *cfg;
+  h->occ_on = true;
+  h->occ_built = false;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_occupancy_build(tloam_b200_handle* h, tloam_occupancy_info* info) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on || !h->occ_on) return TLOAM_B200_ERR_NOT_READY;
+  OccLib lib;
+  int rc = occ_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  GMapState st;
+  if ((rc = gmc_read(h, &st)) != TLOAM_B200_OK) return rc;   // the sticky flags stay for the next size / download call
+  h->occ_built = false;
+  const tloam_occupancy_config& c = h->occ_cfg;
+  tloam_occupancy_info out;
+  memset(&out, 0, sizeof(out));
+  out.resolution = c.resolution;
+  out.frames = st.frames;
+  if (st.frames) {
+    tloam_occ_build_args a;
+    memset(&a, 0, sizeof(a));
+    a.p = occ_params(h);
+    a.free_margin = c.free_margin; a.resolution = c.resolution;
+    const double za = std::fabs(c.z_lo) > std::fabs(c.z_hi) ? std::fabs(c.z_lo) : std::fabs(c.z_hi);
+    a.W = (c.max_range + za) + c.resolution;
+    a.scans = h->d_occ_scans;
+    a.poses = h->gmc_on ? h->d_gmc_P : h->d_occ_poses;
+    a.n_frames = st.frames;
+    a.extent = reinterpret_cast<double*>(h->d_occ_small);
+    a.dropped = reinterpret_cast<unsigned long long*>(h->d_occ_small + 64);
+    a.device = h->device; a.stream = h->stream;
+    int e = 0, launches = 0;
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.extent(&a, &launches)));
+    if ((rc = occ_status(h, e, "k_occ_extent")) != TLOAM_B200_OK) return rc;
+    double ext[4];
+    CU_TRY(cudaMemcpyAsync(ext, a.extent, sizeof(ext), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    const double r = c.resolution;
+    const double ox = r * std::floor((ext[0] - a.W) / r), oy = r * std::floor((ext[1] - a.W) / r);
+    const double fw = std::floor(((ext[2] + a.W) - ox) / r) + 1.0, fh = std::floor(((ext[3] + a.W) - oy) / r) + 1.0;
+    if (!std::isfinite(ox) || !std::isfinite(oy) || !std::isfinite(fw) || !std::isfinite(fh) || !(fw >= 1.0) || !(fh >= 1.0) ||
+        fw > (double)(1u << 28) || fh > (double)(1u << 28) || fw * fh > (double)(1u << 28))
+      return TLOAM_B200_ERR_VOXEL_RANGE;
+    a.origin_x = ox; a.origin_y = oy;
+    a.width = (unsigned)fw; a.height = (unsigned)fh;
+    a.nwin = (int)std::ceil(2.0 * a.W / r) + 3;          // any cell with |c - t| <= W lies in these candidates
+    const size_t cells = (size_t)a.width * a.height;
+    if (cells > h->cap_occ_grid) {
+      cudaFree(h->d_occ_grid); h->d_occ_grid = nullptr; h->cap_occ_grid = 0;
+      const size_t cap = cells + cells / 2;
+      CU_TRY(cudaMalloc(&h->d_occ_grid, cap * (2 * sizeof(unsigned) + 1)));
+      h->cap_occ_grid = cap;
+    }
+    a.occupied = reinterpret_cast<unsigned*>(h->d_occ_grid);
+    a.free_count = a.occupied + h->cap_occ_grid;
+    a.cells = reinterpret_cast<signed char*>(a.free_count + h->cap_occ_grid);
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.rasterise(&a, &launches)));
+    h->launches += launches > 0 ? launches - 1 : 0;
+    if ((rc = occ_status(h, e, "k_occ_free / _hits / _value")) != TLOAM_B200_OK) return rc;
+    unsigned long long dropped = 0;
+    CU_TRY(cudaMemcpyAsync(&dropped, a.dropped, sizeof(dropped), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    out.origin_x = ox; out.origin_y = oy; out.width = a.width; out.height = a.height;
+    out.dropped = dropped;
+    out.cell_tests = (unsigned long long)st.frames * (unsigned long long)a.nwin * (unsigned long long)a.nwin;
+  }
+  h->occ_info = out;
+  h->occ_built = true;
+  if (info) *info = out;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_occupancy_download(tloam_b200_handle* h, signed char* cells, unsigned* occupied, unsigned* free_count,
+                                  size_t capacity) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on || !h->occ_on || !h->occ_built) return TLOAM_B200_ERR_NOT_READY;
+  const size_t n = h->occ_info.width * h->occ_info.height;
+  if (capacity < n) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  if (n) {
+    const unsigned* occ = reinterpret_cast<const unsigned*>(h->d_occ_grid);
+    const unsigned* fr = occ + h->cap_occ_grid;
+    const signed char* v = reinterpret_cast<const signed char*>(fr + h->cap_occ_grid);
+    if (cells) CU_TRY(cudaMemcpyAsync(cells, v, n, cudaMemcpyDeviceToHost, h->stream));
+    if (occupied) CU_TRY(cudaMemcpyAsync(occupied, occ, n * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+    if (free_count) CU_TRY(cudaMemcpyAsync(free_count, fr, n * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+  }
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_occupancy_scans_download(tloam_b200_handle* h, size_t first, size_t count, double* scans, double* poses) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on || !h->occ_on) return TLOAM_B200_ERR_NOT_READY;
+  GMapState st;
+  int rc = gmc_read(h, &st);
+  if (rc != TLOAM_B200_OK) return rc;
+  if (first > st.frames || count > st.frames - first) return TLOAM_B200_ERR_INVALID_ARG;
+  const size_t per = (size_t)h->occ_cfg.n_cols * TLOAM_OCC_SLOT;
+  if (count && scans)
+    CU_TRY(cudaMemcpyAsync(scans, h->d_occ_scans + per * first, count * per * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (count && poses)
+    CU_TRY(cudaMemcpyAsync(poses, h->d_occ_poses + 16 * first, count * 16 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   CU_TRY(cudaStreamSynchronize(h->stream));
   return TLOAM_B200_OK;
 }

@@ -194,6 +194,22 @@ class MapUpdateResult:
 
 
 @dataclasses.dataclass(frozen=True)
+class OccupancyGrid:
+    """a built occupancy grid (include/tloam_b200.h "Occupancy grid"): cells (height, width) int8 in nav_msgs/OccupancyGrid's
+    values (-1 unknown, 0 .. 100), row j along y and column i along x, with the counts it came from (uint32 each); origin
+    = (x, y) of the corner of cell (0, 0); dropped = the hits outside the grid; cell_tests = the window cells the free
+    pass visited."""
+    cells: np.ndarray
+    occupied: np.ndarray
+    free: np.ndarray
+    origin: tuple
+    resolution: float
+    frames: int
+    dropped: int
+    cell_tests: int
+
+
+@dataclasses.dataclass(frozen=True)
 class PoseGraphResult:
     """tloam_pose_graph_result: termination is one of PoseGraphResult.CONVERGED .. NO_LOOPS; the costs are sum r^T Omega r
     at the odometry poses and at the returned poses; step_* are the last step's largest |upsilon| / |omega| component."""
@@ -1389,6 +1405,47 @@ class LocalRegistration:
         self._check(self._L.tloam_b200_map_update_additions(self._h, 0, n, _dp(xyz), f.ctypes.data_as(C.POINTER(C.c_uint))),
                     "map_update_additions")
         return xyz, f
+
+    # ---- occupancy grid (include/tloam_b200.h "Occupancy grid") ----
+    def occupancy_enable(self, **overrides):
+        """record a 2D scan per later append (only on an empty map); overrides: fields of tloam_occupancy_config
+        (resolution, n_cols, z_lo, z_hi, min_range, max_range, free_margin)"""
+        cfg = _lib.OccupancyConfig()
+        self._L.tloam_b200_occupancy_default_config(C.byref(cfg))
+        for k, v in overrides.items():
+            if not any(f[0] == k for f in cfg._fields_):
+                raise TypeError(f"unknown occupancy field {k!r}")
+            setattr(cfg, k, v)
+        self._check(self._L.tloam_b200_occupancy_enable(self._h, C.byref(cfg)), "occupancy_enable")
+        self._occupancy_cols = cfg.n_cols
+
+    def occupancy_build(self):
+        """rasterise every map frame at its current pose; returns an OccupancyGrid"""
+        info = _lib.OccupancyInfo()
+        self._check(self._L.tloam_b200_occupancy_build(self._h, C.byref(info)), "occupancy_build")
+        shape = (info.height, info.width)
+        cells = np.zeros(shape, dtype=np.int8)
+        occ, free = np.zeros(shape, dtype=np.uint32), np.zeros(shape, dtype=np.uint32)
+        up = C.POINTER(C.c_uint)
+        self._check(self._L.tloam_b200_occupancy_download(self._h, cells.ctypes.data_as(C.POINTER(C.c_byte)),
+                                                          occ.ctypes.data_as(up), free.ctypes.data_as(up), cells.size),
+                    "occupancy_download")
+        return OccupancyGrid(cells, occ, free, (info.origin_x, info.origin_y), info.resolution, info.frames, info.dropped,
+                             info.cell_tests)
+
+    def occupancy_scans(self, first=0, count=None):
+        """(obstacles (count, n_cols, 3), floors (count, n_cols), poses (count, 4, 4)) of map frames [first, first + count):
+        each sector's obstacle in the sensor frame and its floor range (NaN when absent), and the pose recorded at the
+        append"""
+        if count is None:
+            count = self.global_map_size()[1] - first
+        if first < 0 or count < 0:
+            raise RegistrationError(_lib.ERR_INVALID_ARG, "occupancy_scans_download")
+        n_cols = getattr(self, "_occupancy_cols", 0)
+        scans, poses = np.zeros((count, n_cols, 4)), np.zeros((count, 16))
+        self._check(self._L.tloam_b200_occupancy_scans_download(self._h, int(first), int(count), _dp(scans), _dp(poses)),
+                    "occupancy_scans_download")
+        return scans[:, :, :3].copy(), scans[:, :, 3].copy(), poses.reshape(count, 4, 4).transpose(0, 2, 1).copy()
 
     def localize_set_map_updated(self):
         """load the last map_update_build on the device as the prior map"""
