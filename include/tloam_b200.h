@@ -1460,6 +1460,83 @@ int tloam_b200_occupancy_download(tloam_b200_handle* h, signed char* cells, unsi
  * grid off.  INVALID_ARG past the last frame. */
 int tloam_b200_occupancy_scans_download(tloam_b200_handle* h, size_t first, size_t count, double* scans, double* poses);
 
+/* ---- Distance field and costmap: the distance from every cell of an occupancy grid to the nearest obstacle, for an
+ * optimisation-based planner, and costmap_2d's inflated costs, for a search-based one.
+ *   - Source.  tloam_b200_distance_build takes the last tloam_b200_occupancy_build's values on the device (NOT_READY when
+ *     the grid is off or not built since the enable or the last reset).  tloam_b200_distance_build_grid takes a host grid
+ *     in nav_msgs/OccupancyGrid's layout (int8, width x height, row-major from cell (0, 0), i along x, the origin at that
+ *     cell's corner) and works on any handle, mapping on or off: a map_server PGM saved by save_occupancy_map, say.
+ *   - Classes, those map_saver writes: obstacle v >= 65, free 0 <= v <= 25, unknown anything else (-1 included).  Unknown
+ *     cells are not obstacles.
+ *   - sq (uint32, cells^2): for a non-obstacle cell the least di^2 + dj^2 over the obstacle cells, for an obstacle cell
+ *     the same over the non-obstacle cells; 0xFFFFFFFF when that set is empty.  Exact integer arithmetic.
+ *   - sd (float32, m): (float)(sqrt((double)sq) * resolution), each operation rounded on its own, negated at obstacle
+ *     cells; +inf / -inf when sq is 0xFFFFFFFF.
+ *   - Cost (uint8, costmap_2d's codes; InflationLayer's costs at the exact distance).  An obstacle cell is 254 (LETHAL).
+ *     Otherwise, with R_c = (unsigned) ceil(inflation_radius / resolution) and dist = sqrt((double)sq): c = 253 if
+ *     sq <= R_c^2 and dist resolution <= inscribed_radius; (unsigned char)(252.0 exp(-cost_scaling_factor (dist
+ *     resolution - inscribed_radius))) if sq <= R_c^2 otherwise; 0 if sq > R_c^2.  A free cell gets c; an unknown cell
+ *     gets 253 if c = 253, else 255 (ROS 1's rule with inflate_unknown false).  The table of c by sq (R_c^2 + 1 entries)
+ *     is computed per build by this library with std::sqrt / std::exp and uploaded; the device only indexes it.
+ *     costmap_2d reaches cells through a wavefront from the obstacle cells, which can give a cell a farther obstacle than
+ *     the nearest one; this field uses the exact nearest obstacle and does not reproduce those cells.
+ *   - Values (int8): costmap_2d's Costmap2DPublisher table, 0 -> 0, 1 .. 252 -> 1 + (97 (c - 1)) / 251 in integer
+ *     arithmetic, 253 -> 99, 254 -> 100, 255 -> -1, so a node publishes the costmap as a nav_msgs/OccupancyGrid with one
+ *     copy.
+ *   - Query.  tloam_b200_distance_query gives the bilinear interpolation of sd at the cell centres and its gradient, in
+ *     FP64 with each product, sum and quotient rounded on its own (no FMA), left to right: u = (x - origin_x) / resolution
+ *     - 0.5, v likewise for y; a point is valid iff width >= 2, height >= 2, 0 <= u <= width - 1, 0 <= v <= height - 1;
+ *     i = min(floor(u), width - 2), j = min(floor(v), height - 2), a = u - i, b = v - j; with s_pq = sd(i + p, j + q):
+ *     d = (1 - b)((1 - a) s00 + a s10) + b((1 - a) s01 + a s11), gx = ((1 - b)(s10 - s00) + b(s11 - s01)) / resolution,
+ *     gy = ((1 - a)(s01 - s00) + a(s11 - s10)) / resolution.  An invalid point, and every point of a field with an infinite
+ *     value (no obstacle, or only obstacles), gives NaN in all three.
+ *   - Lifetime.  A field is a snapshot: a later occupancy build, a map reset or a correction leaves it alone.  The next
+ *     distance build replaces it (a build refused with INVALID_ARG, NOT_READY or VOXEL_RANGE keeps it) and
+ *     tloam_b200_destroy frees it.
+ *   - Limits.  (width - 1)^2 + (height - 1)^2 < 2^32 - 1, otherwise VOXEL_RANGE (a 5 528 x 6 238 grid is at 6.9e7).  A host
+ *     grid has 1 .. 2^28 cells, a finite origin and a finite resolution > 0; R_c <= 4096; 0 <= inscribed_radius <=
+ *     inflation_radius and cost_scaling_factor >= 0, all finite; otherwise INVALID_ARG.  A 0 x 0 occupancy grid (an empty
+ *     map) gives a 0 x 0 field.
+ *   - Unchanged.  Nothing is hooked into appends, captures or the occupancy build: the map, its tables, the occupancy
+ *     grid and the launch counts of every other call keep their bits, and nothing is allocated or loaded before the first
+ *     distance call.
+ *   - Device.  A build is k_dist_bands and k_dist_cols (the column pass, one thread per column and 64-row band),
+ *     k_dist_rows (one thread per row and source class: the lower envelope of g^2 + (i - k)^2 with every test in 64-bit
+ *     integers, cross-multiplied) and k_dist_cost (one per cell), then a read-back of the obstacle count: it synchronises.
+ *     A query is k_dist_query, one thread per point.  Memory: 19 B per cell (sq 4, sd 4, the column distance 4, the row
+ *     pass's stacks 4, a host grid's copy 1, cost 1, value 1), 16 B per column and band, R_c^2 + 1 B of table and 40 B per
+ *     query point, allocated by the first call that needs them, grown only and freed by tloam_b200_destroy.
+ *   - The kernels live in libtloam_b200_dist.so, loaded from this library's directory by the first distance call; if it
+ *     is missing the calls return ERR_CUDA (tloam_b200_last_error names the file). */
+typedef struct tloam_distance_config {
+  double inscribed_radius;             /* m: a cell this close to an obstacle is 253 (INSCRIBED) */
+  double inflation_radius;             /* m: the costs reach this far */
+  double cost_scaling_factor;          /* 1/m: the decay of the cost beyond the inscribed radius */
+} tloam_distance_config;
+typedef struct tloam_distance_info {
+  double origin_x, origin_y;           /* the corner of cell (0, 0), m */
+  double resolution;
+  size_t width, height;                /* cells along x and y */
+  size_t obstacles;                    /* obstacle cells (v >= 65) */
+} tloam_distance_info;
+/* inscribed_radius 0.9 m (half of a 1.8 m-wide car), inflation_radius 3.0 m, cost_scaling_factor 3.0 (nav2's
+ * inflation-layer default).  These are robot parameters, not calibrated: set them for the robot that plans. */
+void tloam_b200_distance_default_config(tloam_distance_config* c);
+/* from the last occupancy build; synchronises.  INVALID_ARG: cfg null or out of range.  NOT_READY: the occupancy grid off
+ * or not built.  VOXEL_RANGE: the grid is too large (Limits).  info may be null. */
+int tloam_b200_distance_build(tloam_b200_handle* h, const tloam_distance_config* cfg, tloam_distance_info* info);
+/* from a host grid (cells: width x height int8); synchronises.  INVALID_ARG / VOXEL_RANGE as in Limits.  info may be null. */
+int tloam_b200_distance_build_grid(tloam_b200_handle* h, const tloam_distance_config* cfg, const signed char* cells,
+                                   size_t width, size_t height, double origin_x, double origin_y, double resolution,
+                                   tloam_distance_info* info);
+/* the last build's sd, sq, costs and values (width x height each, the grid's layout; any output may be null);
+ * synchronises.  NOT_READY before any build.  INVALID_ARG: capacity < width x height. */
+int tloam_b200_distance_download(tloam_b200_handle* h, float* sd, unsigned* sq, unsigned char* costs, signed char* values,
+                                 size_t capacity);
+/* n points xy (n x 2, m) -> distance (n) and gradient (n x 2, m per m), either may be null; synchronises.  NOT_READY
+ * before any build.  INVALID_ARG: xy null with n > 0. */
+int tloam_b200_distance_query(tloam_b200_handle* h, const double* xy, size_t n, double* distance, double* gradient);
+
 /* Pinned host memory helpers (optional; pinned inputs make set_* a direct DMA, no staging threads). */
 int tloam_b200_host_alloc(void** p, size_t bytes);
 int tloam_b200_host_free(void* p);

@@ -21,6 +21,8 @@
 // enableLocalization / localizeFrame register each frame against a prior map; enableRelocalization / setPlaces /
 // relocalizeFrame find the first pose in that map (or the pose after tracking is lost) from a recorded session's places;
 // enableMapUpdate / addMapUpdateFrame / buildUpdatedMap keep that map up to date from the localized frames.
+// enableOccupancy / occupancyGrid give a 2D occupancy grid of the map; distanceField / queryDistance its distance field
+// and inflated costmap, or those of a saved grid.
 // Without the reference headers (this repository's tests) define TLOAM_B200_MOCK_HOST_TYPES and provide the host types
 // (tests/mock/mock_tloam.hpp).
 #ifndef TLOAM_B200_FRONT_END_B200_HPP
@@ -316,6 +318,32 @@ class FrontEndB200 {
                                                 cells.size()), "occupancyGrid");
   }
 
+  // The distance field and costmap (include/tloam_b200.h "Distance field and costmap") of the last occupancyGrid, or of a
+  // host grid in nav_msgs/OccupancyGrid's layout (a saved map in a localization session).  sd is the signed distance in
+  // m, costs costmap_2d's codes, values the costmap as nav_msgs/OccupancyGrid data (one copy into the message).
+  bool distanceField(const tloam_distance_config& cfg, std::vector<float>& sd, std::vector<uint8_t>& costs,
+                     std::vector<int8_t>& values, tloam_distance_info& info) {
+    if (!report(tloam_b200_distance_build(h_, &cfg, &info), "distanceField")) return false;
+    return downloadDistance(sd, costs, values, info);
+  }
+  bool distanceField(const tloam_distance_config& cfg, const std::vector<int8_t>& cells, size_t width, size_t height,
+                     double origin_x, double origin_y, double resolution, std::vector<float>& sd,
+                     std::vector<uint8_t>& costs, std::vector<int8_t>& values, tloam_distance_info& info) {
+    if (cells.size() != width * height) return report(TLOAM_B200_ERR_INVALID_ARG, "distanceField");
+    if (!report(tloam_b200_distance_build_grid(h_, &cfg, reinterpret_cast<const signed char*>(cells.data()), width, height,
+                                               origin_x, origin_y, resolution, &info), "distanceField"))
+      return false;
+    return downloadDistance(sd, costs, values, info);
+  }
+  // the last field's distance at the points xy (n x 2, m) and its gradient (n x 2), bilinear between the cell centres;
+  // NaN outside them
+  bool queryDistance(const std::vector<double>& xy, std::vector<double>& distance, std::vector<double>& gradient) {
+    const size_t n = xy.size() / 2;
+    distance.resize(n);
+    gradient.resize(2 * n);
+    return report(tloam_b200_distance_query(h_, xy.data(), n, distance.data(), gradient.data()), "queryDistance");
+  }
+
   // The merged map (include/tloam_b200.h "Merged global map"): the whole map, or with static_only the points
   // staticGlobalMap keeps, merged into one voxel grid -- VoxelDownSample(voxel) of the map, the cloud to publish or save.
   bool mergedGlobalMap(double voxel, bool static_only, std::vector<Eigen::Vector3d>& out) {
@@ -470,6 +498,15 @@ class FrontEndB200 {
     return !c.cloud_ptr->intensity_.empty() && c.cloud_ptr->intensity_.size() == c.cloud_ptr->points_.size();
   }
   static const double* intensity(const CloudData& c) { return c.cloud_ptr->intensity_.data(); }
+  bool downloadDistance(std::vector<float>& sd, std::vector<uint8_t>& costs, std::vector<int8_t>& values,
+                        const tloam_distance_info& info) {
+    const size_t n = info.width * info.height;
+    sd.resize(n);
+    costs.resize(n);
+    values.resize(n);
+    return report(tloam_b200_distance_download(h_, sd.data(), nullptr, costs.data(), reinterpret_cast<signed char*>(values.data()),
+                                               n), "distanceField");
+  }
   bool report(int rc, const char* where) {
     last_status_ = rc;
     if (rc != TLOAM_B200_OK)

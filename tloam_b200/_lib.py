@@ -160,6 +160,17 @@ class OccupancyInfo(C.Structure):
                 ("height", C.c_size_t), ("frames", C.c_size_t), ("dropped", C.c_ulonglong), ("cell_tests", C.c_ulonglong)]
 
 
+class DistanceConfig(C.Structure):
+    """tloam_distance_config (include/tloam_b200.h "Distance field and costmap")."""
+    _fields_ = [("inscribed_radius", C.c_double), ("inflation_radius", C.c_double), ("cost_scaling_factor", C.c_double)]
+
+
+class DistanceInfo(C.Structure):
+    """tloam_distance_info: the field's origin, resolution and size, and its obstacle cells."""
+    _fields_ = [("origin_x", C.c_double), ("origin_y", C.c_double), ("resolution", C.c_double), ("width", C.c_size_t),
+                ("height", C.c_size_t), ("obstacles", C.c_size_t)]
+
+
 class PoseGraphConfig(C.Structure):
     """tloam_pose_graph_config (include/tloam_b200.h "Pose graph"): the edges' sigmas and the Gauss-Newton schedule."""
     _fields_ = [("sigma_odom_translation", C.c_double), ("sigma_odom_rotation", C.c_double),
@@ -308,6 +319,8 @@ EXPORTS = [
     "tloam_b200_map_update_votes", "tloam_b200_map_update_additions", "tloam_b200_localize_set_map_updated",
     "tloam_b200_occupancy_default_config", "tloam_b200_occupancy_enable", "tloam_b200_occupancy_build",
     "tloam_b200_occupancy_download", "tloam_b200_occupancy_scans_download",
+    "tloam_b200_distance_default_config", "tloam_b200_distance_build", "tloam_b200_distance_build_grid",
+    "tloam_b200_distance_download", "tloam_b200_distance_query",
 ]
 
 _lib = None
@@ -547,5 +560,13 @@ def load():
     L.tloam_b200_occupancy_build.argtypes = [vp, C.POINTER(OccupancyInfo)]
     L.tloam_b200_occupancy_download.argtypes = [vp, C.POINTER(C.c_byte), up, up, C.c_size_t]
     L.tloam_b200_occupancy_scans_download.argtypes = [vp, C.c_size_t, C.c_size_t, dp, dp]
+    L.tloam_b200_distance_default_config.argtypes = [C.POINTER(DistanceConfig)]
+    L.tloam_b200_distance_default_config.restype = None
+    L.tloam_b200_distance_build.argtypes = [vp, C.POINTER(DistanceConfig), C.POINTER(DistanceInfo)]
+    L.tloam_b200_distance_build_grid.argtypes = [vp, C.POINTER(DistanceConfig), C.POINTER(C.c_byte), C.c_size_t, C.c_size_t,
+                                                 C.c_double, C.c_double, C.c_double, C.POINTER(DistanceInfo)]
+    L.tloam_b200_distance_download.argtypes = [vp, C.POINTER(C.c_float), up, C.POINTER(C.c_ubyte), C.POINTER(C.c_byte),
+                                               C.c_size_t]
+    L.tloam_b200_distance_query.argtypes = [vp, dp, C.c_size_t, dp, dp]
     _lib = L
     return L

@@ -41,6 +41,7 @@
 #include "relocalize.h"
 #include "map_update.h"
 #include "occupancy.h"
+#include "distance.h"
 
 
 
@@ -241,6 +242,15 @@ struct tloam_b200_handle {
   unsigned char* d_occ_grid = nullptr;     size_t cap_occ_grid = 0;                            // cells of the buffer
   unsigned char* d_occ_small = nullptr;    // the extent at 0, dropped at 64
   bool occ_built = false;                  tloam_occupancy_info occ_info;
+  // ---- the distance field (tloam_b200_distance*, libtloam_b200_dist.so): the last build's cells (sq, sd, the column
+  //      distance, the row pass's stacks, a host grid's copy, costs, values: 19 B each), the column pass's band records,
+  //      the cost table and the query's points; allocated by the first call that needs them, grown only ----
+  unsigned char* d_dist = nullptr;         size_t cap_dist = 0;                                // cells of the buffer
+  unsigned* d_dist_bands = nullptr;        size_t cap_dist_bands = 0;
+  unsigned char* d_dist_table = nullptr;   size_t cap_dist_table = 0;
+  unsigned long long* d_dist_small = nullptr;                                                  // the obstacle count
+  double* d_dist_q = nullptr;              size_t cap_dist_q = 0;                              // points: xy, distance, gradient
+  bool dist_built = false;                 tloam_distance_info dist_info;
   // ---- the merged map (tloam_b200_global_map_merge*, libtloam_b200_gmm.so): the radix sort's scratch (24 B per map row)
   //      and the last merge's voxels (32 B each), allocated by the first merge and grown; the snapshot is dropped by
   //      enable / reset and by the next merge ----
@@ -553,6 +563,7 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   cudaFree(h->d_gmd_through); cudaFree(h->d_gmd_hits); cudaFree(h->d_gmd_image); cudaFree(h->d_gmd_window);
   cudaFree(h->d_gmd_bounds); cudaFree(h->d_gmd_scratch);
   cudaFree(h->d_occ_scans); cudaFree(h->d_occ_poses); cudaFree(h->d_occ_dirs); cudaFree(h->d_occ_grid); cudaFree(h->d_occ_small);
+  cudaFree(h->d_dist); cudaFree(h->d_dist_bands); cudaFree(h->d_dist_table); cudaFree(h->d_dist_small); cudaFree(h->d_dist_q);
   cudaFree(h->d_gmm_scratch); cudaFree(h->d_gmm_out);
   cudaFree(h->d_loc_map); cudaFree(h->d_loc_scratch); cudaFree(h->d_loc_qst); cudaFree(h->d_loc_reg); cudaFree(h->d_loc_fin);
   cudaFree(h->d_loc_q); cudaFree(h->d_loc_in); cudaFree(h->d_loc_run);
@@ -5396,6 +5407,228 @@ int tloam_b200_occupancy_scans_download(tloam_b200_handle* h, size_t first, size
     CU_TRY(cudaMemcpyAsync(scans, h->d_occ_scans + per * first, count * per * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   if (count && poses)
     CU_TRY(cudaMemcpyAsync(poses, h->d_occ_poses + 16 * first, count * 16 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Distance field and costmap (the checks, the cost table and the buffers here; the kernels in distance.cu, loaded from
+// libtloam_b200_dist.so by the first distance call, so that the kernels of this library keep their SASS).
+// ---------------------------------------------------------------------------------------------
+struct DistLib { tloam_dist_build_fn build = nullptr; tloam_dist_query_fn query = nullptr; };
+static std::mutex g_dist_mu;
+static DistLib g_dist;
+
+static int dist_load(tloam_b200_handle* h, DistLib* out) {
+  std::lock_guard<std::mutex> lk(g_dist_mu);
+  if (!g_dist.build) {
+    const std::string path = sibling_path("libtloam_b200_dist.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    DistLib l;
+    if (so) {
+      l.build = reinterpret_cast<tloam_dist_build_fn>(dlsym(so, "tloam_dist_build"));
+      l.query = reinterpret_cast<tloam_dist_query_fn>(dlsym(so, "tloam_dist_query"));
+    }
+    if (!l.build || !l.query) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "distance field: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_dist = l;
+  }
+  *out = g_dist;
+  return TLOAM_B200_OK;
+}
+
+static int dist_status(tloam_b200_handle* h, int e, const char* where) {
+  if (e == cudaSuccess) return TLOAM_B200_OK;
+  snprintf(h->last_error, sizeof(h->last_error), "distance field: %s: %s", where, cudaGetErrorString((cudaError_t)e));
+  return TLOAM_B200_ERR_CUDA;
+}
+
+void tloam_b200_distance_default_config(tloam_distance_config* c) {
+  c->inscribed_radius = 0.9;               // half of a 1.8 m-wide car; robot parameters, not calibrated
+  c->inflation_radius = 3.0;
+  c->cost_scaling_factor = 3.0;            // nav2's inflation-layer default
+}
+
+static bool dist_config_valid(const tloam_distance_config* c) {
+  const auto fin = [](double v) { return std::isfinite(v); };
+  if (!fin(c->inscribed_radius) || !fin(c->inflation_radius) || !fin(c->cost_scaling_factor)) return false;
+  return c->inscribed_radius >= 0.0 && c->inscribed_radius <= c->inflation_radius && c->cost_scaling_factor >= 0.0;
+}
+
+// R_c^2 of cfg at this resolution; false when R_c > 4096
+static bool dist_r2(const tloam_distance_config* c, double resolution, unsigned* r2) {
+  const double rc = std::ceil(c->inflation_radius / resolution);
+  if (!(rc <= 4096.0)) return false;
+  *r2 = (unsigned)rc * (unsigned)rc;
+  return true;
+}
+
+// the build of a grid whose cells are on the device at `cells` (width x height, checked); info may be null
+static int dist_run(tloam_b200_handle* h, const DistLib& lib, const tloam_distance_config* cfg, const signed char* cells,
+                    bool upload_from_host, size_t width, size_t height, double ox, double oy, double res, unsigned r2,
+                    tloam_distance_info* info) {
+  h->dist_built = false;
+  const size_t n = width * height;
+  tloam_distance_info out;
+  memset(&out, 0, sizeof(out));
+  out.origin_x = ox; out.origin_y = oy; out.resolution = res; out.width = width; out.height = height;
+  CU_TRY(cudaSetDevice(h->device));
+  if (n) {
+    if (n > h->cap_dist) {
+      CU_TRY(cudaStreamSynchronize(h->stream));
+      cudaFree(h->d_dist); h->d_dist = nullptr; h->cap_dist = 0;
+      CU_TRY(cudaMalloc(&h->d_dist, n * 19));
+      h->cap_dist = n;
+    }
+    const size_t nb = width * ((height + TLOAM_DIST_BAND - 1) / TLOAM_DIST_BAND);
+    if (nb > h->cap_dist_bands) {
+      CU_TRY(cudaStreamSynchronize(h->stream));
+      cudaFree(h->d_dist_bands); h->d_dist_bands = nullptr; h->cap_dist_bands = 0;
+      CU_TRY(cudaMalloc(&h->d_dist_bands, nb * 4 * sizeof(unsigned)));
+      h->cap_dist_bands = nb;
+    }
+    if ((size_t)r2 + 1 > h->cap_dist_table) {
+      CU_TRY(cudaStreamSynchronize(h->stream));
+      cudaFree(h->d_dist_table); h->d_dist_table = nullptr; h->cap_dist_table = 0;
+      CU_TRY(cudaMalloc(&h->d_dist_table, (size_t)r2 + 1));
+      h->cap_dist_table = (size_t)r2 + 1;
+    }
+    if (!h->d_dist_small) CU_TRY(cudaMalloc(&h->d_dist_small, 64));
+    // c by sq: InflationLayer::computeCost of the distance sqrt(sq) in cells
+    std::vector<unsigned char> table((size_t)r2 + 1);
+    table[0] = 254;
+    for (unsigned s = 1; s <= r2; ++s) {
+      const double dist = std::sqrt((double)s);
+      table[s] = dist * res <= cfg->inscribed_radius ? (unsigned char)253
+               : (unsigned char)(252.0 * std::exp(-cfg->cost_scaling_factor * (dist * res - cfg->inscribed_radius)));
+    }
+    CU_TRY(cudaMemcpyAsync(h->d_dist_table, table.data(), table.size(), cudaMemcpyHostToDevice, h->stream));
+    const size_t cap = h->cap_dist;
+    tloam_dist_build_args a;
+    memset(&a, 0, sizeof(a));
+    a.sq = reinterpret_cast<unsigned*>(h->d_dist);
+    a.sd = reinterpret_cast<float*>(h->d_dist + 4 * cap);
+    a.g = reinterpret_cast<unsigned*>(h->d_dist + 8 * cap);
+    a.stack = reinterpret_cast<unsigned short*>(h->d_dist + 12 * cap);
+    signed char* grid = reinterpret_cast<signed char*>(h->d_dist + 16 * cap);
+    a.costs = h->d_dist + 17 * cap;
+    a.values = reinterpret_cast<signed char*>(h->d_dist + 18 * cap);
+    if (upload_from_host) CU_TRY(cudaMemcpyAsync(grid, cells, n, cudaMemcpyHostToDevice, h->stream));
+    a.cells = upload_from_host ? grid : cells;   // the kernels read the source only during the build
+    a.width = (unsigned)width; a.height = (unsigned)height; a.resolution = res;
+    a.bands = h->d_dist_bands;
+    a.table = h->d_dist_table; a.r2 = r2;
+    a.obstacles = h->d_dist_small;
+    a.device = h->device; a.stream = h->stream;
+    int e = 0, launches = 0;
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.build(&a, &launches)));
+    h->launches += launches > 0 ? launches - 1 : 0;
+    int rc = dist_status(h, e, "k_dist_bands / _cols / _rows / _cost");
+    if (rc != TLOAM_B200_OK) return rc;
+    unsigned long long obstacles = 0;
+    CU_TRY(cudaMemcpyAsync(&obstacles, h->d_dist_small, sizeof(obstacles), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    out.obstacles = (size_t)obstacles;
+  }
+  h->dist_info = out;
+  h->dist_built = true;
+  if (info) *info = out;
+  return TLOAM_B200_OK;
+}
+
+static bool dist_shape_ok(size_t width, size_t height) {   // (width - 1)^2 + (height - 1)^2 < 2^32 - 1
+  if (width == 0 || height == 0) return true;
+  if (width > 65537 || height > 65537) return false;
+  const unsigned long long a = width - 1, b = height - 1;
+  return a * a + b * b < 0xFFFFFFFFull;
+}
+
+int tloam_b200_distance_build(tloam_b200_handle* h, const tloam_distance_config* cfg, tloam_distance_info* info) {
+  if (!h || !cfg || !dist_config_valid(cfg)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on || !h->occ_on || !h->occ_built) return TLOAM_B200_ERR_NOT_READY;
+  const tloam_occupancy_info& g = h->occ_info;
+  unsigned r2 = 0;
+  if (!dist_r2(cfg, g.resolution, &r2)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!dist_shape_ok(g.width, g.height)) return TLOAM_B200_ERR_VOXEL_RANGE;
+  DistLib lib;
+  int rc = dist_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  const unsigned* occ = reinterpret_cast<const unsigned*>(h->d_occ_grid);
+  const signed char* values = reinterpret_cast<const signed char*>(occ + 2 * h->cap_occ_grid);
+  return dist_run(h, lib, cfg, values, false, g.width, g.height, g.origin_x, g.origin_y, g.resolution, r2, info);
+}
+
+int tloam_b200_distance_build_grid(tloam_b200_handle* h, const tloam_distance_config* cfg, const signed char* cells,
+                                   size_t width, size_t height, double origin_x, double origin_y, double resolution,
+                                   tloam_distance_info* info) {
+  if (!h || !cfg || !dist_config_valid(cfg) || !cells || width == 0 || height == 0 || width > (1u << 28) ||
+      height > (1u << 28) || width * height > (1u << 28) || !std::isfinite(origin_x) || !std::isfinite(origin_y) ||
+      !std::isfinite(resolution) || !(resolution > 0.0))
+    return TLOAM_B200_ERR_INVALID_ARG;
+  unsigned r2 = 0;
+  if (!dist_r2(cfg, resolution, &r2)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!dist_shape_ok(width, height)) return TLOAM_B200_ERR_VOXEL_RANGE;
+  DistLib lib;
+  int rc = dist_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  return dist_run(h, lib, cfg, cells, true, width, height, origin_x, origin_y, resolution, r2, info);
+}
+
+int tloam_b200_distance_download(tloam_b200_handle* h, float* sd, unsigned* sq, unsigned char* costs, signed char* values,
+                                 size_t capacity) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->dist_built) return TLOAM_B200_ERR_NOT_READY;
+  const size_t n = h->dist_info.width * h->dist_info.height;
+  if (capacity < n) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  if (n) {
+    const size_t cap = h->cap_dist;
+    if (sq) CU_TRY(cudaMemcpyAsync(sq, h->d_dist, n * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+    if (sd) CU_TRY(cudaMemcpyAsync(sd, h->d_dist + 4 * cap, n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+    if (costs) CU_TRY(cudaMemcpyAsync(costs, h->d_dist + 17 * cap, n, cudaMemcpyDeviceToHost, h->stream));
+    if (values) CU_TRY(cudaMemcpyAsync(values, h->d_dist + 18 * cap, n, cudaMemcpyDeviceToHost, h->stream));
+  }
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_distance_query(tloam_b200_handle* h, const double* xy, size_t n, double* distance, double* gradient) {
+  if (!h || (n && !xy)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->dist_built) return TLOAM_B200_ERR_NOT_READY;
+  DistLib lib;
+  int rc = dist_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  if (n) {
+    if (n > h->cap_dist_q) {
+      CU_TRY(cudaStreamSynchronize(h->stream));
+      cudaFree(h->d_dist_q); h->d_dist_q = nullptr; h->cap_dist_q = 0;
+      CU_TRY(cudaMalloc(&h->d_dist_q, n * 5 * sizeof(double)));
+      h->cap_dist_q = n;
+    }
+    const tloam_distance_info& f = h->dist_info;
+    const size_t cells = f.width * f.height;
+    tloam_dist_query_args a;
+    memset(&a, 0, sizeof(a));
+    a.sd = reinterpret_cast<const float*>(h->d_dist + 4 * h->cap_dist);
+    a.width = (unsigned)f.width; a.height = (unsigned)f.height;
+    a.origin_x = f.origin_x; a.origin_y = f.origin_y; a.resolution = f.resolution;
+    a.finite = f.obstacles > 0 && f.obstacles < cells;          // else every sd is +inf or -inf
+    a.xy = h->d_dist_q; a.n = n;
+    a.distance = h->d_dist_q + 2 * n; a.gradient = h->d_dist_q + 3 * n;
+    a.device = h->device; a.stream = h->stream;
+    CU_TRY(cudaMemcpyAsync(h->d_dist_q, xy, n * 2 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    int e = 0, launches = 0;
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.query(&a, &launches)));
+    h->launches += launches > 0 ? launches - 1 : 0;
+    if ((rc = dist_status(h, e, "k_dist_query")) != TLOAM_B200_OK) return rc;
+    if (distance) CU_TRY(cudaMemcpyAsync(distance, a.distance, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    if (gradient) CU_TRY(cudaMemcpyAsync(gradient, a.gradient, n * 2 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  }
   CU_TRY(cudaStreamSynchronize(h->stream));
   return TLOAM_B200_OK;
 }

@@ -194,6 +194,21 @@ class MapUpdateResult:
 
 
 @dataclasses.dataclass(frozen=True)
+class DistanceField:
+    """a built distance field (include/tloam_b200.h "Distance field and costmap"), each (height, width) in the grid's
+    layout: signed = sd (float32, m, negative at obstacle cells, +-inf without a cell of the other class), sq (uint32,
+    the squared distance in cells), costs (uint8, costmap_2d's codes), values (int8, Costmap2DPublisher's values); origin
+    = (x, y) of the corner of cell (0, 0); obstacles = the obstacle cells."""
+    signed: np.ndarray
+    sq: np.ndarray
+    costs: np.ndarray
+    values: np.ndarray
+    origin: tuple
+    resolution: float
+    obstacles: int
+
+
+@dataclasses.dataclass(frozen=True)
 class OccupancyGrid:
     """a built occupancy grid (include/tloam_b200.h "Occupancy grid"): cells (height, width) int8 in nav_msgs/OccupancyGrid's
     values (-1 unknown, 0 .. 100), row j along y and column i along x, with the counts it came from (uint32 each); origin
@@ -1446,6 +1461,44 @@ class LocalRegistration:
         self._check(self._L.tloam_b200_occupancy_scans_download(self._h, int(first), int(count), _dp(scans), _dp(poses)),
                     "occupancy_scans_download")
         return scans[:, :, :3].copy(), scans[:, :, 3].copy(), poses.reshape(count, 4, 4).transpose(0, 2, 1).copy()
+
+    # ---- distance field and costmap (include/tloam_b200.h "Distance field and costmap") ----
+    def distance_build(self, grid=None, origin=None, resolution=None, **overrides):
+        """the distance field and costmap of the last occupancy_build (grid None), or of a host grid: (height, width) int8
+        in nav_msgs/OccupancyGrid's values with its origin (x, y) and resolution; overrides: fields of
+        tloam_distance_config (inscribed_radius, inflation_radius, cost_scaling_factor).  Returns a DistanceField."""
+        cfg = _lib.DistanceConfig()
+        self._L.tloam_b200_distance_default_config(C.byref(cfg))
+        for k, v in overrides.items():
+            if not any(f[0] == k for f in cfg._fields_):
+                raise TypeError(f"unknown distance field {k!r}")
+            setattr(cfg, k, v)
+        info = _lib.DistanceInfo()
+        if grid is None:
+            self._check(self._L.tloam_b200_distance_build(self._h, C.byref(cfg), C.byref(info)), "distance_build")
+        else:
+            g = np.ascontiguousarray(grid, dtype=np.int8)
+            if g.ndim != 2 or origin is None or resolution is None:
+                raise RegistrationError(_lib.ERR_INVALID_ARG, "distance_build_grid")
+            self._check(self._L.tloam_b200_distance_build_grid(
+                self._h, C.byref(cfg), g.ctypes.data_as(C.POINTER(C.c_byte)), g.shape[1], g.shape[0], float(origin[0]),
+                float(origin[1]), float(resolution), C.byref(info)), "distance_build_grid")
+        shape = (info.height, info.width)
+        sd, sq = np.zeros(shape, dtype=np.float32), np.zeros(shape, dtype=np.uint32)
+        costs, values = np.zeros(shape, dtype=np.uint8), np.zeros(shape, dtype=np.int8)
+        self._check(self._L.tloam_b200_distance_download(
+            self._h, sd.ctypes.data_as(C.POINTER(C.c_float)), sq.ctypes.data_as(C.POINTER(C.c_uint)),
+            costs.ctypes.data_as(C.POINTER(C.c_ubyte)), values.ctypes.data_as(C.POINTER(C.c_byte)), sd.size),
+            "distance_download")
+        return DistanceField(sd, sq, costs, values, (info.origin_x, info.origin_y), info.resolution, info.obstacles)
+
+    def distance_query(self, xy):
+        """(distance (n,), gradient (n, 2)) of the last distance_build at the points xy (n, 2): sd interpolated bilinearly
+        between the cell centres, NaN outside them or on a field with an infinite value"""
+        p = np.ascontiguousarray(xy, dtype=np.float64).reshape(-1, 2)
+        d, g = np.zeros(len(p)), np.zeros((len(p), 2))
+        self._check(self._L.tloam_b200_distance_query(self._h, _dp(p), len(p), _dp(d), _dp(g)), "distance_query")
+        return d, g
 
     def localize_set_map_updated(self):
         """load the last map_update_build on the device as the prior map"""
