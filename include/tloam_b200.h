@@ -1537,6 +1537,83 @@ int tloam_b200_distance_download(tloam_b200_handle* h, float* sd, unsigned* sq, 
  * before any build.  INVALID_ARG: xy null with n > 0. */
 int tloam_b200_distance_query(tloam_b200_handle* h, const double* xy, size_t n, double* distance, double* gradient);
 
+/* ---- Path planning: the cost-to-go of every cell of the costmap to a goal (a global planner's potential), and the path
+ * down it from any start.
+ *   - Source.  The costs (costmap_2d's codes) of the last successful tloam_b200_distance_build or _build_grid, so a plan
+ *     runs on the device's own occupancy grid or on a host grid (a localization session's saved PGM).  NOT_READY before
+ *     any distance build.
+ *   - Cell cost.  A cell is passable when its code c is 0 .. 252, or 255 with allow_unknown set; its traversal cost is then
+ *     t = neutral_cost + cost_factor c, with c = 252 for an unknown cell, in integer arithmetic.  253 (INSCRIBED) and 254
+ *     (LETHAL) are never passable, nor 255 with allow_unknown 0.  Limits: neutral_cost >= 1, neutral_cost + 252
+ *     cost_factor <= 65535 (every t fits 16 bits), allow_unknown 0 or 1; otherwise INVALID_ARG.
+ *   - Moves.  8-connected.  A move into a passable neighbour u costs 70 t(u) to a side neighbour and 99 t(u) to a diagonal
+ *     one (99 / 70 = 1.41429); a diagonal move is allowed only when both side cells that share its corner are passable, so
+ *     no path cuts a corner.  The cost is charged on the cell entered: the goal's t counts, the start's does not.
+ *   - Potential P (uint64): the least total cost of a path from a cell to the goal, 0xFFFFFFFFFFFFFFFF at impassable cells
+ *     and at cells that cannot reach the goal.  It is the unique solution of P(goal) = 0, P(v) = min over the allowed moves
+ *     v -> u of (k t(u) + P(u)): unique because every move costs at least 70, so any order of relaxation gives the same
+ *     bits.  Every finite P is below 2^53, so a float64 Dijkstra is exact on the same costs.
+ *   - Cells from points: (floor((x - origin_x) / resolution), floor((y - origin_y) / resolution)), each operation rounded
+ *     on its own (the occupancy build's hit rule).  A goal that is not finite, lies outside the grid or falls on an
+ *     impassable cell gives INVALID_ARG.
+ *   - Paths.  From a start s the path repeats one step until it reaches the goal: the next cell is the first allowed
+ *     neighbour, in the order (di, dj) = (+1, 0), (0, +1), (-1, 0), (0, -1), (+1, +1), (-1, +1), (-1, -1), (+1, -1), that
+ *     minimises k t(u) + P(u).  That minimum is P(v), so every step lowers P by at least 70 and the walk ends.  A path
+ *     lists its cells from the start to the goal, both included (one cell for a start on the goal); its cost is P(start).
+ *     Status per start: 0 reached; 1 the start is not finite or lies outside the grid; 2 the start cell is impassable; 3
+ *     the goal cannot be reached.  A start with a status other than 0 has no cells and the cost 0xFFFFFFFFFFFFFFFF.  The
+ *     xy of a path cell is its centre, origin + (i + 0.5) resolution, each operation rounded on its own.
+ *   - Lifetime.  A build copies t into the plan's own memory, so the potential is a snapshot: a later distance build,
+ *     occupancy build or map call leaves it and the kept paths alone.  The next plan build replaces it and drops the kept
+ *     paths (a build refused with INVALID_ARG or NOT_READY keeps both); the next tloam_b200_plan_paths replaces the paths;
+ *     tloam_b200_destroy frees them.
+ *   - Unchanged.  Nothing is hooked into any other call: the distance field, the occupancy grid, the map and the launch
+ *     counts of every other call keep their bits, and nothing is allocated or loaded before the first plan call.
+ *   - Device.  A build is k_plan_init (one thread per cell: t, P = INF but 0 at the goal; the goal's 32 x 32-cell tile
+ *     and the tiles around it as the first round's work), then rounds of k_plan_round, launched in batches of 32 with a read-back of the next round's work
+ *     count after each batch.  A round's blocks each take tiles of the round's worklist, stage a tile's P and t with a
+ *     one-cell halo in shared memory, relax it in place to local convergence and write back the cells that fell with a
+ *     64-bit atomicMin; a tile whose halo holds a cell that fell is queued for the next round, once per round.  Then
+ *     k_plan_count counts the reachable cells: it synchronises.  Paths are k_plan_length (one thread per start: the status,
+ *     the cost and the path's length), a read-back of the lengths, the offsets summed on the host and k_plan_walk (one
+ *     thread per start: the cells).  Memory: 10 B per cell (P 8, t 2), 12 B per tile (a stamp and two worklists), 32 B
+ *     per start and 8 B per path cell, allocated by the first call that needs them, grown only and freed by
+ *     tloam_b200_destroy.
+ *   - The kernels live in libtloam_b200_plan.so, loaded from this library's directory by the first plan call; if it is
+ *     missing the calls return ERR_CUDA (tloam_b200_last_error names the file). */
+typedef struct tloam_plan_config {
+  unsigned neutral_cost;               /* the cost of a free cell, per 70 of a side move */
+  unsigned cost_factor;                /* the cost per costmap code */
+  int allow_unknown;                   /* 1: unknown cells (255) are passable at code 252 */
+} tloam_plan_config;
+typedef struct tloam_plan_info {
+  double origin_x, origin_y;           /* the corner of cell (0, 0), m: the distance field's */
+  double resolution;
+  size_t width, height;                /* cells along x and y */
+  size_t goal_i, goal_j;               /* the goal's cell */
+  size_t reachable;                    /* cells with a finite potential, the goal included */
+  unsigned long long rounds;           /* rounds of k_plan_round that had work */
+  unsigned long long tiles;            /* tiles those rounds relaxed */
+} tloam_plan_info;
+/* neutral_cost 50, cost_factor 3, allow_unknown 1 (global_planner's defaults) */
+void tloam_b200_plan_default_config(tloam_plan_config* c);
+/* the potential to the goal (goal_x, goal_y) on the last distance field's costs; synchronises.  INVALID_ARG: cfg null or
+ * out of range, or a bad goal (Cells from points).  NOT_READY: no distance build yet.  info may be null. */
+int tloam_b200_plan_build(tloam_b200_handle* h, const tloam_plan_config* cfg, double goal_x, double goal_y,
+                          tloam_plan_info* info);
+/* the last plan's P (width x height, the grid's layout; may be null); synchronises.  NOT_READY before any plan build.
+ * INVALID_ARG: capacity < width x height. */
+int tloam_b200_plan_download(tloam_b200_handle* h, unsigned long long* potential, size_t capacity);
+/* the paths from n starts (starts_xy: n x 2, m) down the last plan, kept on the device for tloam_b200_plan_path_cells:
+ * offsets (n + 1: path s is cells offsets[s] .. offsets[s + 1] - 1), statuses (n) and costs (n), each may be null;
+ * synchronises.  NOT_READY before any plan build.  INVALID_ARG: starts_xy null with n > 0, or n > 2^24. */
+int tloam_b200_plan_paths(tloam_b200_handle* h, const double* starts_xy, size_t n, size_t* offsets, int* statuses,
+                          unsigned long long* costs);
+/* the cells of the last tloam_b200_plan_paths, all paths one after the other: ij (2 ints each) and xy (the centres, 2
+ * FP64 each), either may be null; synchronises.  NOT_READY before any tloam_b200_plan_paths since the last plan build.
+ * INVALID_ARG: capacity < offsets[n] of that call. */
+int tloam_b200_plan_path_cells(tloam_b200_handle* h, int* ij, double* xy, size_t capacity);
+
 /* Pinned host memory helpers (optional; pinned inputs make set_* a direct DMA, no staging threads). */
 int tloam_b200_host_alloc(void** p, size_t bytes);
 int tloam_b200_host_free(void* p);

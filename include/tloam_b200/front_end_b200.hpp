@@ -22,7 +22,7 @@
 // relocalizeFrame find the first pose in that map (or the pose after tracking is lost) from a recorded session's places;
 // enableMapUpdate / addMapUpdateFrame / buildUpdatedMap keep that map up to date from the localized frames.
 // enableOccupancy / occupancyGrid give a 2D occupancy grid of the map; distanceField / queryDistance its distance field
-// and inflated costmap, or those of a saved grid.
+// and inflated costmap, or those of a saved grid; planPotential / planPaths plan paths on that costmap.
 // Without the reference headers (this repository's tests) define TLOAM_B200_MOCK_HOST_TYPES and provide the host types
 // (tests/mock/mock_tloam.hpp).
 #ifndef TLOAM_B200_FRONT_END_B200_HPP
@@ -342,6 +342,33 @@ class FrontEndB200 {
     distance.resize(n);
     gradient.resize(2 * n);
     return report(tloam_b200_distance_query(h_, xy.data(), n, distance.data(), gradient.data()), "queryDistance");
+  }
+
+  // Path planning (include/tloam_b200.h "Path planning") on the last distanceField's costs: the potential to the goal
+  // (goal_x, goal_y), width x height in the grid's layout (0xFFFFFFFFFFFFFFFF: impassable or cut off).
+  bool planPotential(const tloam_plan_config& cfg, double goal_x, double goal_y, std::vector<unsigned long long>& potential,
+                     tloam_plan_info& info) {
+    if (!report(tloam_b200_plan_build(h_, &cfg, goal_x, goal_y, &info), "planPotential")) return false;
+    potential.resize(info.width * info.height);
+    return report(tloam_b200_plan_download(h_, potential.data(), potential.size()), "planPotential");
+  }
+  // the paths from the starts xy (n x 2, m) down the last planPotential: per start the cell centres from the start to the
+  // goal as x, y pairs (a nav_msgs/Path's poses, empty unless the status is 0), the status (0 reached, 1 start outside
+  // the grid, 2 start impassable, 3 goal unreachable) and the cost
+  bool planPaths(const std::vector<double>& starts_xy, std::vector<std::vector<double>>& paths_xy,
+                 std::vector<int>& statuses, std::vector<unsigned long long>& costs) {
+    const size_t n = starts_xy.size() / 2;
+    std::vector<size_t> offsets(n + 1);
+    statuses.resize(n);
+    costs.resize(n);
+    if (!report(tloam_b200_plan_paths(h_, starts_xy.data(), n, offsets.data(), statuses.data(), costs.data()), "planPaths"))
+      return false;
+    std::vector<double> xy(2 * offsets[n]);
+    if (!report(tloam_b200_plan_path_cells(h_, nullptr, xy.data(), offsets[n]), "planPaths")) return false;
+    paths_xy.assign(n, std::vector<double>());
+    for (size_t s = 0; s < n; ++s)
+      paths_xy[s].assign(xy.begin() + 2 * offsets[s], xy.begin() + 2 * offsets[s + 1]);
+    return true;
   }
 
   // The merged map (include/tloam_b200.h "Merged global map"): the whole map, or with static_only the points

@@ -6,5 +6,5 @@ synthetic-scene generator used by tests and bench.py.  Importing it never touche
 """
 from .occupancy import save_occupancy_map  # noqa: F401
 from .registration import (BatchRegistration, DistanceField, Frame, LocalRegistration, LoopResult, LoopVerifyResult,  # noqa: F401
-                           OccupancyGrid, PoseGraphResult, PoseGraphRobustResult, RegistrationError, default_config, packed_scan,
-                           packed_time)
+                           OccupancyGrid, PlanField, PlanPath, PoseGraphResult, PoseGraphRobustResult, RegistrationError,
+                           default_config, packed_scan, packed_time)

@@ -171,6 +171,18 @@ class DistanceInfo(C.Structure):
                 ("height", C.c_size_t), ("obstacles", C.c_size_t)]
 
 
+class PlanConfig(C.Structure):
+    """tloam_plan_config (include/tloam_b200.h "Path planning")."""
+    _fields_ = [("neutral_cost", C.c_uint), ("cost_factor", C.c_uint), ("allow_unknown", C.c_int)]
+
+
+class PlanInfo(C.Structure):
+    """tloam_plan_info: the plan's origin, resolution and size, its goal cell, reachable cells, rounds and tiles."""
+    _fields_ = [("origin_x", C.c_double), ("origin_y", C.c_double), ("resolution", C.c_double), ("width", C.c_size_t),
+                ("height", C.c_size_t), ("goal_i", C.c_size_t), ("goal_j", C.c_size_t), ("reachable", C.c_size_t),
+                ("rounds", C.c_ulonglong), ("tiles", C.c_ulonglong)]
+
+
 class PoseGraphConfig(C.Structure):
     """tloam_pose_graph_config (include/tloam_b200.h "Pose graph"): the edges' sigmas and the Gauss-Newton schedule."""
     _fields_ = [("sigma_odom_translation", C.c_double), ("sigma_odom_rotation", C.c_double),
@@ -321,6 +333,8 @@ EXPORTS = [
     "tloam_b200_occupancy_download", "tloam_b200_occupancy_scans_download",
     "tloam_b200_distance_default_config", "tloam_b200_distance_build", "tloam_b200_distance_build_grid",
     "tloam_b200_distance_download", "tloam_b200_distance_query",
+    "tloam_b200_plan_default_config", "tloam_b200_plan_build", "tloam_b200_plan_download", "tloam_b200_plan_paths",
+    "tloam_b200_plan_path_cells",
 ]
 
 _lib = None
@@ -568,5 +582,12 @@ def load():
     L.tloam_b200_distance_download.argtypes = [vp, C.POINTER(C.c_float), up, C.POINTER(C.c_ubyte), C.POINTER(C.c_byte),
                                                C.c_size_t]
     L.tloam_b200_distance_query.argtypes = [vp, dp, C.c_size_t, dp, dp]
+    L.tloam_b200_plan_default_config.argtypes = [C.POINTER(PlanConfig)]
+    L.tloam_b200_plan_default_config.restype = None
+    L.tloam_b200_plan_build.argtypes = [vp, C.POINTER(PlanConfig), C.c_double, C.c_double, C.POINTER(PlanInfo)]
+    L.tloam_b200_plan_download.argtypes = [vp, C.POINTER(C.c_ulonglong), C.c_size_t]
+    L.tloam_b200_plan_paths.argtypes = [vp, dp, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_int),
+                                        C.POINTER(C.c_ulonglong)]
+    L.tloam_b200_plan_path_cells.argtypes = [vp, C.POINTER(C.c_int), dp, C.c_size_t]
     _lib = L
     return L

@@ -42,6 +42,7 @@
 #include "map_update.h"
 #include "occupancy.h"
 #include "distance.h"
+#include "plan.h"
 
 
 
@@ -251,6 +252,16 @@ struct tloam_b200_handle {
   unsigned long long* d_dist_small = nullptr;                                                  // the obstacle count
   double* d_dist_q = nullptr;              size_t cap_dist_q = 0;                              // points: xy, distance, gradient
   bool dist_built = false;                 tloam_distance_info dist_info;
+  // ---- the plan (tloam_b200_plan*, libtloam_b200_plan.so): the last build's cells (P 8, t 2: 10 B each), the tile
+  //      stamps and the two worklists (12 B per tile), the worklists' state, the last paths' starts and outputs (24 B per
+  //      start) and cells (8 B each); allocated by the first call that needs them, grown only ----
+  unsigned char* d_plan = nullptr;         size_t cap_plan = 0;                                // cells of the buffer
+  unsigned* d_plan_tiles = nullptr;        size_t cap_plan_tiles = 0;                          // stamps, then 2 lists
+  tloam_plan_state* d_plan_state = nullptr;
+  unsigned char* d_plan_q = nullptr;       size_t cap_plan_q = 0;                              // starts of the buffer
+  int* d_plan_cells = nullptr;             size_t cap_plan_cells = 0;                          // path cells of the buffer
+  bool plan_built = false;                 tloam_plan_info plan_info;
+  bool plan_paths_kept = false;            size_t plan_path_total = 0;                         // cells of the last paths
   // ---- the merged map (tloam_b200_global_map_merge*, libtloam_b200_gmm.so): the radix sort's scratch (24 B per map row)
   //      and the last merge's voxels (32 B each), allocated by the first merge and grown; the snapshot is dropped by
   //      enable / reset and by the next merge ----
@@ -564,6 +575,7 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   cudaFree(h->d_gmd_bounds); cudaFree(h->d_gmd_scratch);
   cudaFree(h->d_occ_scans); cudaFree(h->d_occ_poses); cudaFree(h->d_occ_dirs); cudaFree(h->d_occ_grid); cudaFree(h->d_occ_small);
   cudaFree(h->d_dist); cudaFree(h->d_dist_bands); cudaFree(h->d_dist_table); cudaFree(h->d_dist_small); cudaFree(h->d_dist_q);
+  cudaFree(h->d_plan); cudaFree(h->d_plan_tiles); cudaFree(h->d_plan_state); cudaFree(h->d_plan_q); cudaFree(h->d_plan_cells);
   cudaFree(h->d_gmm_scratch); cudaFree(h->d_gmm_out);
   cudaFree(h->d_loc_map); cudaFree(h->d_loc_scratch); cudaFree(h->d_loc_qst); cudaFree(h->d_loc_reg); cudaFree(h->d_loc_fin);
   cudaFree(h->d_loc_q); cudaFree(h->d_loc_in); cudaFree(h->d_loc_run);
@@ -5630,6 +5642,251 @@ int tloam_b200_distance_query(tloam_b200_handle* h, const double* xy, size_t n, 
     if (gradient) CU_TRY(cudaMemcpyAsync(gradient, a.gradient, n * 2 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   }
   CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Path planning (the checks, the host loop over rounds and the buffers here; the kernels in plan.cu, loaded from
+// libtloam_b200_plan.so by the first plan call, so that the kernels of this library keep their SASS).
+// ---------------------------------------------------------------------------------------------
+struct PlanLib {
+  tloam_plan_init_fn init = nullptr; tloam_plan_rounds_fn rounds = nullptr; tloam_plan_count_fn count = nullptr;
+  tloam_plan_path_fn length = nullptr; tloam_plan_path_fn walk = nullptr;
+};
+static std::mutex g_plan_mu;
+static PlanLib g_plan;
+
+static int plan_load(tloam_b200_handle* h, PlanLib* out) {
+  std::lock_guard<std::mutex> lk(g_plan_mu);
+  if (!g_plan.init) {
+    const std::string path = sibling_path("libtloam_b200_plan.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    PlanLib l;
+    if (so) {
+      l.init = reinterpret_cast<tloam_plan_init_fn>(dlsym(so, "tloam_plan_init"));
+      l.rounds = reinterpret_cast<tloam_plan_rounds_fn>(dlsym(so, "tloam_plan_rounds"));
+      l.count = reinterpret_cast<tloam_plan_count_fn>(dlsym(so, "tloam_plan_count"));
+      l.length = reinterpret_cast<tloam_plan_path_fn>(dlsym(so, "tloam_plan_length"));
+      l.walk = reinterpret_cast<tloam_plan_path_fn>(dlsym(so, "tloam_plan_walk"));
+    }
+    if (!l.init || !l.rounds || !l.count || !l.length || !l.walk) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "path planning: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_plan = l;
+  }
+  *out = g_plan;
+  return TLOAM_B200_OK;
+}
+
+static int plan_status(tloam_b200_handle* h, int e, const char* where) {
+  if (e == cudaSuccess) return TLOAM_B200_OK;
+  snprintf(h->last_error, sizeof(h->last_error), "path planning: %s: %s", where, cudaGetErrorString((cudaError_t)e));
+  return TLOAM_B200_ERR_CUDA;
+}
+
+void tloam_b200_plan_default_config(tloam_plan_config* c) {
+  c->neutral_cost = 50;                    // global_planner's defaults
+  c->cost_factor = 3;
+  c->allow_unknown = 1;
+}
+
+static bool plan_config_valid(const tloam_plan_config* c) {
+  return c->neutral_cost >= 1 && (unsigned long long)c->neutral_cost + 252ull * c->cost_factor <= 65535ull &&
+         (c->allow_unknown == 0 || c->allow_unknown == 1);
+}
+
+// the cell of (x, y) in the last distance field: (floor((x - origin_x) / resolution), likewise for y); false when x or y
+// is not finite or the cell lies outside the grid
+static bool plan_cell(const tloam_distance_info& f, double x, double y, long long* i, long long* j) {
+  if (!std::isfinite(x) || !std::isfinite(y)) return false;
+  const double u = std::floor((x - f.origin_x) / f.resolution), v = std::floor((y - f.origin_y) / f.resolution);
+  if (!(u >= 0.0 && u < (double)f.width && v >= 0.0 && v < (double)f.height)) return false;
+  *i = (long long)u; *j = (long long)v;
+  return true;
+}
+
+int tloam_b200_plan_build(tloam_b200_handle* h, const tloam_plan_config* cfg, double goal_x, double goal_y,
+                          tloam_plan_info* info) {
+  if (!h || !cfg || !plan_config_valid(cfg)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->dist_built) return TLOAM_B200_ERR_NOT_READY;
+  const tloam_distance_info f = h->dist_info;
+  long long gi = 0, gj = 0;
+  if (!plan_cell(f, goal_x, goal_y, &gi, &gj)) return TLOAM_B200_ERR_INVALID_ARG;
+  PlanLib lib;
+  int rc = plan_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  const unsigned char* costs = h->d_dist + 17 * h->cap_dist;
+  const size_t n = f.width * f.height;
+  unsigned char code = 0;
+  CU_TRY(cudaMemcpyAsync(&code, costs + (size_t)gj * f.width + (size_t)gi, 1, cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (!(code <= 252 || (code == 255 && cfg->allow_unknown))) return TLOAM_B200_ERR_INVALID_ARG;   // the goal is impassable
+  h->plan_built = false;
+  h->plan_paths_kept = false;
+  if (n > h->cap_plan) {
+    cudaFree(h->d_plan); h->d_plan = nullptr; h->cap_plan = 0;
+    CU_TRY(cudaMalloc(&h->d_plan, n * 10));
+    h->cap_plan = n;
+  }
+  const size_t ntiles = ((f.width + TLOAM_PLAN_TILE - 1) / TLOAM_PLAN_TILE) * ((f.height + TLOAM_PLAN_TILE - 1) / TLOAM_PLAN_TILE);
+  if (ntiles > h->cap_plan_tiles) {
+    cudaFree(h->d_plan_tiles); h->d_plan_tiles = nullptr; h->cap_plan_tiles = 0;
+    CU_TRY(cudaMalloc(&h->d_plan_tiles, ntiles * 3 * sizeof(unsigned)));
+    h->cap_plan_tiles = ntiles;
+  }
+  if (!h->d_plan_state) CU_TRY(cudaMalloc(&h->d_plan_state, sizeof(tloam_plan_state)));
+  tloam_plan_args a;
+  memset(&a, 0, sizeof(a));
+  a.costs = costs;
+  a.width = (unsigned)f.width; a.height = (unsigned)f.height;
+  a.neutral_cost = cfg->neutral_cost; a.cost_factor = cfg->cost_factor; a.allow_unknown = cfg->allow_unknown;
+  a.goal_i = (unsigned)gi; a.goal_j = (unsigned)gj;
+  a.P = reinterpret_cast<unsigned long long*>(h->d_plan);
+  a.t = reinterpret_cast<unsigned short*>(h->d_plan + 8 * h->cap_plan);
+  a.stamp = h->d_plan_tiles;
+  a.list = h->d_plan_tiles + ntiles;
+  a.state = h->d_plan_state;
+  a.device = h->device; a.stream = h->stream;
+  int e = 0, launches = 0;
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.init(&a, &launches)));
+  h->launches += launches > 0 ? launches - 1 : 0;
+  if ((rc = plan_status(h, e, "k_plan_init")) != TLOAM_B200_OK) return rc;
+  // rounds in batches; after each, the next round's work count decides whether to go on (an empty round exits at once)
+  const unsigned kBatch = 32;
+  tloam_plan_state st;
+  for (unsigned first = 1;; first += kBatch) {
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.rounds(&a, first, kBatch, &launches)));
+    h->launches += launches > 0 ? launches - 1 : 0;
+    if ((rc = plan_status(h, e, "k_plan_round")) != TLOAM_B200_OK) return rc;
+    CU_TRY(cudaMemcpyAsync(&st, h->d_plan_state, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    if (st.count[(first + kBatch) % 3] == 0) break;
+  }
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.count(&a, &launches)));
+  h->launches += launches > 0 ? launches - 1 : 0;
+  if ((rc = plan_status(h, e, "k_plan_count")) != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaMemcpyAsync(&st, h->d_plan_state, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  tloam_plan_info out;
+  memset(&out, 0, sizeof(out));
+  out.origin_x = f.origin_x; out.origin_y = f.origin_y; out.resolution = f.resolution;
+  out.width = f.width; out.height = f.height;
+  out.goal_i = (size_t)gi; out.goal_j = (size_t)gj;
+  out.reachable = (size_t)st.reachable;
+  out.rounds = st.rounds; out.tiles = st.tiles;
+  h->plan_info = out;
+  h->plan_built = true;
+  if (info) *info = out;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_plan_download(tloam_b200_handle* h, unsigned long long* potential, size_t capacity) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->plan_built) return TLOAM_B200_ERR_NOT_READY;
+  const size_t n = h->plan_info.width * h->plan_info.height;
+  if (capacity < n) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  if (potential) CU_TRY(cudaMemcpyAsync(potential, h->d_plan, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_plan_paths(tloam_b200_handle* h, const double* starts_xy, size_t n, size_t* offsets, int* statuses,
+                          unsigned long long* costs) {
+  if (!h || (n && !starts_xy) || n > (size_t(1) << 24)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->plan_built) return TLOAM_B200_ERR_NOT_READY;
+  PlanLib lib;
+  int rc = plan_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  h->plan_paths_kept = false;
+  const tloam_plan_info& f = h->plan_info;
+  tloam_distance_info g;
+  memset(&g, 0, sizeof(g));
+  g.origin_x = f.origin_x; g.origin_y = f.origin_y; g.resolution = f.resolution; g.width = f.width; g.height = f.height;
+  // per start: the cell (2 int), the status (int), the length (unsigned), the cost and the offset (8 B each)
+  if (n > h->cap_plan_q) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_plan_q); h->d_plan_q = nullptr; h->cap_plan_q = 0;
+    CU_TRY(cudaMalloc(&h->d_plan_q, n * 32));
+    h->cap_plan_q = n;
+  }
+  std::vector<int> start(2 * n);
+  for (size_t s = 0; s < n; ++s) {
+    long long i = -1, j = -1;
+    if (!plan_cell(g, starts_xy[2 * s], starts_xy[2 * s + 1], &i, &j)) i = j = -1;
+    start[2 * s] = (int)i; start[2 * s + 1] = (int)j;
+  }
+  const size_t cap = h->cap_plan_q;
+  tloam_plan_path_args a;
+  memset(&a, 0, sizeof(a));
+  a.P = reinterpret_cast<const unsigned long long*>(h->d_plan);
+  a.t = reinterpret_cast<const unsigned short*>(h->d_plan + 8 * h->cap_plan);
+  a.width = (unsigned)f.width; a.height = (unsigned)f.height;
+  a.n = (unsigned)n;
+  unsigned long long* cost = reinterpret_cast<unsigned long long*>(h->d_plan_q);
+  unsigned long long* offset = cost + cap;
+  int* cell = reinterpret_cast<int*>(offset + cap);
+  a.cost = cost; a.offset = offset; a.start = cell;
+  a.status = cell + 2 * cap;
+  a.length = reinterpret_cast<unsigned*>(cell + 3 * cap);
+  a.device = h->device; a.stream = h->stream;
+  std::vector<int> status(n);
+  std::vector<unsigned long long> cost_h(n);
+  std::vector<unsigned> length(n);
+  std::vector<unsigned long long> offset_h(n + 1, 0);
+  int e = 0, launches = 0;
+  if (n) {
+    CU_TRY(cudaMemcpyAsync(cell, start.data(), 2 * n * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.length(&a, &launches)));
+    h->launches += launches > 0 ? launches - 1 : 0;
+    if ((rc = plan_status(h, e, "k_plan_length")) != TLOAM_B200_OK) return rc;
+    CU_TRY(cudaMemcpyAsync(status.data(), a.status, n * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaMemcpyAsync(cost_h.data(), cost, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaMemcpyAsync(length.data(), a.length, n * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    for (size_t s = 0; s < n; ++s) offset_h[s + 1] = offset_h[s] + length[s];
+    const size_t total = (size_t)offset_h[n];
+    if (total > h->cap_plan_cells) {
+      cudaFree(h->d_plan_cells); h->d_plan_cells = nullptr; h->cap_plan_cells = 0;
+      CU_TRY(cudaMalloc(&h->d_plan_cells, total * 2 * sizeof(int)));
+      h->cap_plan_cells = total;
+    }
+    a.cells = h->d_plan_cells;
+    CU_TRY(cudaMemcpyAsync(offset, offset_h.data(), n * sizeof(unsigned long long), cudaMemcpyHostToDevice, h->stream));
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.walk(&a, &launches)));
+    h->launches += launches > 0 ? launches - 1 : 0;
+    if ((rc = plan_status(h, e, "k_plan_walk")) != TLOAM_B200_OK) return rc;
+    CU_TRY(cudaStreamSynchronize(h->stream));
+  }
+  for (size_t s = 0; s <= n; ++s)
+    if (offsets) offsets[s] = (size_t)offset_h[s];
+  if (statuses) std::copy(status.begin(), status.end(), statuses);
+  if (costs) std::copy(cost_h.begin(), cost_h.end(), costs);
+  h->plan_path_total = (size_t)offset_h[n];
+  h->plan_paths_kept = true;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_plan_path_cells(tloam_b200_handle* h, int* ij, double* xy, size_t capacity) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->plan_paths_kept) return TLOAM_B200_ERR_NOT_READY;
+  const size_t m = h->plan_path_total;
+  if (capacity < m) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  std::vector<int> cells(xy ? 2 * m : 0);
+  int* dst = ij ? ij : cells.data();
+  if (m && (ij || xy)) CU_TRY(cudaMemcpyAsync(dst, h->d_plan_cells, m * 2 * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (xy) {
+    const tloam_plan_info& f = h->plan_info;
+    for (size_t k = 0; k < 2 * m; ++k)        // the centre, each operation rounded on its own
+      xy[k] = (k % 2 ? f.origin_y : f.origin_x) + ((double)dst[k] + 0.5) * f.resolution;
+  }
   return TLOAM_B200_OK;
 }
 

@@ -209,6 +209,32 @@ class DistanceField:
 
 
 @dataclasses.dataclass(frozen=True)
+class PlanField:
+    """a built plan (include/tloam_b200.h "Path planning"): potential (height, width) uint64, the least cost of a path
+    from each cell to the goal (0xFFFFFFFFFFFFFFFF: impassable or cut off), in the grid's layout; origin = (x, y) of the
+    corner of cell (0, 0); goal = its cell (i, j); reachable = the cells with a finite potential; rounds and tiles = the
+    relaxation rounds that had work and the tiles they relaxed."""
+    potential: np.ndarray
+    origin: tuple
+    resolution: float
+    goal: tuple
+    reachable: int
+    rounds: int
+    tiles: int
+
+
+@dataclasses.dataclass(frozen=True)
+class PlanPath:
+    """one start's path down the last plan: cells (m, 2) int32 (i, j) from the start to the goal, xy (m, 2) their centres
+    in m, cost = the start's potential, status 0 reached, 1 start not finite or outside the grid, 2 start impassable, 3
+    goal unreachable (no cells, cost 0xFFFFFFFFFFFFFFFF unless the status is 0)."""
+    cells: np.ndarray
+    xy: np.ndarray
+    cost: int
+    status: int
+
+
+@dataclasses.dataclass(frozen=True)
 class OccupancyGrid:
     """a built occupancy grid (include/tloam_b200.h "Occupancy grid"): cells (height, width) int8 in nav_msgs/OccupancyGrid's
     values (-1 unknown, 0 .. 100), row j along y and column i along x, with the counts it came from (uint32 each); origin
@@ -1499,6 +1525,43 @@ class LocalRegistration:
         d, g = np.zeros(len(p)), np.zeros((len(p), 2))
         self._check(self._L.tloam_b200_distance_query(self._h, _dp(p), len(p), _dp(d), _dp(g)), "distance_query")
         return d, g
+
+    # ---- path planning (include/tloam_b200.h "Path planning") ----
+    def plan_build(self, goal, **overrides):
+        """the potential to the goal (x, y) on the last distance_build's costs; overrides: fields of tloam_plan_config
+        (neutral_cost, cost_factor, allow_unknown).  Returns a PlanField."""
+        cfg = _lib.PlanConfig()
+        self._L.tloam_b200_plan_default_config(C.byref(cfg))
+        for k, v in overrides.items():
+            if not any(f[0] == k for f in cfg._fields_):
+                raise TypeError(f"unknown plan field {k!r}")
+            setattr(cfg, k, v)
+        info = _lib.PlanInfo()
+        self._check(self._L.tloam_b200_plan_build(self._h, C.byref(cfg), float(goal[0]), float(goal[1]), C.byref(info)),
+                    "plan_build")
+        P = np.zeros((info.height, info.width), dtype=np.uint64)
+        self._check(self._L.tloam_b200_plan_download(self._h, P.ctypes.data_as(C.POINTER(C.c_ulonglong)), P.size),
+                    "plan_download")
+        return PlanField(P, (info.origin_x, info.origin_y), info.resolution, (info.goal_i, info.goal_j), info.reachable,
+                         info.rounds, info.tiles)
+
+    def plan_paths(self, starts):
+        """one PlanPath per start (n, 2) of xy, down the last plan_build"""
+        p = np.ascontiguousarray(starts, dtype=np.float64).reshape(-1, 2)
+        n = len(p)
+        offsets = np.zeros(n + 1, dtype=np.uintp)
+        statuses = np.zeros(n, dtype=np.int32)
+        costs = np.zeros(n, dtype=np.uint64)
+        self._check(self._L.tloam_b200_plan_paths(
+            self._h, _dp(p), n, offsets.ctypes.data_as(C.POINTER(C.c_size_t)), statuses.ctypes.data_as(C.POINTER(C.c_int)),
+            costs.ctypes.data_as(C.POINTER(C.c_ulonglong))), "plan_paths")
+        m = int(offsets[-1])
+        ij = np.zeros((m, 2), dtype=np.int32)
+        xy = np.zeros((m, 2))
+        self._check(self._L.tloam_b200_plan_path_cells(self._h, ij.ctypes.data_as(C.POINTER(C.c_int)), _dp(xy), m),
+                    "plan_path_cells")
+        return [PlanPath(ij[offsets[s]:offsets[s + 1]], xy[offsets[s]:offsets[s + 1]], int(costs[s]), int(statuses[s]))
+                for s in range(n)]
 
     def localize_set_map_updated(self):
         """load the last map_update_build on the device as the prior map"""
