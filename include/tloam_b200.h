@@ -58,8 +58,10 @@ typedef enum tloam_b200_status {
   TLOAM_B200_ERR_NOT_READY = 6,      /* scan_match before set_source / set_target */
   TLOAM_B200_ERR_NUMERIC = 7,        /* non-finite value met inside the solve */
   TLOAM_B200_ERR_MAP_DENSITY = 8,    /* a map cell (edge = search radius) holds more than 65535 points */
-  TLOAM_B200_ERR_VOXEL_RANGE = 9     /* a global-map frame, or the map being merged, spans 2^21 or more voxels on an axis
-                                        (voxel too small): the frame is not appended, the merge produces nothing */
+  TLOAM_B200_ERR_VOXEL_RANGE = 9     /* a cloud to be voxel-down-sampled spans 2^21 or more voxels on an axis (voxel too
+                                        small), or a host cloud's finite rows n and voxel reach n * voxel >= 2^23 m (the
+                                        headroom of the fixed-point sums; conservative): a global-map frame is not
+                                        appended, the merge produces nothing, a host-input call launches nothing */
 } tloam_b200_status;
 
 /* The "TLS:" YAML block (ref: config/mapping/lidar_odometry.yaml:23-39, read at registration.cpp:212-230)
@@ -278,7 +280,11 @@ typedef struct tloam_submap_config {   /* ref: config/mapping/lidar_odometry.yam
 } tloam_submap_config;
 void tloam_b200_submap_default_config(tloam_submap_config* c);
 /* First frame: edge = raw edge cloud, ground_raw = raw ground cloud (voxel-down-sampled at ground_down_sample
- * inside), planar_sub / sphere_sub = the "submap index" selections of the general cloud.  HOST pointers. */
+ * inside), planar_sub / sphere_sub = the "submap index" selections of the general cloud.  HOST pointers.
+ * INVALID_ARG: a crop length and submap voxel with 2 L / voxel + 1 >= 2^21 (a cropped cloud could then reach the key
+ * range, which bounds every later update), or a submap voxel not > 0.  VOXEL_RANGE: ground_raw as in
+ * tloam_b200_voxel_down_sample (nothing is changed).  A later update's per-voxel count is not checked against the
+ * 2^23 m headroom: an accumulator would need 2^23 m / voxel rows in one voxel. */
 int tloam_b200_submap_init(tloam_b200_handle* h, const tloam_submap_config* cfg, const double* edge, size_t ne,
                            const double* ground_raw, size_t ng, const double* planar_sub, size_t np,
                            const double* sphere_sub, size_t ns);
@@ -294,7 +300,10 @@ int tloam_b200_submap_update_chained(tloam_b200_handle* h, const double* planar_
 int tloam_b200_submap_sizes(tloam_b200_handle* h, size_t n[4]);   /* exact sizes (synchronises) */
 /* copies map cloud `cloud` (0 edge, 1 sphere, 2 planar, 3 ground; world frame, FP64 AoS) to the host */
 int tloam_b200_submap_download(tloam_b200_handle* h, int cloud, double* out, size_t capacity_points);
-/* PointCloud2::VoxelDownSample on the device (HOST in / out; out must hold n points). */
+/* PointCloud2::VoxelDownSample on the device (HOST in / out; out must hold n points).  Rows with a non-finite coordinate
+ * are left out (they do not move the min bound).  Each average is within 2^-41 + 2^-51 voxel + 1.5 ulp(max |p|) of the
+ * exact mean of its voxel's rows, and bit-reproducible.  INVALID_ARG: voxel not > 0 with n > 0.  VOXEL_RANGE (checked on
+ * the host, nothing launched): the finite rows span 2^21 voxels on an axis, or their count n reaches n * voxel >= 2^23 m. */
 int tloam_b200_voxel_down_sample(tloam_b200_handle* h, const double* pts, size_t n, double voxel, double* out, size_t* n_out);
 
 /* ------------------------------------------------------------------------------------------------
@@ -447,7 +456,9 @@ int tloam_b200_segment_raw_scan_packed(tloam_b200_handle* h, const tloam_ground_
  * planar, ground).
  *   - The down-sampled ground / edge features come out in ascending voxel index (ix, iy, iz) -- the registration caps
  *     (*_maxnum) take features in index order, so the order is part of the result -- with the averages in the fixed-point
- *     form of tloam_b200_voxel_down_sample (within 1e-12 m of an FP64 running sum, bit-reproducible).
+ *     form of tloam_b200_voxel_down_sample (within 2^-41 + 2^-51 voxel + 1.5 ulp(max |p|) of the exact mean, bit-reproducible).
+ *   - VOXEL_RANGE: the ground or the edge cloud fails tloam_b200_voxel_down_sample's limits at its voxel (checked on the
+ *     host before anything is uploaded; the last processed frame is kept).
  *   - The sphere feature is general[0 .. n_sphere_scan): the reference's sphere lists hold ranks, not point indices
  *     (feature_extract.cpp:183-188; see tloam_b200_extract_planar_sphere), and SelectByIndex takes them literally.
  *   - The frame's raw edge and ground clouds, its planar-submap selection general[planar_submap_index] and its sphere-submap
@@ -462,7 +473,9 @@ int tloam_b200_process_cloud(tloam_b200_handle* h, const tloam_feature_config* f
                              size_t n_source[4]);
 /* tloam_b200_segment_raw_scan followed by tloam_b200_process_cloud without the host in between: the raw scan (HOST, may hold
  * NaN / Inf rows) is uploaded once, segmented on the device, the ground / edge / general clouds are gathered from it on the
- * device, then processed as above.  An all-NaN or all-near scan gives four empty sources and OK. */
+ * device, then processed as above.  An all-NaN or all-near scan gives four empty sources and OK.  VOXEL_RANGE: the scan's
+ * finite rows fail tloam_b200_voxel_down_sample's limits at ground_down_sample or edge_down_sample (the ground and edge
+ * clouds are subsets of them), checked on the host before the upload. */
 int tloam_b200_process_raw_scan(tloam_b200_handle* h, const tloam_ground_config* gcfg, const tloam_dcvc_config* dcfg, int ring_min_num,
                                 double near_dis, const tloam_feature_config* fcfg, double ground_down_sample, double edge_down_sample,
                                 const double* xyz, size_t n, size_t n_source[4]);
@@ -486,6 +499,8 @@ int tloam_b200_process_raw_scan_packed(tloam_b200_handle* h, const tloam_ground_
  *     corrected) and as the raw scan tloam_b200_global_map_append_frame* and tloam_b200_registered_scan_download read.
  *   - The kernels live in libtloam_b200_deskew.so, loaded from this library's directory on the first timed call; if it is
  *     missing these calls return ERR_CUDA (tloam_b200_last_error names the file).
+ *   - The key-range and headroom check (VOXEL_RANGE) reads the scan before the correction; the corrected rows' extent is
+ *     not checked, and tloam_b200_submap_init_frame after a timed call does not check its ground cloud either.
  *   - INVALID_ARG, besides the untimed call's: time null with n > 0, frame_period not finite or not > 0, and for a packed
  *     time field: offset < 0 or offset + size > point_step, a datatype other than 6 / 7 / 8, unit not finite or not > 0. */
 /* a time field of a tloam_packed_scan record: a record's time is the field's value times unit */
@@ -509,7 +524,8 @@ int tloam_b200_process_raw_scan_packed_timed(tloam_b200_handle* h, const tloam_g
 int tloam_b200_source_download(tloam_b200_handle* h, int cloud, double* out, size_t capacity_points);
 /* tloam_b200_submap_init from the last processed frame (front_end.cpp:285-305): edge = its raw edge cloud, ground =
  * VoxelDownSample(cfg->ground_down_sample) of its raw ground cloud, planar = general[planar_submap_index], sphere =
- * general[0 .. n_sphere_submap).  NOT_READY before any processed frame. */
+ * general[0 .. n_sphere_submap).  NOT_READY before any processed frame.  INVALID_ARG / VOXEL_RANGE as in
+ * tloam_b200_submap_init, the ground cloud's extent being the one the processing call read on the host. */
 int tloam_b200_submap_init_frame(tloam_b200_handle* h, const tloam_submap_config* cfg);
 /* tloam_b200_submap_update / _chained with planar_sub = the last processed frame's planar-submap selection, read on the
  * device.  NOT_READY before any processed frame. */

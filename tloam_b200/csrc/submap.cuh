@@ -10,9 +10,9 @@
 // PCIe, instead of the whole 12 MB map (set_target).
 //
 // VoxelDownSample on the device: voxel index = floor((p - (min_bound - voxel/2)) / voxel) like the reference;
-// the per-voxel average is accumulated in 64-bit FIXED POINT (offsets inside the voxel, 2^-40 m resolution), so
-// the VALUES do not depend on the order of the atomics (bit-reproducible) and differ from the reference's
-// FP64 running sum by < 1e-12 m.  The output ORDER is not reproducible: slots are claimed by CAS and k_vox_emit takes
+// the per-voxel average is accumulated in 64-bit FIXED POINT (offsets inside the voxel, 2^-40 m resolution), so the VALUES
+// do not depend on the order of the atomics (bit-reproducible); each is within 2^-41 + 2^-51 voxel + 1.5 ulp(max |p|) of the
+// voxel's EXACT mean (tests/voxel_edges_oracle.py).  The output ORDER is not reproducible: slots are claimed by CAS and k_vox_emit takes
 // its output base with one atomicAdd per block, so it follows block scheduling (the reference's own order is
 // std::unordered_map iteration order -- implementation-defined).  Downstream, point order only enters the kNN
 // tie-break (d2, original index): it can matter for EXACT distance ties between two averaged voxel centres, nowhere else

@@ -51,6 +51,10 @@
 // =================================================================================================
 using namespace tloam;
 
+// bounds and count of a host cloud's finite rows, the rows the voxel kernels keep (vox_in_box drops a row with a
+// non-finite coordinate); n == 0: none
+struct VoxExtent { double lo[3] = {0, 0, 0}, hi[3] = {0, 0, 0}; size_t n = 0; bool known = true; };
+
 #define CU_TRY(expr)                                                                                   \
   do {                                                                                                 \
     cudaError_t e__ = (expr);                                                                          \
@@ -156,6 +160,7 @@ struct tloam_b200_handle {
   double* d_frame = nullptr;               size_t cap_frame = 0;
   size_t fr_ng = 0, fr_ne = 0, fr_nn = 0, fr_np_sub = 0, fr_ns_sub = 0;
   bool have_frame = false;
+  VoxExtent fr_ground_ext;                 // a bound of the raw ground cloud's extent (submap_init_frame's key range check)
   // pipelined results (async_inputs): two pinned result slots + events, so that the host can stay one frame ahead
   cudaEvent_t ev_res[2] = {nullptr, nullptr};
   long long frames_enqueued = 0, frames_fetched = 0;
@@ -421,7 +426,7 @@ const char* tloam_b200_status_string(int s) {
     case TLOAM_B200_ERR_NOT_READY: return "source or target not set";
     case TLOAM_B200_ERR_NUMERIC: return "non-finite value in the solve";
     case TLOAM_B200_ERR_MAP_DENSITY: return "a map cell holds more than 65535 points";
-    case TLOAM_B200_ERR_VOXEL_RANGE: return "a global-map frame spans 2^21 or more voxels on an axis (voxel size too small)";
+    case TLOAM_B200_ERR_VOXEL_RANGE: return "a cloud spans 2^21 or more voxels on an axis (voxel size too small), or n * voxel >= 2^23 m";
     default: return "unknown status";
   }
 }
@@ -2021,6 +2026,50 @@ static int ensure_dev(tloam_b200_handle* h, double** p, size_t* cap, size_t need
   return TLOAM_B200_OK;
 }
 
+// ---- limits of the voxel kernels, checked on the host for clouds that come from the host (nothing is launched when a
+//      cloud fails them: the caller returns VOXEL_RANGE) ----
+//   key range: k_vox_accum packs each axis's index into kGMapKeyBits bits (cell_key), so an index of 2^21 or more would
+//     land in the voxel of index mod 2^21 and vox_average would write its mean there.  k_gmap_guard's expression on the
+//     finite rows' bounds gives the largest index exactly: floor((p - min_bound) / voxel) is monotone in p.
+//   headroom: each row adds llrint(offset * 2^40) to a signed 64-bit sum, with offset = p - (voxel's base) at most the
+//     voxel plus rounding: below 2^-52 (3 |p| + 4 voxel) for a keyable index, padded here to 2^-49 (|p| + voxel), plus the
+//     half unit of llrint.  n rows times that stays below 2^63 / 2^40 = 2^23 m whatever voxel they share.
+static void vox_extent_add(VoxExtent& e, double x, double y, double z) {
+  if (!std::isfinite(x) || !std::isfinite(y) || !std::isfinite(z)) return;
+  const double p[3] = {x, y, z};
+  for (int d = 0; d < 3; ++d) {
+    e.lo[d] = e.n ? std::fmin(e.lo[d], p[d]) : p[d];
+    e.hi[d] = e.n ? std::fmax(e.hi[d], p[d]) : p[d];
+  }
+  ++e.n;
+}
+static VoxExtent vox_extent(const double* p, size_t n) {
+  VoxExtent e;
+  for (size_t i = 0; i < n; ++i) vox_extent_add(e, p[3 * i], p[3 * i + 1], p[3 * i + 2]);
+  return e;
+}
+static VoxExtent vox_extent_packed(const tloam_packed_scan* s) {   // the FLOAT32 fields, as unpack_packed widens them
+  VoxExtent e;
+  const unsigned char* r = static_cast<const unsigned char*>(s->data);
+  for (size_t i = 0; i < s->n; ++i, r += s->point_step) {
+    float f[3];
+    memcpy(&f[0], r + s->x_offset, 4); memcpy(&f[1], r + s->y_offset, 4); memcpy(&f[2], r + s->z_offset, 4);
+    vox_extent_add(e, f[0], f[1], f[2]);
+  }
+  return e;
+}
+static bool vox_fits(const VoxExtent& e, double voxel) {
+  if (!e.known || e.n == 0) return true;
+  double big = 0.0;
+  for (int d = 0; d < 3; ++d) {
+    const double mb = e.lo[d] - voxel * 0.5;
+    const double ref = (e.hi[d] - mb) / voxel;
+    if (!(ref < (double)(1u << kGMapKeyBits))) return false;
+    big = std::fmax(big, std::fmax(std::fabs(e.lo[d]), std::fabs(e.hi[d])));
+  }
+  return (double)e.n * (voxel + 0x1p-49 * (big + voxel) + 0x1p-40) < 0x1p23;
+}
+
 // crop + VoxelDownSample of d_in into d_out, enqueued without any host round trip: the voxel count lands in
 // *out_count (device).  The input holds n_bound points at most; its exact count is n_bound itself (n_dev == nullptr)
 // or *n_dev + n_add.  The crop box is lo/hi (host values; nullptr = none) or pose.t +- box_len with the pose in
@@ -2305,6 +2354,9 @@ int tloam_b200_pca_info(tloam_b200_handle* h, const tloam_feature_config* cfg, c
 
 int tloam_b200_voxel_down_sample(tloam_b200_handle* h, const double* pts, size_t n, double voxel, double* out, size_t* n_out) {
   if (!h || (!pts && n) || !out || !n_out) return TLOAM_B200_ERR_INVALID_ARG;
+  *n_out = 0;
+  if (n && !(voxel > 0.0)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!vox_fits(vox_extent(pts, n), voxel)) return TLOAM_B200_ERR_VOXEL_RANGE;
   CU_TRY(cudaSetDevice(h->device));
   int rc = upload_points(h, pts, n);
   if (rc != TLOAM_B200_OK) return rc;
@@ -2328,6 +2380,14 @@ static int submap_init_impl(tloam_b200_handle* h, const tloam_submap_config* cfg
                             const double* sphere_sub, size_t ns, bool on_device) {
   if (!h || !cfg || (!edge && ne) || (!ground_raw && ng) || (!planar_sub && np) || (!sphere_sub && ns)) return TLOAM_B200_ERR_INVALID_ARG;
   if (cfg->planar_frame_size < 1 || cfg->planar_frame_size > 64) return TLOAM_B200_ERR_INVALID_ARG;
+  // every submap_update crops to pose.t +- L before its voxel pass, so 2 L / voxel + 1 < 2^21 keeps each cropped cloud's
+  // indices keyable (the extra voxel covers the min bound's half-voxel margin and the rounding of the box)
+  const double crop_len[2] = {cfg->edge_crop_box_length, cfg->ground_crop_box_length};
+  const double crop_vox[2] = {cfg->edge_down_sample_submap, cfg->ground_down_sample_submap};
+  for (int k = 0; k < 2; ++k)
+    if (!(crop_vox[k] > 0.0) || !(2.0 * crop_len[k] / crop_vox[k] + 1.0 < (double)(1u << kGMapKeyBits))) return TLOAM_B200_ERR_INVALID_ARG;
+  if (ng && !(cfg->ground_down_sample > 0.0)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!vox_fits(on_device ? h->fr_ground_ext : vox_extent(ground_raw, ng), cfg->ground_down_sample)) return TLOAM_B200_ERR_VOXEL_RANGE;
   CU_TRY(cudaSetDevice(h->device));
   h->scfg = *cfg;
   if (!h->d_pose) CU_TRY(cudaMalloc(&h->d_pose, 16 * sizeof(double)));
@@ -3318,8 +3378,11 @@ int tloam_b200_process_cloud(tloam_b200_handle* h, const tloam_feature_config* f
   for (int k = 0; k < 4; ++k) n_source[k] = 0;
   if (!(ground_down_sample > 0.0) || !(edge_down_sample > 0.0)) return TLOAM_B200_ERR_INVALID_ARG;
   if (ng > ((size_t)1 << 30) || ne > ((size_t)1 << 30) || nn > ((size_t)1 << 30)) return TLOAM_B200_ERR_INVALID_ARG;
+  const VoxExtent ground_ext = vox_extent(ground, ng);
+  if (!vox_fits(ground_ext, ground_down_sample) || !vox_fits(vox_extent(edge, ne), edge_down_sample)) return TLOAM_B200_ERR_VOXEL_RANGE;
   CU_TRY(cudaSetDevice(h->device));
   h->have_frame = false;
+  h->fr_ground_ext = ground_ext;
   int rc = reserve_frame(h, ng, ne, nn);
   if (rc != TLOAM_B200_OK) return rc;
   const double* src[3] = {ground, edge, general};
@@ -3348,8 +3411,15 @@ static int process_raw(tloam_b200_handle* h, const tloam_ground_config* gcfg, co
     if (in.packed ? (in.ptime ? !packed_time_valid(in.ptime, in.packed->point_step) : in.n > 0) : (!in.time && in.n))
       return TLOAM_B200_ERR_INVALID_ARG;
   }
+  // the ground and edge clouds are subsets of the scan's finite rows, so the scan's extent bounds theirs; a timed call
+  // moves rows on the device after this check (not covered: see Deskewing in the header)
+  if (in.packed && !packed_valid(in.packed)) return TLOAM_B200_ERR_INVALID_ARG;
+  VoxExtent scan_ext = in.packed ? vox_extent_packed(in.packed) : vox_extent(in.xyz, in.n);
+  if (!vox_fits(scan_ext, ground_down_sample) || !vox_fits(scan_ext, edge_down_sample)) return TLOAM_B200_ERR_VOXEL_RANGE;
+  scan_ext.known = !in.timed;
   CU_TRY(cudaSetDevice(h->device));
   h->have_frame = false;
+  h->fr_ground_ext = scan_ext;
   size_t unused[1];                                       // the index lists stay on the device (ChainKeep)
   size_t ng = 0, ne = 0, nn = 0;
   int n_clusters = 0;
