@@ -1630,6 +1630,118 @@ int tloam_b200_plan_paths(tloam_b200_handle* h, const double* starts_xy, size_t 
  * INVALID_ARG: capacity < offsets[n] of that call. */
 int tloam_b200_plan_path_cells(tloam_b200_handle* h, int* ij, double* xy, size_t capacity);
 
+/* ---- Global registration (opt-in): two clouds aligned with no initial guess, by FPFH features (Rusu 2009, as PCL and
+ * Open3D define them), mutual matches, a RANSAC search and a truncated-least-squares refinement.  The result is meant as
+ * the guess of tloam_b200_loop_verify* and tloam_b200_localize*.  Every device operation is FP64 and separately rounded
+ * (no FMA, no transcendental function), so tests/global_registration_oracle.py reproduces every bit.  "Sum in order" below
+ * means a running sum s = s + x_k, k ascending.
+ *   - Keypoints.  A host cloud: its finite rows down-sampled as tloam_b200_localize's query is (VoxelDownSample(voxel) by
+ *     the global map's ordered path at pose I), in buffers of this feature.  A loop keyframe: as stored.  Each cloud is in
+ *     its sensor's frame: the viewpoint is the origin.
+ *   - Index and normals.  Each side is indexed and given normals exactly as a prior map of "Localization in a prior map"
+ *     is (grid of `cell`, normal_radius, min_normal_neighbours), with max_planarity = 1: every normal with enough
+ *     neighbours is valid.  Then n <- -n when n . p > 0 (n . p = (nx px + ny py) + nz pz; 0 keeps the sign).
+ *   - Neighbours.  Row i's neighbours are the rows v != i with a valid normal and 0 < d2 <= r^2 (d2 as the index's), in
+ *     ascending sorted position of the index (cell key, then row): the walk over the cells from p - r(1 + 1e-7) to
+ *     p + r(1 + 1e-7), r = feature_radius.
+ *   - Pair (p1, n1) -> (p2, n2), d = p2 - p1.  When |n1 . d| < |n2 . d| the roles swap (p1 <-> p2, n1 <-> n2, d <- -d).
+ *     u = n1; v = (d x u) / |d x u| per component (no pair when |d x u| = 0); w = u x v; a x b = (a1 b2 - a2 b1, ...);
+ *     |x| = sqrt(x . x).  theta = atan2(w . n2, u . n2), alpha = v . n2, phi = (u . d) / sqrt(d2).
+ *     Bins: theta's bin is the number of k in 1 .. 10 with theta >= beta_k = (2k / 11 - 1) pi, decided without atan2 from
+ *     (x, y) = (u . n2, w . n2) and the host's (c_k, s_k) = (cos beta_k, sin beta_k): s = (c_k y - s_k x >= 0); for k <= 5
+ *     the test is y >= 0 or s, for k >= 6 it is (y > 0 or (y == 0 and x < 0)) and s.  alpha and phi: floor(11 ((f + 1)
+ *     0.5)) clamped to [0, 10].  Bins 0 .. 10 are theta's, 11 .. 21 alpha's, 22 .. 32 phi's.
+ *   - SPFH.  Integer counts per bin over row i's pairs (i as p1), with a valid normal at i; pairs(i) = the pairs counted.
+ *     SPFH_k(j) = (count * 100) / pairs(k).
+ *   - FPFH.  A row with pairs(i) > 0 has a feature: over its neighbours k with pairs(k) > 0, in order, val = SPFH_k(j) / d2
+ *     is summed in order into acc(j) and into sum(block of j) (11 bins per block, k then j ascending); then F(j) =
+ *     (acc(j) * 100) / sum + SPFH_i(j), or acc(j) + SPFH_i(j) when that sum is 0.  A row without pairs has no feature.
+ *   - Matches.  Each source feature's nearest target feature by sum over j in order of (a_j - b_j)^2, the lower row on a
+ *     tie; the same from the target.  The mutual pairs (i, j) are kept in source order.  Fewer than 3: termination
+ *     FEW_CORRESPONDENCES, T = I.
+ *   - Hypotheses h = 0 .. n_hypotheses - 1, all evaluated.  With splitmix64(x) (Steele et al. 2014; z = x + 0x9e37..7c15,
+ *     ...), r_d = splitmix64(seed ^ splitmix64((h << 2) | d)) (64-bit wrap): i0 = r_0 % n, i1 = r_1 % (n - 1) + (1 when
+ *     >= i0), i2 = r_2 % (n - 2), then +1 when >= min(i0, i1), then +1 when >= max(i0, i1): three distinct pairs.  Rejected
+ *     unless every edge passes Open3D's length check (ds >= dt * edge_similarity and dt >= ds * edge_similarity, d =
+ *     sqrt(d2)) and both triangles' |(x1 - x0) x (x2 - x0)| >= min_triangle_area.  T_h: the frames e1 = a / |a|, b = u -
+ *     (u . e1) e1, e2 = b / |b|, e3 = e1 x e2 (a = x1 - x0, u = x2 - x0) of the source (E) and target (F) triangles;
+ *     R(r, c) = (F1r E1c + F2r E2c) + F3r E3c; t = c_q - R c_p with c = ((x0 + x1) + x2) / 3.  A hypothesis's inliers: the
+ *     pairs with |R p + t - q|^2 < tau^2, R p + t = ((R_r0 px + R_r1 py) + R_r2 pz) + t_r.  The best has the most inliers,
+ *     the lower h on a tie; none valid: NO_HYPOTHESIS, T = I.
+ *   - Refinement by truncated least squares: S = the best's inliers; while fewer than max_refine_iterations fits were made
+ *     and |S| >= 3 (else FEW_INLIERS): T = fit(S), S' = inliers under T, and CONVERGED when S' = S; S = S'.  ITERATION_LIMIT
+ *     after max_refine_iterations fits.  Each step does not increase sum min(r^2, tau^2).  fit(S): Horn's method with
+ *     every sum in pair order: c_p = sum p / |S|, c_q likewise, S_ab = sum (p_a - c_pa)(q_b - c_qb); N = [[xx+yy+zz,
+ *     yz-zy, zx-xz, xy-yx], [., xx-yy-zz, xy+yx, zx+xz], [., ., yy-xx-zz, yz+zy], [., ., ., zz-xx-yy]] (left to right);
+ *     nf_jacobi3's cyclic Jacobi on 4 x 4 (pairs (0,1) .. (2,3)); q = the eigenvector of the largest eigenvalue (the lower
+ *     index on a tie) over sqrt(((q0^2 + q1^2) + q2^2) + q3^2); R from q = (w, x, y, z) as ((ww + xx) - yy) - zz, 2 (xy -
+ *     wz), ...; t = c_q - R c_p.
+ *   - Result.  inliers = |S| under the final T, inlier_rmse = sqrt(sum r^2 in order / inliers) (0 without inliers);
+ *     fitness = the fraction of source keypoints with a target keypoint at d2 < tau^2 under T (the target's grid);
+ *     accepted = inliers >= min_inliers and fitness >= min_fitness.  A side without keypoints: EMPTY, T = I, and no
+ *     k_gr_* kernel runs (the other side has already been down-sampled and indexed; tloam_b200_global_registration_side
+ *     then gives its keypoints, validity and unoriented normals, and zero counts and features).
+ *   - The kernels live in libtloam_b200_greg.so, loaded from this library's directory by the enable call.  A call changes
+ *     nothing else: odometry, maps, loop database and keyframes, pose graph and localization are untouched. */
+typedef struct tloam_global_registration_config {
+  double voxel;                        /* keypoint down-sample of a host cloud, m */
+  double cell;                         /* index cell, m */
+  double normal_radius;                /* m, <= 3 cell */
+  int min_normal_neighbours;           /* >= 3 */
+  double feature_radius;               /* m, <= 3 cell */
+  double max_correspondence_distance;  /* tau, m */
+  int n_hypotheses;                    /* 1 .. 2^20 */
+  unsigned long long seed;
+  double edge_similarity;              /* (0, 1] */
+  double min_triangle_area;            /* |cross product|, m^2, > 0 */
+  int max_refine_iterations;           /* 1 .. 100 */
+  int min_inliers;                     /* >= 0 */
+  double min_fitness;                  /* [0, 1] */
+} tloam_global_registration_config;
+enum {
+  TLOAM_GLOBAL_REGISTRATION_CONVERGED = 0,
+  TLOAM_GLOBAL_REGISTRATION_ITERATION_LIMIT = 1,
+  TLOAM_GLOBAL_REGISTRATION_FEW_INLIERS = 2,          /* fewer than 3 inliers to fit */
+  TLOAM_GLOBAL_REGISTRATION_FEW_CORRESPONDENCES = 3,  /* fewer than 3 mutual pairs */
+  TLOAM_GLOBAL_REGISTRATION_NO_HYPOTHESIS = 4,        /* every hypothesis rejected */
+  TLOAM_GLOBAL_REGISTRATION_EMPTY = 5                 /* a side without keypoints */
+};
+typedef struct tloam_global_registration_result {
+  double T[16];                        /* target <- source, column-major (the loop call: T_cand_query) */
+  long long n_source_points, n_target_points;        /* keypoints */
+  long long n_source_features, n_target_features;
+  long long n_correspondences;         /* mutual pairs */
+  int n_valid_hypotheses, best_hypothesis, best_inliers;   /* best_hypothesis -1: none */
+  int inliers;
+  double inlier_rmse, fitness;
+  int refine_iterations, termination, accepted;
+} tloam_global_registration_result;
+/* voxel 0.5 m, cell 1 m, normal_radius 1 m, min_normal_neighbours 5, feature_radius 2.5 m, tau 0.75 m, n_hypotheses
+ * 65536, seed 0, edge_similarity 0.9, min_triangle_area 1 m^2, max_refine_iterations 10, min_inliers 30, min_fitness 0.3
+ * (DESIGN.md section 4c has how they were chosen) */
+void tloam_b200_global_registration_default_config(tloam_global_registration_config* c);
+/* turns the feature on (loading libtloam_b200_greg.so and libtloam_b200_loc.so) and drops the last run.  INVALID_ARG: cfg
+ * null or a value outside the ranges above. */
+int tloam_b200_global_registration_enable(tloam_b200_handle* h, const tloam_global_registration_config* cfg);
+/* aligns host cloud src (n_src x 3) to host cloud tgt (n_tgt x 3); synchronises.  NOT_READY: off.  INVALID_ARG: out null,
+ * a null cloud with rows, or more than 2^30 rows.  VOXEL_RANGE: a cloud the down-sample's key or the index cannot hold. */
+int tloam_b200_global_register(tloam_b200_handle* h, const double* src, size_t n_src, const double* tgt, size_t n_tgt,
+                               tloam_global_registration_result* out);
+/* aligns loop keyframe query to loop keyframe candidate (T = T_cand_query, a guess for tloam_b200_loop_verify*);
+ * synchronises.  NOT_READY: this feature or loop verification off.  INVALID_ARG: an index out of range. */
+int tloam_b200_global_register_loop(tloam_b200_handle* h, long long query, long long candidate,
+                                    tloam_global_registration_result* out);
+/* the last run's side (0 source, 1 target): keypoints (n x 3), oriented normals (n x 3; unoriented after an EMPTY run),
+ * normal validity (n), SPFH counts
+ * (n x 33), features (n x 33) and feature flags (n); each may be null; *n = the side's keypoints; synchronises.
+ * NOT_READY: no run since enable.  INVALID_ARG: side not 0 or 1, capacity < *n. */
+int tloam_b200_global_registration_side(tloam_b200_handle* h, int side, double* xyz, double* normal, unsigned char* valid,
+                                        int* spfh, double* feature, unsigned char* has_feature, size_t capacity, size_t* n);
+/* the last run's mutual pairs (source row, target row) in source order (n x 2, may be null); *n = their count. */
+int tloam_b200_global_registration_correspondences(tloam_b200_handle* h, int* pairs, size_t capacity, size_t* n);
+/* the last run's inliers per hypothesis (-1: rejected; may be null); *n = n_hypotheses, or 0 after an EMPTY run. */
+int tloam_b200_global_registration_hypotheses(tloam_b200_handle* h, int* inliers, size_t capacity, size_t* n);
+
 /* Pinned host memory helpers (optional; pinned inputs make set_* a direct DMA, no staging threads). */
 int tloam_b200_host_alloc(void** p, size_t bytes);
 int tloam_b200_host_free(void* p);

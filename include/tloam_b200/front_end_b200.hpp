@@ -23,6 +23,8 @@
 // enableMapUpdate / addMapUpdateFrame / buildUpdatedMap keep that map up to date from the localized frames.
 // enableOccupancy / occupancyGrid give a 2D occupancy grid of the map; distanceField / queryDistance its distance field
 // and inflated costmap, or those of a saved grid; planPotential / planPaths plan paths on that costmap.
+// enableGlobalRegistration / globalRegister / globalRegisterLoop align two clouds, or two loop keyframes, with no initial
+// guess: the guess for verifyLoop's ICP or for localizeFrame.
 // Without the reference headers (this repository's tests) define TLOAM_B200_MOCK_HOST_TYPES and provide the host types
 // (tests/mock/mock_tloam.hpp).
 #ifndef TLOAM_B200_FRONT_END_B200_HPP
@@ -369,6 +371,26 @@ class FrontEndB200 {
     for (size_t s = 0; s < n; ++s)
       paths_xy[s].assign(xy.begin() + 2 * offsets[s], xy.begin() + 2 * offsets[s + 1]);
     return true;
+  }
+
+  // Global registration (include/tloam_b200.h "Global registration"): two clouds aligned with no initial guess by FPFH
+  // features, mutual matches, RANSAC and a truncated-least-squares refinement on the GPU.  Each cloud is in its sensor's
+  // frame (normals point to the origin).  out.T is target <- source (column-major); hand it on when out.accepted.
+  bool enableGlobalRegistration(const tloam_global_registration_config& cfg) {
+    return report(tloam_b200_global_registration_enable(h_, &cfg), "enableGlobalRegistration");
+  }
+  bool enableGlobalRegistration() {
+    tloam_global_registration_config c;
+    tloam_b200_global_registration_default_config(&c);
+    return enableGlobalRegistration(c);
+  }
+  bool globalRegister(const CloudData& source, const CloudData& target, tloam_global_registration_result& out) {
+    return report(tloam_b200_global_register(h_, data(source), size(source), data(target), size(target), &out), "globalRegister");
+  }
+  // loop keyframe query to loop keyframe candidate (needs enableLoopVerification): out.T = T_cand_query, the guess that
+  // tloam_b200_loop_verify takes where Scan Context's yaw would not reach
+  bool globalRegisterLoop(long long query, long long candidate, tloam_global_registration_result& out) {
+    return report(tloam_b200_global_register_loop(h_, query, candidate, &out), "globalRegisterLoop");
   }
 
   // The merged map (include/tloam_b200.h "Merged global map"): the whole map, or with static_only the points

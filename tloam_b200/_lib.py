@@ -183,6 +183,23 @@ class PlanInfo(C.Structure):
                 ("rounds", C.c_ulonglong), ("tiles", C.c_ulonglong)]
 
 
+class GlobalRegistrationConfig(C.Structure):
+    """tloam_global_registration_config (include/tloam_b200.h "Global registration")."""
+    _fields_ = [("voxel", C.c_double), ("cell", C.c_double), ("normal_radius", C.c_double), ("min_normal_neighbours", C.c_int),
+                ("feature_radius", C.c_double), ("max_correspondence_distance", C.c_double), ("n_hypotheses", C.c_int),
+                ("seed", C.c_ulonglong), ("edge_similarity", C.c_double), ("min_triangle_area", C.c_double),
+                ("max_refine_iterations", C.c_int), ("min_inliers", C.c_int), ("min_fitness", C.c_double)]
+
+
+class GlobalRegistrationResult(C.Structure):
+    """tloam_global_registration_result: T (target <- source, column-major), the counts of each stage and the verdict."""
+    _fields_ = [("T", C.c_double * 16), ("n_source_points", C.c_longlong), ("n_target_points", C.c_longlong),
+                ("n_source_features", C.c_longlong), ("n_target_features", C.c_longlong), ("n_correspondences", C.c_longlong),
+                ("n_valid_hypotheses", C.c_int), ("best_hypothesis", C.c_int), ("best_inliers", C.c_int), ("inliers", C.c_int),
+                ("inlier_rmse", C.c_double), ("fitness", C.c_double), ("refine_iterations", C.c_int), ("termination", C.c_int),
+                ("accepted", C.c_int)]
+
+
 class PoseGraphConfig(C.Structure):
     """tloam_pose_graph_config (include/tloam_b200.h "Pose graph"): the edges' sigmas and the Gauss-Newton schedule."""
     _fields_ = [("sigma_odom_translation", C.c_double), ("sigma_odom_rotation", C.c_double),
@@ -335,6 +352,9 @@ EXPORTS = [
     "tloam_b200_distance_download", "tloam_b200_distance_query",
     "tloam_b200_plan_default_config", "tloam_b200_plan_build", "tloam_b200_plan_download", "tloam_b200_plan_paths",
     "tloam_b200_plan_path_cells",
+    "tloam_b200_global_registration_default_config", "tloam_b200_global_registration_enable", "tloam_b200_global_register",
+    "tloam_b200_global_register_loop", "tloam_b200_global_registration_side", "tloam_b200_global_registration_correspondences",
+    "tloam_b200_global_registration_hypotheses",
 ]
 
 _lib = None
@@ -589,5 +609,14 @@ def load():
     L.tloam_b200_plan_paths.argtypes = [vp, dp, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_int),
                                         C.POINTER(C.c_ulonglong)]
     L.tloam_b200_plan_path_cells.argtypes = [vp, C.POINTER(C.c_int), dp, C.c_size_t]
+    L.tloam_b200_global_registration_default_config.argtypes = [C.POINTER(GlobalRegistrationConfig)]
+    L.tloam_b200_global_registration_default_config.restype = None
+    L.tloam_b200_global_registration_enable.argtypes = [vp, C.POINTER(GlobalRegistrationConfig)]
+    L.tloam_b200_global_register.argtypes = [vp, dp, C.c_size_t, dp, C.c_size_t, C.POINTER(GlobalRegistrationResult)]
+    L.tloam_b200_global_register_loop.argtypes = [vp, C.c_longlong, C.c_longlong, C.POINTER(GlobalRegistrationResult)]
+    L.tloam_b200_global_registration_side.argtypes = [vp, C.c_int, dp, dp, C.POINTER(C.c_ubyte), ip, dp, C.POINTER(C.c_ubyte),
+                                                      C.c_size_t, szp]
+    L.tloam_b200_global_registration_correspondences.argtypes = [vp, ip, C.c_size_t, szp]
+    L.tloam_b200_global_registration_hypotheses.argtypes = [vp, ip, C.c_size_t, szp]
     _lib = L
     return L

@@ -43,6 +43,7 @@
 #include "occupancy.h"
 #include "distance.h"
 #include "plan.h"
+#include "global_registration.h"
 
 
 
@@ -372,6 +373,19 @@ struct tloam_b200_handle {
   tloam_pg_state* d_pg_state = nullptr;
   const double* d_pg_T = nullptr;          size_t pg_opt_nodes = 0;                            // the last optimisation
   const double* d_pgr_w = nullptr;         size_t pgr_w_edges = 0;                             // its loop weights (robust)
+  // ---- global registration (tloam_b200_global_register*, libtloam_b200_greg.so): per side the keypoints, their index,
+  //      normals and features in one buffer; the host clouds' down-sample and the run's pairs, hypotheses and state;
+  //      nothing is allocated or launched until it is enabled ----
+  bool gr_on = false;                      tloam_global_registration_config gr_cfg;
+  unsigned char* d_gr_side[2] = {nullptr, nullptr};  size_t cap_gr_side[2] = {0, 0};
+  unsigned char* d_gr_scratch = nullptr;   size_t cap_gr_scratch = 0;  // an index build's radix sort
+  unsigned char* d_gr_small = nullptr;     // the down-sample's GMapState at 0, the identity pose at 256
+  double* d_gr_reg = nullptr;              size_t cap_gr_reg = 0;
+  double* d_gr_fin = nullptr;              size_t cap_gr_fin = 0;
+  double* d_gr_q = nullptr;                size_t cap_gr_q = 0;        // a host cloud's keypoints
+  double* d_gr_in = nullptr;               size_t cap_gr_in = 0;       // a host cloud
+  unsigned char* d_gr_run = nullptr;       size_t cap_gr_run = 0;      // state, pairs, hypotheses, inlier sets
+  bool gr_ran = false;                     tloam_gr_args gr_last;      unsigned long long gr_nc = 0;  int gr_nh = 0;
 };
 
 // launch bookkeeping: counts the kernel and, in profiling mode, brackets it with events
@@ -587,6 +601,8 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   cudaFree(h->d_rl_dirs); cudaFree(h->d_rl_places); cudaFree(h->d_rl_small); cudaFree(h->d_rl_q); cudaFree(h->d_rl_run);
   cudaFree(h->d_mu_tables); cudaFree(h->d_mu_image); cudaFree(h->d_mu_window); cudaFree(h->d_mu_prior); cudaFree(h->d_mu_add);
   cudaFree(h->d_mu_small); cudaFree(h->d_mu_q); cudaFree(h->d_mu_build); cudaFree(h->d_mu_out);
+  cudaFree(h->d_gr_side[0]); cudaFree(h->d_gr_side[1]); cudaFree(h->d_gr_scratch); cudaFree(h->d_gr_small);
+  cudaFree(h->d_gr_reg); cudaFree(h->d_gr_fin); cudaFree(h->d_gr_q); cudaFree(h->d_gr_in); cudaFree(h->d_gr_run);
   for (void* p : h->mu_retired) cudaFree(p);
   for (int i = 0; i < 2; ++i) if (h->ev_stage_free[i]) cudaEventDestroy(h->ev_stage_free[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_fit[i]) cudaEventDestroy(h->ev_fit[i]);
@@ -6382,39 +6398,43 @@ int tloam_b200_localize_enable(tloam_b200_handle* h, const tloam_localize_config
   return TLOAM_B200_OK;
 }
 
-// the map (already at the start of d_loc_map) indexed: bounds, key range, sort, cells, normals; synchronises
-static int loc_build(tloam_b200_handle* h, size_t n) {
-  LocLib lib;
-  int rc = loc_load(h, &lib);
-  if (rc != TLOAM_B200_OK) return rc;
-  unsigned char* b = h->d_loc_map;
-  tloam_loc_index_args a;
-  memset(&a, 0, sizeof(a));
+// an n-row index laid out from b: the map, the sorted map, normals, cell keys, sorted rows, cell starts, neighbour counts,
+// validity and the state; the pointers into a (a->map is the first n x 3 FP64 block).  Returns the bytes it spans.
+static size_t loc_carve_index(unsigned char* b, size_t n, tloam_loc_index_args* a) {
   size_t o = 0;
-  a.map = reinterpret_cast<const double*>(b + o);   o += round_up(n * 24, 256);
-  a.sxyz = reinterpret_cast<double*>(b + o);        o += round_up(n * 24, 256);
-  a.normal = reinterpret_cast<double*>(b + o);      o += round_up(n * 24, 256);
-  a.ckey = reinterpret_cast<unsigned long long*>(b + o); o += round_up(n * 8, 256);
-  a.srow = reinterpret_cast<unsigned*>(b + o);      o += round_up(n * 4, 256);
-  a.cstart = reinterpret_cast<unsigned*>(b + o);    o += round_up((n + 1) * 4, 256);
-  a.neighbours = reinterpret_cast<int*>(b + o);     o += round_up(n * 4, 256);
-  a.valid = b + o;                                  o += round_up(n, 256);
-  a.st = reinterpret_cast<tloam_gmm_state*>(b + o);
+  if (a) a->map = reinterpret_cast<const double*>(b + o);          o += round_up(n * 24, 256);
+  if (a) a->sxyz = reinterpret_cast<double*>(b + o);               o += round_up(n * 24, 256);
+  if (a) a->normal = reinterpret_cast<double*>(b + o);             o += round_up(n * 24, 256);
+  if (a) a->ckey = reinterpret_cast<unsigned long long*>(b + o);   o += round_up(n * 8, 256);
+  if (a) a->srow = reinterpret_cast<unsigned*>(b + o);             o += round_up(n * 4, 256);
+  if (a) a->cstart = reinterpret_cast<unsigned*>(b + o);           o += round_up((n + 1) * 4, 256);
+  if (a) a->neighbours = reinterpret_cast<int*>(b + o);            o += round_up(n * 4, 256);
+  if (a) a->valid = b + o;                                          o += round_up(n, 256);
+  if (a) a->st = reinterpret_cast<tloam_gmm_state*>(b + o);        o += round_up(sizeof(tloam_gmm_state), 256);
+  return o;
+}
+
+// the index of the n rows at a->map (carved by loc_carve_index) with the given cell and normal rule: bounds (synchronises),
+// the key range and rounding checks, then keys, sort, cells and normals, enqueued; the radix sort's scratch grown in
+// *scratch.  INVALID_ARG for a non-finite row, VOXEL_RANGE for an extent or coordinates the grid cannot hold.
+static int loc_index_build(tloam_b200_handle* h, const LocLib& lib, tloam_loc_index_args& a, size_t n, double cell,
+                           double normal_radius, double max_planarity, int min_normal_neighbours, unsigned char** scratch,
+                           size_t* cap_scratch) {
   a.n = n;
-  a.normal_radius = h->loc_cfg.normal_radius; a.max_planarity = h->loc_cfg.max_planarity;
-  a.min_normal_neighbours = h->loc_cfg.min_normal_neighbours;
+  a.normal_radius = normal_radius; a.max_planarity = max_planarity;
+  a.min_normal_neighbours = min_normal_neighbours;
   a.grid.sxyz = a.sxyz; a.grid.srow = a.srow; a.grid.ckey = a.ckey; a.grid.cstart = a.cstart; a.grid.st = a.st;
-  a.grid.cell = h->loc_cfg.cell;
+  a.grid.cell = cell;
   a.device = h->device; a.stream = h->stream;
   const size_t bytes = lib.scratch_bytes(n ? n : 1);
-  if (bytes > h->cap_loc_scratch) {
+  if (bytes > *cap_scratch) {
     CU_TRY(cudaStreamSynchronize(h->stream));
-    cudaFree(h->d_loc_scratch); h->d_loc_scratch = nullptr; h->cap_loc_scratch = 0;
-    CU_TRY(cudaMalloc(&h->d_loc_scratch, bytes));
-    h->cap_loc_scratch = bytes;
+    cudaFree(*scratch); *scratch = nullptr; *cap_scratch = 0;
+    CU_TRY(cudaMalloc(scratch, bytes));
+    *cap_scratch = bytes;
   }
-  a.scratch = h->d_loc_scratch;
-  int e = 0, launches = 0;
+  a.scratch = *scratch;
+  int e = 0, launches = 0, rc;
   TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.bounds(&a, &launches)));
   h->launches += launches > 0 ? launches - 1 : 0;
   if ((rc = loc_status(h, e, "k_loc_bounds")) != TLOAM_B200_OK) return rc;
@@ -6439,8 +6459,22 @@ static int loc_build(tloam_b200_handle* h, size_t n) {
     TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.index(&a, &launches)));
     h->launches += launches > 0 ? launches - 1 : 0;
     if ((rc = loc_status(h, e, "k_loc_keys / k_gmm_* / k_loc_cells / k_loc_normals")) != TLOAM_B200_OK) return rc;
-    CU_TRY(cudaStreamSynchronize(h->stream));
   }
+  return TLOAM_B200_OK;
+}
+
+// the map (already at the start of d_loc_map) indexed: bounds, key range, sort, cells, normals; synchronises
+static int loc_build(tloam_b200_handle* h, size_t n) {
+  LocLib lib;
+  int rc = loc_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  tloam_loc_index_args a;
+  memset(&a, 0, sizeof(a));
+  loc_carve_index(h->d_loc_map, n, &a);
+  if ((rc = loc_index_build(h, lib, a, n, h->loc_cfg.cell, h->loc_cfg.normal_radius, h->loc_cfg.max_planarity,
+                            h->loc_cfg.min_normal_neighbours, &h->d_loc_scratch, &h->cap_loc_scratch)) != TLOAM_B200_OK)
+    return rc;
+  if (n) CU_TRY(cudaStreamSynchronize(h->stream));
   h->loc_index = a;
   h->loc_n = n; h->loc_loaded = true;
   return TLOAM_B200_OK;
@@ -6448,8 +6482,7 @@ static int loc_build(tloam_b200_handle* h, size_t n) {
 
 // room for an n-row map and its index at the start of d_loc_map (the old map is dropped)
 static int loc_reserve_map(tloam_b200_handle* h, size_t n) {
-  const size_t need = 3 * round_up(n * 24, 256) + round_up(n * 8, 256) + round_up(n * 4, 256) + round_up((n + 1) * 4, 256) +
-                      round_up(n * 4, 256) + round_up(n, 256) + round_up(sizeof(tloam_gmm_state), 256);
+  const size_t need = loc_carve_index(nullptr, n, nullptr);
   if (need > h->cap_loc_map) {
     CU_TRY(cudaStreamSynchronize(h->stream));
     cudaFree(h->d_loc_map); h->d_loc_map = nullptr; h->cap_loc_map = 0;
@@ -6490,18 +6523,19 @@ int tloam_b200_localize_set_map_merged(tloam_b200_handle* h) {
 // the query: VoxelDownSample(voxel) of the finite rows of the n rows at d_in by the global map's ordered path at pose I
 // (the keyframe path of loop verification, in buffers of its own) into *q with its state at st (the localization's, or
 // relocalization's own); synchronises and returns its row count
-static int loc_query(tloam_b200_handle* h, const double* d_in, size_t n, size_t* nq, GMapState* st, double** q, size_t* cap_q) {
+// the same down-sample at `voxel` into the given buffers (reg, fin: the transform's scratch; eye: the identity on the device)
+static int ordered_query(tloam_b200_handle* h, const double* d_in, size_t n, double voxel, const double* eye, double** reg,
+                         size_t* cap_reg, double** fin, size_t* cap_fin, GMapState* st, double** q, size_t* cap_q, size_t* nq) {
   int rc;
-  if ((rc = ensure_dev(h, &h->d_loc_reg, &h->cap_loc_reg, n, false)) != TLOAM_B200_OK) return rc;
-  if ((rc = ensure_dev(h, &h->d_loc_fin, &h->cap_loc_fin, n, false)) != TLOAM_B200_OK) return rc;
+  if ((rc = ensure_dev(h, reg, cap_reg, n, false)) != TLOAM_B200_OK) return rc;
+  if ((rc = ensure_dev(h, fin, cap_fin, n, false)) != TLOAM_B200_OK) return rc;
   if ((rc = ensure_dev(h, q, cap_q, n, false)) != TLOAM_B200_OK) return rc;
-  const double voxel = h->loc_cfg.voxel;
   CU_TRY(cudaMemsetAsync(st, 0, sizeof(GMapState), h->stream));
   const unsigned tb = 256, gb = (unsigned)((n + tb - 1) / tb);
-  if (n) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_transform<<<gb, tb, 0, h->stream>>>(d_in, (unsigned)n, loc_eye(h), h->d_loc_reg, h->d_loc_fin, st)));
+  if (n) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_transform<<<gb, tb, 0, h->stream>>>(d_in, (unsigned)n, eye, *reg, *fin, st)));
   if (n) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_guard<<<1, 32, 0, h->stream>>>(st, voxel)));
   VoxSorted vs;
-  if ((rc = voxel_pipeline(h, h->d_loc_fin, n, &st->n_fin, 0u, nullptr, nullptr, nullptr, 0.0, voxel, nullptr, &st->n_vox,
+  if ((rc = voxel_pipeline(h, *fin, n, &st->n_fin, 0u, nullptr, nullptr, nullptr, 0.0, voxel, nullptr, &st->n_vox,
                            h->stream, 0, &vs)) != TLOAM_B200_OK) return rc;
   if (n) TL_LAUNCH(TLOAM_B200_K_SUBMAP, (k_gmap_emit<<<gb, tb, 0, h->stream>>>(vs.a, vs.slots, *q, st, *cap_q)));
   CU_TRY(cudaGetLastError());
@@ -6511,6 +6545,11 @@ static int loc_query(tloam_b200_handle* h, const double* d_in, size_t n, size_t*
   if (s.refused) return TLOAM_B200_ERR_VOXEL_RANGE;
   *nq = s.refused ? 0 : s.n_vox;
   return TLOAM_B200_OK;
+}
+
+static int loc_query(tloam_b200_handle* h, const double* d_in, size_t n, size_t* nq, GMapState* st, double** q, size_t* cap_q) {
+  return ordered_query(h, d_in, n, h->loc_cfg.voxel, loc_eye(h), &h->d_loc_reg, &h->cap_loc_reg, &h->d_loc_fin, &h->cap_loc_fin,
+                       st, q, cap_q, nq);
 }
 
 static int loc_run(tloam_b200_handle* h, const double* d_in, size_t n, const double* guess, tloam_localize_result* out) {
@@ -7421,6 +7460,274 @@ int tloam_b200_localize_set_map_updated(tloam_b200_handle* h) {
   if ((rc = loc_reserve_map(h, n)) != TLOAM_B200_OK) return rc;
   if (n) CU_TRY(cudaMemcpyAsync(h->d_loc_map, h->d_mu_out, n * 24, cudaMemcpyDeviceToDevice, h->stream));
   return mu_after_load(h, loc_build(h, n));
+}
+
+// ---------------------------------------------------------------------------------------------
+// Global registration (the checks, the keypoints' down-sample, the loader and the buffers here; each side's index and
+// normals from localize.cu's tloam_loc_index, the rest in global_registration.cu, loaded from libtloam_b200_greg.so by
+// the enable call).
+// ---------------------------------------------------------------------------------------------
+static std::mutex g_gr_mu;
+static tloam_gr_run_fn g_gr_run = nullptr;
+
+static int gr_load(tloam_b200_handle* h, tloam_gr_run_fn* out) {
+  std::lock_guard<std::mutex> lk(g_gr_mu);
+  if (!g_gr_run) {
+    const std::string path = sibling_path("libtloam_b200_greg.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    tloam_gr_run_fn f = so ? reinterpret_cast<tloam_gr_run_fn>(dlsym(so, "tloam_gr_run")) : nullptr;
+    if (!f) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "global registration: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_gr_run = f;
+  }
+  *out = g_gr_run;
+  return TLOAM_B200_OK;
+}
+
+static int gr_status(tloam_b200_handle* h, int e, const char* where) {
+  if (e == cudaSuccess) return TLOAM_B200_OK;
+  snprintf(h->last_error, sizeof(h->last_error), "global registration: %s: %s", where, cudaGetErrorString((cudaError_t)e));
+  return TLOAM_B200_ERR_CUDA;
+}
+
+void tloam_b200_global_registration_default_config(tloam_global_registration_config* c) {
+  c->voxel = 0.5; c->cell = 1.0; c->normal_radius = 1.0; c->min_normal_neighbours = 5; c->feature_radius = 2.5;
+  c->max_correspondence_distance = 0.75; c->n_hypotheses = 65536; c->seed = 0; c->edge_similarity = 0.9;
+  c->min_triangle_area = 1.0; c->max_refine_iterations = 10; c->min_inliers = 30; c->min_fitness = 0.3;
+}
+
+int tloam_b200_global_registration_enable(tloam_b200_handle* h, const tloam_global_registration_config* c) {
+  if (!h || !c) return TLOAM_B200_ERR_INVALID_ARG;
+  const double v[7] = {c->voxel, c->cell, c->normal_radius, c->feature_radius, c->max_correspondence_distance, c->edge_similarity,
+                       c->min_triangle_area};
+  for (double x : v)
+    if (!std::isfinite(x) || !(x > 0.0)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (c->min_normal_neighbours < 3 || c->normal_radius > 3.0 * c->cell || c->feature_radius > 3.0 * c->cell ||
+      c->n_hypotheses < 1 || c->n_hypotheses > (1 << 20) || c->edge_similarity > 1.0 || c->max_refine_iterations < 1 ||
+      c->max_refine_iterations > 100 || c->min_inliers < 0 || !(c->min_fitness >= 0.0 && c->min_fitness <= 1.0))
+    return TLOAM_B200_ERR_INVALID_ARG;
+  tloam_gr_run_fn run;
+  int rc = gr_load(h, &run);
+  if (rc != TLOAM_B200_OK) return rc;
+  LocLib lib;
+  if ((rc = loc_load(h, &lib)) != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (!h->d_gr_small) {
+    CU_TRY(cudaMalloc(&h->d_gr_small, 512));
+    const double eye[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+    CU_TRY(cudaMemcpy(h->d_gr_small + 256, eye, sizeof(eye), cudaMemcpyHostToDevice));
+  }
+  h->gr_cfg = *c;
+  h->gr_on = true;
+  h->gr_ran = false; h->gr_nc = 0; h->gr_nh = 0;
+  return TLOAM_B200_OK;
+}
+
+// a host cloud's keypoints: the finite rows of the n rows at d_in down-sampled as loc_query does, in this feature's
+// buffers, into d_gr_q; synchronises and returns their count
+static int gr_query(tloam_b200_handle* h, const double* d_in, size_t n, size_t* nq) {
+  return ordered_query(h, d_in, n, h->gr_cfg.voxel, reinterpret_cast<const double*>(h->d_gr_small + 256), &h->d_gr_reg,
+                       &h->cap_gr_reg, &h->d_gr_fin, &h->cap_gr_fin, reinterpret_cast<GMapState*>(h->d_gr_small), &h->d_gr_q,
+                       &h->cap_gr_q, nq);
+}
+
+// side k: the n keypoints at d_pts copied into its buffer and indexed with normals as a localization map is
+// (loc_carve_index / loc_index_build, max_planarity 1), then the feature's arrays; synchronises after the bounds
+static int gr_side(tloam_b200_handle* h, int k, const double* d_pts, size_t n, tloam_gr_side* out) {
+  LocLib lib;
+  int rc = loc_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  const size_t base = loc_carve_index(nullptr, n, nullptr);
+  const size_t need = base + round_up(n * TLOAM_GR_BINS * 4, 256) + round_up(n * 4, 256) + round_up(n * TLOAM_GR_BINS * 8, 256) +
+                      round_up(n, 256) + n * 4;
+  if (need > h->cap_gr_side[k]) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_gr_side[k]); h->d_gr_side[k] = nullptr; h->cap_gr_side[k] = 0;
+    CU_TRY(cudaMalloc(&h->d_gr_side[k], need));
+    h->cap_gr_side[k] = need;
+  }
+  unsigned char* b = h->d_gr_side[k];
+  tloam_loc_index_args a;
+  memset(&a, 0, sizeof(a));
+  memset(out, 0, sizeof(*out));
+  size_t o = loc_carve_index(b, n, &a);
+  out->spfh = reinterpret_cast<int*>(b + o);        o += round_up(n * TLOAM_GR_BINS * 4, 256);
+  out->pairs = reinterpret_cast<int*>(b + o);       o += round_up(n * 4, 256);
+  out->feature = reinterpret_cast<double*>(b + o);  o += round_up(n * TLOAM_GR_BINS * 8, 256);
+  out->has_feature = b + o;                         o += round_up(n, 256);
+  out->nn = reinterpret_cast<int*>(b + o);
+  if (n) CU_TRY(cudaMemcpyAsync(const_cast<double*>(a.map), d_pts, n * 24, cudaMemcpyDeviceToDevice, h->stream));
+  const tloam_global_registration_config& c = h->gr_cfg;
+  if ((rc = loc_index_build(h, lib, a, n, c.cell, c.normal_radius, 1.0, c.min_normal_neighbours, &h->d_gr_scratch,
+                            &h->cap_gr_scratch)) != TLOAM_B200_OK)
+    return rc;
+  out->grid = a.grid;
+  out->xyz = a.map; out->normal = a.normal; out->valid = a.valid; out->n = n;
+  return TLOAM_B200_OK;
+}
+
+// the run over the two sides built by gr_side; one copy of the state home
+static int gr_run(tloam_b200_handle* h, tloam_gr_side src, tloam_gr_side tgt, tloam_global_registration_result* out) {
+  tloam_gr_run_fn run;
+  int rc = gr_load(h, &run);
+  if (rc != TLOAM_B200_OK) return rc;
+  const tloam_global_registration_config& c = h->gr_cfg;
+  memset(out, 0, sizeof(*out));
+  out->T[0] = out->T[5] = out->T[10] = out->T[15] = 1.0;
+  out->n_source_points = (long long)src.n; out->n_target_points = (long long)tgt.n;
+  out->best_hypothesis = -1;
+  tloam_gr_args a;
+  memset(&a, 0, sizeof(a));
+  a.src = src; a.tgt = tgt;
+  h->gr_last = a; h->gr_ran = true; h->gr_nc = 0; h->gr_nh = 0;
+  if (!src.n || !tgt.n) {
+    out->termination = TLOAM_GLOBAL_REGISTRATION_EMPTY;
+    return TLOAM_B200_OK;
+  }
+  const size_t ns = src.n, nh = (size_t)c.n_hypotheses;
+  const size_t o_corr = round_up(sizeof(tloam_gr_state), 256);
+  const size_t o_hyp = o_corr + round_up(ns * 2 * sizeof(int), 256);
+  const size_t o_set = o_hyp + round_up(nh * sizeof(int), 256);
+  const size_t bytes = o_set + 2 * ns;
+  if (bytes > h->cap_gr_run) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_gr_run); h->d_gr_run = nullptr; h->cap_gr_run = 0;
+    CU_TRY(cudaMalloc(&h->d_gr_run, bytes));
+    h->cap_gr_run = bytes;
+  }
+  unsigned char* base = h->d_gr_run;
+  a.state = reinterpret_cast<tloam_gr_state*>(base);
+  a.src.n_features = &a.state->n_features[0];
+  a.tgt.n_features = &a.state->n_features[1];
+  a.feature_radius = c.feature_radius; a.tau = c.max_correspondence_distance;
+  for (int k = 0; k < 10; ++k) {   // volatile: the boundaries' cos and sin from the C library at run time, never folded
+    volatile double beta = (2.0 * (k + 1) / 11.0 - 1.0) * M_PI;
+    a.theta_cs[2 * k] = std::cos(beta);
+    a.theta_cs[2 * k + 1] = std::sin(beta);
+  }
+  a.n_hypotheses = c.n_hypotheses; a.seed = c.seed;
+  a.edge_similarity = c.edge_similarity; a.min_triangle_area = c.min_triangle_area;
+  a.max_refine_iterations = c.max_refine_iterations;
+  a.corr = reinterpret_cast<int*>(base + o_corr);
+  a.hyp_inliers = reinterpret_cast<int*>(base + o_hyp);
+  a.in_set = base + o_set;
+  a.device = h->device; a.stream = h->stream;
+  int e = 0, launches = 0;
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = run(&a, &launches)));
+  h->launches += launches > 0 ? launches - 1 : 0;
+  if ((rc = gr_status(h, e, "k_gr_*")) != TLOAM_B200_OK) return rc;
+  tloam_gr_state s;
+  CU_TRY(cudaMemcpyAsync(&s, a.state, sizeof(s), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  for (int r = 0; r < 3; ++r) {
+    for (int j = 0; j < 3; ++j) out->T[4 * j + r] = s.R[3 * r + j];
+    out->T[12 + r] = s.t[r];
+  }
+  out->n_source_features = (long long)s.n_features[0]; out->n_target_features = (long long)s.n_features[1];
+  out->n_correspondences = (long long)s.n_corr;
+  out->n_valid_hypotheses = s.n_valid; out->best_hypothesis = s.best; out->best_inliers = s.best_inliers;
+  out->inliers = s.inliers; out->inlier_rmse = s.rmse; out->refine_iterations = s.iterations; out->termination = s.term;
+  out->fitness = (double)s.fit_count / (double)src.n;
+  out->accepted = out->inliers >= c.min_inliers && out->fitness >= c.min_fitness ? 1 : 0;
+  h->gr_last = a; h->gr_nc = s.n_corr; h->gr_nh = c.n_hypotheses;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_global_register(tloam_b200_handle* h, const double* src, size_t n_src, const double* tgt, size_t n_tgt,
+                               tloam_global_registration_result* out) {
+  if (!h || !out || (!src && n_src) || (!tgt && n_tgt) || n_src > ((size_t)1 << 30) || n_tgt > ((size_t)1 << 30))
+    return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gr_on) return TLOAM_B200_ERR_NOT_READY;
+  CU_TRY(cudaSetDevice(h->device));
+  h->gr_ran = false;
+  tloam_gr_side side[2];
+  const double* cloud[2] = {src, tgt};
+  const size_t n[2] = {n_src, n_tgt};
+  int rc;
+  for (int k = 0; k < 2; ++k) {
+    if ((rc = ensure_dev(h, &h->d_gr_in, &h->cap_gr_in, n[k], false)) != TLOAM_B200_OK) return rc;
+    if (n[k] && (rc = upload_host(h, h->d_gr_in, cloud[k], n[k] * 24)) != TLOAM_B200_OK) return rc;
+    size_t nq = 0;
+    if ((rc = gr_query(h, h->d_gr_in, n[k], &nq)) != TLOAM_B200_OK) return rc;
+    if ((rc = gr_side(h, k, h->d_gr_q, nq, &side[k])) != TLOAM_B200_OK) return rc;
+  }
+  return gr_run(h, side[0], side[1], out);
+}
+
+int tloam_b200_global_register_loop(tloam_b200_handle* h, long long query, long long candidate,
+                                    tloam_global_registration_result* out) {
+  if (!h || !out) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gr_on || !h->lv_on) return TLOAM_B200_ERR_NOT_READY;
+  if (query < 0 || candidate < 0 || (size_t)query >= h->loop_frames || (size_t)candidate >= h->loop_frames)
+    return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  h->gr_ran = false;
+  tloam_gr_side side[2];
+  const long long f[2] = {query, candidate};
+  int rc;
+  for (int k = 0; k < 2; ++k) {
+    unsigned long long first = 0, cnt = 0;
+    if ((rc = lv_range(h, (size_t)f[k], &first, &cnt)) != TLOAM_B200_OK) return rc;
+    if ((rc = gr_side(h, k, h->d_lv_pts + 3 * first, cnt, &side[k])) != TLOAM_B200_OK) return rc;
+  }
+  return gr_run(h, side[0], side[1], out);
+}
+
+int tloam_b200_global_registration_side(tloam_b200_handle* h, int side, double* xyz, double* normal, unsigned char* valid,
+                                        int* spfh, double* feature, unsigned char* has_feature, size_t capacity, size_t* n) {
+  if (!h || !n) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gr_on || !h->gr_ran) return TLOAM_B200_ERR_NOT_READY;
+  if (side != 0 && side != 1) return TLOAM_B200_ERR_INVALID_ARG;
+  const tloam_gr_side& s = side ? h->gr_last.tgt : h->gr_last.src;
+  const size_t m = s.n;
+  *n = m;
+  if (capacity < m) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!m) return TLOAM_B200_OK;
+  const bool featured = h->gr_nh > 0;                        // an EMPTY run computed no feature
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (xyz) CU_TRY(cudaMemcpyAsync(xyz, s.xyz, m * 24, cudaMemcpyDeviceToHost, h->stream));
+  if (normal) CU_TRY(cudaMemcpyAsync(normal, s.normal, m * 24, cudaMemcpyDeviceToHost, h->stream));
+  if (valid) CU_TRY(cudaMemcpyAsync(valid, s.valid, m, cudaMemcpyDeviceToHost, h->stream));
+  if (featured && spfh) CU_TRY(cudaMemcpyAsync(spfh, s.spfh, m * TLOAM_GR_BINS * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  if (featured && feature) CU_TRY(cudaMemcpyAsync(feature, s.feature, m * TLOAM_GR_BINS * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (featured && has_feature) CU_TRY(cudaMemcpyAsync(has_feature, s.has_feature, m, cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  if (!featured) {
+    if (spfh) memset(spfh, 0, m * TLOAM_GR_BINS * sizeof(int));
+    if (feature) memset(feature, 0, m * TLOAM_GR_BINS * sizeof(double));
+    if (has_feature) memset(has_feature, 0, m);
+  }
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_global_registration_correspondences(tloam_b200_handle* h, int* pairs, size_t capacity, size_t* n) {
+  if (!h || !n) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gr_on || !h->gr_ran) return TLOAM_B200_ERR_NOT_READY;
+  *n = h->gr_nc;
+  if (capacity < h->gr_nc) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!pairs || !h->gr_nc) return TLOAM_B200_OK;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaMemcpyAsync(pairs, h->gr_last.corr, h->gr_nc * 2 * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_global_registration_hypotheses(tloam_b200_handle* h, int* inliers, size_t capacity, size_t* n) {
+  if (!h || !n) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gr_on || !h->gr_ran) return TLOAM_B200_ERR_NOT_READY;
+  *n = (size_t)h->gr_nh;
+  if (capacity < *n) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!inliers || !*n) return TLOAM_B200_OK;
+  CU_TRY(cudaSetDevice(h->device));
+  CU_TRY(cudaMemcpyAsync(inliers, h->gr_last.hyp_inliers, *n * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
 }
 
 int tloam_b200_host_alloc(void** p, size_t bytes) {

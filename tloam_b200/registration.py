@@ -157,6 +157,29 @@ class LocalizeResult:
 
 
 @dataclasses.dataclass(frozen=True)
+class GlobalRegistrationResult:
+    """tloam_global_registration_result: T (4 x 4) = target <- source (from global_register_loop: T_cand_query, a guess
+    for loop_verify); termination is one of GlobalRegistrationResult.CONVERGED .. EMPTY; accepted = inliers >= min_inliers
+    and fitness >= min_fitness."""
+    T: np.ndarray
+    n_source_points: int
+    n_target_points: int
+    n_source_features: int
+    n_target_features: int
+    n_correspondences: int
+    n_valid_hypotheses: int
+    best_hypothesis: int
+    best_inliers: int
+    inliers: int
+    inlier_rmse: float
+    fitness: float
+    refine_iterations: int
+    termination: int
+    accepted: bool
+    CONVERGED, ITERATION_LIMIT, FEW_INLIERS, FEW_CORRESPONDENCES, NO_HYPOTHESIS, EMPTY = range(6)
+
+
+@dataclasses.dataclass(frozen=True)
 class RelocalizeResult:
     """tloam_relocalize_result: result = the winner's LocalizeResult; place / shift / distance its candidate (place -1
     without hypotheses); winner = its rank; accepted = the winner is accepted and no distinct hypothesis fits about as
@@ -1320,6 +1343,79 @@ class LocalRegistration:
         self._check(self._L.tloam_b200_localize_cells(self._h, rows.ctypes.data_as(up), keys.ctypes.data_as(C.POINTER(C.c_ulonglong)),
                                                       starts.ctypes.data_as(up), n_rows, C.byref(nc)), "localize_cells")
         return rows, keys[:nc.value], starts[:nc.value + 1]
+
+    # ---- global registration (include/tloam_b200.h "Global registration") ----
+    def global_registration_enable(self, **overrides):
+        """turn global registration on; overrides: fields of tloam_global_registration_config (voxel, cell, normal_radius,
+        min_normal_neighbours, feature_radius, max_correspondence_distance, n_hypotheses, seed, edge_similarity,
+        min_triangle_area, max_refine_iterations, min_inliers, min_fitness)"""
+        cfg = _lib.GlobalRegistrationConfig()
+        self._L.tloam_b200_global_registration_default_config(C.byref(cfg))
+        for k, v in overrides.items():
+            if not hasattr(cfg, k):
+                raise KeyError(k)
+            setattr(cfg, k, v)
+        self._check(self._L.tloam_b200_global_registration_enable(self._h, C.byref(cfg)), "global_registration_enable")
+
+    @staticmethod
+    def _global_registration_out(r):
+        return GlobalRegistrationResult(np.array(r.T[:]).reshape(4, 4, order="F"), r.n_source_points, r.n_target_points,
+                                        r.n_source_features, r.n_target_features, r.n_correspondences, r.n_valid_hypotheses,
+                                        r.best_hypothesis, r.best_inliers, r.inliers, r.inlier_rmse, r.fitness,
+                                        r.refine_iterations, r.termination, bool(r.accepted))
+
+    def global_register(self, source, target):
+        """align host cloud source (n x 3) to host cloud target (m x 3) with no guess; returns a GlobalRegistrationResult"""
+        p = np.ascontiguousarray(np.asarray(source, dtype=np.float64).reshape(-1, 3))
+        q = np.ascontiguousarray(np.asarray(target, dtype=np.float64).reshape(-1, 3))
+        r = _lib.GlobalRegistrationResult()
+        self._check(self._L.tloam_b200_global_register(self._h, _dp(p) if len(p) else None, len(p), _dp(q) if len(q) else None,
+                                                       len(q), C.byref(r)), "global_register")
+        return self._global_registration_out(r)
+
+    def global_register_loop(self, query, candidate):
+        """align loop keyframe query to loop keyframe candidate with no guess: T = T_cand_query"""
+        r = _lib.GlobalRegistrationResult()
+        self._check(self._L.tloam_b200_global_register_loop(self._h, int(query), int(candidate), C.byref(r)),
+                    "global_register_loop")
+        return self._global_registration_out(r)
+
+    def global_registration_side(self, side):
+        """the last run's side (0 source, 1 target): dict of keypoints (n x 3), oriented normals (n x 3), valid (n,), SPFH
+        counts (n x 33), features (n x 33) and has_feature (n,)"""
+        n = C.c_size_t(0)
+        self._check(self._L.tloam_b200_global_registration_side(self._h, int(side), None, None, None, None, None, None,
+                                                                1 << 62, C.byref(n)), "global_registration_side")
+        m = n.value
+        out = dict(xyz=np.zeros((m, 3)), normal=np.zeros((m, 3)), valid=np.zeros(m, dtype=np.uint8),
+                   spfh=np.zeros((m, 33), dtype=np.int32), feature=np.zeros((m, 33)), has_feature=np.zeros(m, dtype=np.uint8))
+        ub, ip = C.POINTER(C.c_ubyte), C.POINTER(C.c_int)
+        self._check(self._L.tloam_b200_global_registration_side(
+            self._h, int(side), _dp(out["xyz"]), _dp(out["normal"]), out["valid"].ctypes.data_as(ub), out["spfh"].ctypes.data_as(ip),
+            _dp(out["feature"]), out["has_feature"].ctypes.data_as(ub), m, C.byref(n)), "global_registration_side")
+        out["valid"], out["has_feature"] = out["valid"].astype(bool), out["has_feature"].astype(bool)
+        return out
+
+    def global_registration_correspondences(self):
+        """the last run's mutual pairs (n x 2: source row, target row) in source order"""
+        n = C.c_size_t(0)
+        self._check(self._L.tloam_b200_global_registration_correspondences(self._h, None, 1 << 62, C.byref(n)),
+                    "global_registration_correspondences")
+        out = np.zeros((n.value, 2), dtype=np.int32)
+        self._check(self._L.tloam_b200_global_registration_correspondences(self._h, out.ctypes.data_as(C.POINTER(C.c_int)),
+                                                                            n.value, C.byref(n)),
+                    "global_registration_correspondences")
+        return out
+
+    def global_registration_hypotheses(self):
+        """the last run's inliers per hypothesis (-1: rejected)"""
+        n = C.c_size_t(0)
+        self._check(self._L.tloam_b200_global_registration_hypotheses(self._h, None, 1 << 62, C.byref(n)),
+                    "global_registration_hypotheses")
+        out = np.zeros(n.value, dtype=np.int32)
+        self._check(self._L.tloam_b200_global_registration_hypotheses(self._h, out.ctypes.data_as(C.POINTER(C.c_int)), n.value,
+                                                                       C.byref(n)), "global_registration_hypotheses")
+        return out
 
     # ---- relocalization in a prior map (include/tloam_b200.h "Relocalization in a prior map") ----
     def relocalize_enable(self, **overrides):
