@@ -1630,6 +1630,98 @@ int tloam_b200_plan_paths(tloam_b200_handle* h, const double* starts_xy, size_t 
  * INVALID_ARG: capacity < offsets[n] of that call. */
 int tloam_b200_plan_path_cells(tloam_b200_handle* h, int* ij, double* xy, size_t capacity);
 
+/* ---- Frontiers: the boundaries between known free space and unknown space on the costmap (frontier exploration,
+ * Yamauchi 1997, as explore_lite finds them), each ranked by the plan's path cost to reach it.
+ *   - Source.  The costs (costmap_2d's codes) of the last successful tloam_b200_distance_build or _build_grid, and the
+ *     potential P of the last tloam_b200_plan_build, which must have been built on that same field.  NOT_READY when there
+ *     is no distance build, no plan, or the plan is older than the field.  The plan is meant to have its goal at the
+ *     robot: P(c) is then the cost of the path between c and the robot.
+ *   - Frontier cell (explore_lite's isNewFrontierCell, with a threshold): a cell of code 255 (unknown, not inscribed) with
+ *     at least one 4-neighbour inside the grid of code <= free_max.
+ *   - Frontier: an 8-connected component of frontier cells.  Frontiers are numbered 0, 1, ... (the id) in ascending order
+ *     of their least linear cell index j width + i, so the numbering does not depend on the order of any search.
+ *   - Per frontier: the size n (cells), the integer sums Si, Sj of its cells' i and j, its bounding box, the centroid
+ *     cx = origin_x + ((double)Si / (double)n + 0.5) resolution (likewise cy), and the approach cell: among the
+ *     4-neighbours of code <= free_max of its cells, the one with the least P, ties to the lowest linear index, with its
+ *     centre origin + (i + 0.5) resolution and its P.  free_max <= 252, so every approach cell is passable under any
+ *     plan config.  Status 0 when that P is finite, 1 (unreachable from the plan's goal) otherwise.  Every operation in
+ *     FP64 is rounded on its own (no FMA).
+ *   - Filter and cost.  A frontier is kept iff (double)n resolution >= min_frontier_size.  For a reachable one
+ *     distance = ((double)P / (70.0 (double)neutral_cost)) resolution, the metres of free-cell path of that cost
+ *     (neutral_cost is the plan's), and cost = potential_scale distance - gain_scale ((double)n resolution):
+ *     explore_lite's formula with the path cost in place of its Euclidean distance.  An unreachable frontier has distance
+ *     and cost +infinity.
+ *   - Order.  The kept reachable frontiers by (cost, id) ascending, then the kept unreachable ones by id.
+ *   - Differences to explore_lite.  It walks free space from the robot, so it finds only the frontiers that touch the
+ *     robot's free region; this finds every frontier of the grid and marks the ones the plan cannot reach.  Its distance
+ *     is the Euclidean distance to the nearest frontier cell; this one is the exact path cost to the approach cell.
+ *   - Limits.  free_max <= 252; min_frontier_size, potential_scale and gain_scale finite and >= 0; otherwise INVALID_ARG.
+ *     The distance field's shape limit keeps width x height below 2^32 - 1, so a cell index fits 32 bits.
+ *   - Lifetime.  A search is a snapshot, like a plan: later distance builds, plans and map calls leave its frontiers,
+ *     cells and labels alone; the next search replaces them (a search refused with INVALID_ARG or NOT_READY keeps them)
+ *     and tloam_b200_destroy frees them.
+ *   - Unchanged.  Nothing is hooked into any other call: the distance field, the plan, its kept paths, the map and the
+ *     launch counts of every other call keep their bits, and nothing is allocated or loaded before the first frontier
+ *     call.
+ *   - Device.  A search is k_fr_tile (one block per 32 x 32-cell tile: the frontier flags and a union-find of the tile
+ *     in shared memory, the larger root linked under the smaller), k_fr_border (lock-free unions with atomicMin across
+ *     tile edges and corners), k_fr_flatten (every label its root, which is the component's least index; the frontier
+ *     cells counted), a read-back of their count, k_fr_compact (the frontier cells in index order), the stable radix sort
+ *     of (root, cell) and its head scan (radix_sort.cuh), k_fr_stats (one warp per frontier over its contiguous cells; integer reductions, no
+ *     atomics) and a read-back of the frontiers' statistics.  The cost, the filter and the order are computed on the
+ *     host in FP64; it synchronises.  Memory: 4 B per cell, 1 B per tile and about 93 B per frontier cell (the sort's keys
+ *     and rows 24 B, the heads 4 B, 64 B of statistics per frontier, sized by the cells) on the device, allocated by the
+ *     first search that needs them, grown only and freed by tloam_b200_destroy.
+ *   - The kernels live in libtloam_b200_frontier.so, loaded from this library's directory by the first frontier call; if
+ *     it is missing the calls return ERR_CUDA (tloam_b200_last_error names the file). */
+typedef struct tloam_frontier_config {
+  unsigned free_max;                   /* the highest code of a free cell: 252 every cell a plan can enter, 0 explore_lite's
+                                          FREE_SPACE (nothing within about 2.7 m of an obstacle at the car's inflation) */
+  double min_frontier_size;            /* m: a frontier is kept when n resolution reaches it */
+  double potential_scale;              /* per m of path */
+  double gain_scale;                   /* per m of frontier */
+} tloam_frontier_config;
+typedef struct tloam_frontier {
+  unsigned id;                         /* the frontier's number before the filter */
+  int status;                          /* 0 reachable, 1 unreachable from the plan's goal */
+  size_t size;                         /* cells */
+  unsigned long long sum_i, sum_j;     /* the sums of its cells' i and j */
+  size_t min_i, min_j, max_i, max_j;   /* the bounding box, cells included */
+  double centroid_x, centroid_y;       /* m */
+  size_t approach_i, approach_j;       /* the approach cell */
+  double approach_x, approach_y;       /* its centre, m */
+  unsigned long long approach_potential;   /* P there (0xFFFFFFFFFFFFFFFF when unreachable) */
+  double distance;                     /* m of free-cell path (+infinity when unreachable) */
+  double cost;                         /* potential_scale distance - gain_scale n resolution (+infinity when unreachable) */
+} tloam_frontier;
+typedef struct tloam_frontier_info {
+  double origin_x, origin_y;           /* the corner of cell (0, 0), m: the distance field's */
+  double resolution;
+  size_t width, height;                /* cells along x and y */
+  size_t goal_i, goal_j;               /* the plan's goal cell */
+  size_t cells;                        /* frontier cells */
+  size_t components;                   /* frontiers before the filter */
+  size_t kept;                         /* frontiers after it */
+  size_t reachable;                    /* kept frontiers with status 0 */
+} tloam_frontier_info;
+/* free_max 252, min_frontier_size 0.5 m, potential_scale 3.0, gain_scale 1.0 (explore_lite's scales; robot parameters,
+ * not calibrated) */
+void tloam_b200_frontier_default_config(tloam_frontier_config* c);
+/* the frontiers of the last distance field, ranked by the last plan; synchronises.  INVALID_ARG: cfg null or out of
+ * range.  NOT_READY: see Source.  info may be null. */
+int tloam_b200_frontier_search(tloam_b200_handle* h, const tloam_frontier_config* cfg, tloam_frontier_info* info);
+/* the kept frontiers of the last search in rank order (info.kept of them; out may be null); NOT_READY before any search.
+ * INVALID_ARG: capacity < info.kept. */
+int tloam_b200_frontier_download(tloam_b200_handle* h, tloam_frontier* out, size_t capacity);
+/* the cells of the last search's kept frontiers in rank order, each frontier's cells in ascending linear index: offsets
+ * (info.kept + 1: frontier k is cells offsets[k] .. offsets[k + 1] - 1), ij (2 ints each) and xy (their centres, 2 FP64
+ * each), each may be null; synchronises.  NOT_READY before any search.  INVALID_ARG: capacity < offsets[info.kept]. */
+int tloam_b200_frontier_cells(tloam_b200_handle* h, size_t* offsets, int* ij, double* xy, size_t capacity);
+/* inspection: the last search's label of every cell (width x height, the grid's layout): the id of its frontier before
+ * the filter, 0xFFFFFFFF for a cell that is not a frontier cell; synchronises.  NOT_READY before any search.
+ * INVALID_ARG: capacity < width x height. */
+int tloam_b200_frontier_labels(tloam_b200_handle* h, unsigned* labels, size_t capacity);
+
 /* ---- Global registration (opt-in): two clouds aligned with no initial guess, by FPFH features (Rusu 2009, as PCL and
  * Open3D define them), mutual matches, a RANSAC search and a truncated-least-squares refinement.  The result is meant as
  * the guess of tloam_b200_loop_verify* and tloam_b200_localize*.  Every device operation is FP64 and separately rounded

@@ -22,7 +22,8 @@
 // relocalizeFrame find the first pose in that map (or the pose after tracking is lost) from a recorded session's places;
 // enableMapUpdate / addMapUpdateFrame / buildUpdatedMap keep that map up to date from the localized frames.
 // enableOccupancy / occupancyGrid give a 2D occupancy grid of the map; distanceField / queryDistance its distance field
-// and inflated costmap, or those of a saved grid; planPotential / planPaths plan paths on that costmap.
+// and inflated costmap, or those of a saved grid; planPotential / planPaths plan paths on that costmap; frontiers finds
+// the exploration frontiers on it, ranked by the plan.
 // enableGlobalRegistration / globalRegister / globalRegisterLoop align two clouds, or two loop keyframes, with no initial
 // guess: the guess for verifyLoop's ICP or for localizeFrame.
 // Without the reference headers (this repository's tests) define TLOAM_B200_MOCK_HOST_TYPES and provide the host types
@@ -370,6 +371,25 @@ class FrontEndB200 {
     paths_xy.assign(n, std::vector<double>());
     for (size_t s = 0; s < n; ++s)
       paths_xy[s].assign(xy.begin() + 2 * offsets[s], xy.begin() + 2 * offsets[s + 1]);
+    return true;
+  }
+
+  // Frontiers (include/tloam_b200.h "Frontiers") of the last distanceField, ranked by the last planPotential (built with
+  // its goal at the robot): the kept frontiers in rank order and each one's cell centres as x, y pairs.  The route to a
+  // frontier is planPaths from its approach cell, reversed.
+  bool frontiers(const tloam_frontier_config& cfg, std::vector<tloam_frontier>& out,
+                 std::vector<std::vector<double>>& cells_xy, tloam_frontier_info& info) {
+    if (!report(tloam_b200_frontier_search(h_, &cfg, &info), "frontiers")) return false;
+    out.resize(info.kept);
+    if (!report(tloam_b200_frontier_download(h_, out.data(), out.size()), "frontiers")) return false;
+    size_t m = 0;
+    for (const tloam_frontier& f : out) m += f.size;
+    std::vector<size_t> offsets(info.kept + 1);
+    std::vector<double> xy(2 * m);
+    if (!report(tloam_b200_frontier_cells(h_, offsets.data(), nullptr, xy.data(), m), "frontiers")) return false;
+    cells_xy.assign(info.kept, std::vector<double>());
+    for (size_t k = 0; k < info.kept; ++k)
+      cells_xy[k].assign(xy.begin() + 2 * offsets[k], xy.begin() + 2 * offsets[k + 1]);
     return true;
   }
 

@@ -5,7 +5,7 @@ include/tloam_b200.h).  This package is only the Python host-side mirror of the 
 synthetic-scene generator used by tests and bench.py.  Importing it never touches oracle/.
 """
 from .occupancy import save_occupancy_map  # noqa: F401
-from .registration import (BatchRegistration, DistanceField, Frame, GlobalRegistrationResult, LocalRegistration,  # noqa: F401
-                           LoopResult, LoopVerifyResult,
+from .registration import (BatchRegistration, DistanceField, Frame, Frontier, GlobalRegistrationResult,  # noqa: F401
+                           LocalRegistration, LoopResult, LoopVerifyResult,
                            OccupancyGrid, PlanField, PlanPath, PoseGraphResult, PoseGraphRobustResult, RegistrationError,
                            default_config, packed_scan, packed_time)

@@ -200,6 +200,30 @@ class GlobalRegistrationResult(C.Structure):
                 ("accepted", C.c_int)]
 
 
+class FrontierConfig(C.Structure):
+    """tloam_frontier_config (include/tloam_b200.h "Frontiers")."""
+    _fields_ = [("free_max", C.c_uint), ("min_frontier_size", C.c_double), ("potential_scale", C.c_double),
+                ("gain_scale", C.c_double)]
+
+
+class FrontierRecord(C.Structure):
+    """tloam_frontier: one kept frontier of a search."""
+    _fields_ = [("id", C.c_uint), ("status", C.c_int), ("size", C.c_size_t), ("sum_i", C.c_ulonglong),
+                ("sum_j", C.c_ulonglong), ("min_i", C.c_size_t), ("min_j", C.c_size_t), ("max_i", C.c_size_t),
+                ("max_j", C.c_size_t), ("centroid_x", C.c_double), ("centroid_y", C.c_double),
+                ("approach_i", C.c_size_t), ("approach_j", C.c_size_t), ("approach_x", C.c_double),
+                ("approach_y", C.c_double), ("approach_potential", C.c_ulonglong), ("distance", C.c_double),
+                ("cost", C.c_double)]
+
+
+class FrontierInfo(C.Structure):
+    """tloam_frontier_info: the grid, the plan's goal cell, the frontier cells, the frontiers before and after the filter
+    and the kept reachable ones."""
+    _fields_ = [("origin_x", C.c_double), ("origin_y", C.c_double), ("resolution", C.c_double), ("width", C.c_size_t),
+                ("height", C.c_size_t), ("goal_i", C.c_size_t), ("goal_j", C.c_size_t), ("cells", C.c_size_t),
+                ("components", C.c_size_t), ("kept", C.c_size_t), ("reachable", C.c_size_t)]
+
+
 class PoseGraphConfig(C.Structure):
     """tloam_pose_graph_config (include/tloam_b200.h "Pose graph"): the edges' sigmas and the Gauss-Newton schedule."""
     _fields_ = [("sigma_odom_translation", C.c_double), ("sigma_odom_rotation", C.c_double),
@@ -352,6 +376,8 @@ EXPORTS = [
     "tloam_b200_distance_download", "tloam_b200_distance_query",
     "tloam_b200_plan_default_config", "tloam_b200_plan_build", "tloam_b200_plan_download", "tloam_b200_plan_paths",
     "tloam_b200_plan_path_cells",
+    "tloam_b200_frontier_default_config", "tloam_b200_frontier_search", "tloam_b200_frontier_download",
+    "tloam_b200_frontier_cells", "tloam_b200_frontier_labels",
     "tloam_b200_global_registration_default_config", "tloam_b200_global_registration_enable", "tloam_b200_global_register",
     "tloam_b200_global_register_loop", "tloam_b200_global_registration_side", "tloam_b200_global_registration_correspondences",
     "tloam_b200_global_registration_hypotheses",
@@ -609,6 +635,12 @@ def load():
     L.tloam_b200_plan_paths.argtypes = [vp, dp, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_int),
                                         C.POINTER(C.c_ulonglong)]
     L.tloam_b200_plan_path_cells.argtypes = [vp, C.POINTER(C.c_int), dp, C.c_size_t]
+    L.tloam_b200_frontier_default_config.argtypes = [C.POINTER(FrontierConfig)]
+    L.tloam_b200_frontier_default_config.restype = None
+    L.tloam_b200_frontier_search.argtypes = [vp, C.POINTER(FrontierConfig), C.POINTER(FrontierInfo)]
+    L.tloam_b200_frontier_download.argtypes = [vp, C.POINTER(FrontierRecord), C.c_size_t]
+    L.tloam_b200_frontier_cells.argtypes = [vp, C.POINTER(C.c_size_t), C.POINTER(C.c_int), dp, C.c_size_t]
+    L.tloam_b200_frontier_labels.argtypes = [vp, C.POINTER(C.c_uint), C.c_size_t]
     L.tloam_b200_global_registration_default_config.argtypes = [C.POINTER(GlobalRegistrationConfig)]
     L.tloam_b200_global_registration_default_config.restype = None
     L.tloam_b200_global_registration_enable.argtypes = [vp, C.POINTER(GlobalRegistrationConfig)]

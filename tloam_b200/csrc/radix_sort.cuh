@@ -1,12 +1,13 @@
 // radix_sort.cuh -- the stable LSD radix sort of 64-bit keys with a u32 row payload, and the scan of the sorted keys'
-// heads (hand-written CUDA for sm_90a).  Shared by libtloam_b200_gmm.so (map_merge.cu, the merged map's voxels) and
-// libtloam_b200_loc.so (localize.cu, the prior map's cells), so that both order rows by the same rule:
+// heads (hand-written CUDA for sm_90a).  Shared by libtloam_b200_gmm.so (map_merge.cu, the merged map's voxels),
+// libtloam_b200_loc.so (localize.cu, the prior map's cells), libtloam_b200_mapu.so (map_update.cu) and
+// libtloam_b200_frontier.so (frontier.cu, each frontier's cells), so that all order rows by the same rule:
 //   k_gmm_hist     \
 //   k_gmm_offsets   |   one pass per 8-bit digit: per-tile digit counts, per-digit offsets, a stable scatter; rows with
 //   k_gmm_scatter  /    equal keys stay in row order
 //   k_gmm_head_count \  the positions whose key differs from the previous one, numbered in order: the j-th distinct
 //   k_gmm_head_scatter/ key's first position at start[j], their count in st->n_vox and start[count] = n
-// The kernels keep the names the merge gave them.  This header is included by those two libraries only; including it in
+// The kernels keep the names the merge gave them.  This header is included by those libraries only; including it in
 // libtloam_b200.so would add its kernels there.
 #pragma once
 #include <cuda_runtime.h>

@@ -44,6 +44,7 @@
 #include "distance.h"
 #include "plan.h"
 #include "global_registration.h"
+#include "frontier.h"
 
 
 
@@ -258,6 +259,7 @@ struct tloam_b200_handle {
   unsigned long long* d_dist_small = nullptr;                                                  // the obstacle count
   double* d_dist_q = nullptr;              size_t cap_dist_q = 0;                              // points: xy, distance, gradient
   bool dist_built = false;                 tloam_distance_info dist_info;
+  unsigned long long dist_serial = 0;                                                          // successful builds
   // ---- the plan (tloam_b200_plan*, libtloam_b200_plan.so): the last build's cells (P 8, t 2: 10 B each), the tile
   //      stamps and the two worklists (12 B per tile), the worklists' state, the last paths' starts and outputs (24 B per
   //      start) and cells (8 B each); allocated by the first call that needs them, grown only ----
@@ -268,6 +270,17 @@ struct tloam_b200_handle {
   int* d_plan_cells = nullptr;             size_t cap_plan_cells = 0;                          // path cells of the buffer
   bool plan_built = false;                 tloam_plan_info plan_info;
   bool plan_paths_kept = false;            size_t plan_path_total = 0;                         // cells of the last paths
+  unsigned long long plan_serial = 0;      tloam_plan_config plan_cfg;                         // the field it was built on
+  // ---- the frontiers (tloam_b200_frontier*, libtloam_b200_frontier.so): per cell the label (4 B), per tile a flag, the
+  //      compaction's block counts and the state; per frontier cell the radix sort's keys and rows (24 B), its
+  //      histograms and the heads (4 B); per frontier 64 B of statistics.  Allocated by the first search that needs
+  //      them, grown only; the ranked frontiers on the host ----
+  unsigned* d_fr_labels = nullptr;         size_t cap_fr_labels = 0;                           // cells of the buffer
+  unsigned char* d_fr_tiles = nullptr;     size_t cap_fr_tiles = 0;
+  unsigned char* d_fr_small = nullptr;                                                         // block counts, state
+  unsigned char* d_fr_sort = nullptr;      size_t cap_fr_sort = 0;                             // frontier cells of it
+  bool fr_kept = false;                    tloam_frontier_info fr_info;
+  std::vector<tloam_frontier> fr_ranked;   unsigned fr_sorted = 0;                             // row buffer of the cells
   // ---- the merged map (tloam_b200_global_map_merge*, libtloam_b200_gmm.so): the radix sort's scratch (24 B per map row)
   //      and the last merge's voxels (32 B each), allocated by the first merge and grown; the snapshot is dropped by
   //      enable / reset and by the next merge ----
@@ -595,6 +608,7 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   cudaFree(h->d_occ_scans); cudaFree(h->d_occ_poses); cudaFree(h->d_occ_dirs); cudaFree(h->d_occ_grid); cudaFree(h->d_occ_small);
   cudaFree(h->d_dist); cudaFree(h->d_dist_bands); cudaFree(h->d_dist_table); cudaFree(h->d_dist_small); cudaFree(h->d_dist_q);
   cudaFree(h->d_plan); cudaFree(h->d_plan_tiles); cudaFree(h->d_plan_state); cudaFree(h->d_plan_q); cudaFree(h->d_plan_cells);
+  cudaFree(h->d_fr_labels); cudaFree(h->d_fr_tiles); cudaFree(h->d_fr_small); cudaFree(h->d_fr_sort);
   cudaFree(h->d_gmm_scratch); cudaFree(h->d_gmm_out);
   cudaFree(h->d_loc_map); cudaFree(h->d_loc_scratch); cudaFree(h->d_loc_qst); cudaFree(h->d_loc_reg); cudaFree(h->d_loc_fin);
   cudaFree(h->d_loc_q); cudaFree(h->d_loc_in); cudaFree(h->d_loc_run);
@@ -5634,6 +5648,7 @@ static int dist_run(tloam_b200_handle* h, const DistLib& lib, const tloam_distan
   }
   h->dist_info = out;
   h->dist_built = true;
+  ++h->dist_serial;
   if (info) *info = out;
   return TLOAM_B200_OK;
 }
@@ -5866,6 +5881,8 @@ int tloam_b200_plan_build(tloam_b200_handle* h, const tloam_plan_config* cfg, do
   out.rounds = st.rounds; out.tiles = st.tiles;
   h->plan_info = out;
   h->plan_built = true;
+  h->plan_serial = h->dist_serial;
+  h->plan_cfg = *cfg;
   if (info) *info = out;
   return TLOAM_B200_OK;
 }
@@ -5973,6 +5990,233 @@ int tloam_b200_plan_path_cells(tloam_b200_handle* h, int* ij, double* xy, size_t
     for (size_t k = 0; k < 2 * m; ++k)        // the centre, each operation rounded on its own
       xy[k] = (k % 2 ? f.origin_y : f.origin_x) + ((double)dst[k] + 0.5) * f.resolution;
   }
+  return TLOAM_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Frontiers (the checks, the buffers, the cost, the filter and the order here; the kernels in frontier.cu, loaded from
+// libtloam_b200_frontier.so by the first frontier call, so that the kernels of this library keep their SASS).
+// ---------------------------------------------------------------------------------------------
+struct FrontierLib {
+  tloam_fr_fn label = nullptr; tloam_fr_fn group = nullptr;
+  tloam_fr_sort_bytes_fn sort_bytes = nullptr; tloam_fr_sort_layout_fn sort_layout = nullptr;
+};
+static std::mutex g_fr_mu;
+static FrontierLib g_fr;
+
+static int fr_load(tloam_b200_handle* h, FrontierLib* out) {
+  std::lock_guard<std::mutex> lk(g_fr_mu);
+  if (!g_fr.label) {
+    const std::string path = sibling_path("libtloam_b200_frontier.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    FrontierLib l;
+    if (so) {
+      l.label = reinterpret_cast<tloam_fr_fn>(dlsym(so, "tloam_fr_label"));
+      l.group = reinterpret_cast<tloam_fr_fn>(dlsym(so, "tloam_fr_group"));
+      l.sort_bytes = reinterpret_cast<tloam_fr_sort_bytes_fn>(dlsym(so, "tloam_fr_sort_bytes"));
+      l.sort_layout = reinterpret_cast<tloam_fr_sort_layout_fn>(dlsym(so, "tloam_fr_sort_layout"));
+    }
+    if (!l.label || !l.group || !l.sort_bytes || !l.sort_layout) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "frontiers: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_fr = l;
+  }
+  *out = g_fr;
+  return TLOAM_B200_OK;
+}
+
+static int fr_status(tloam_b200_handle* h, int e, const char* where) {
+  if (e == cudaSuccess) return TLOAM_B200_OK;
+  snprintf(h->last_error, sizeof(h->last_error), "frontiers: %s: %s", where, cudaGetErrorString((cudaError_t)e));
+  return TLOAM_B200_ERR_CUDA;
+}
+
+void tloam_b200_frontier_default_config(tloam_frontier_config* c) {
+  c->free_max = 252;                       // every cell a plan can enter
+  c->min_frontier_size = 0.5;              // explore_lite's defaults; robot parameters, not calibrated
+  c->potential_scale = 3.0;
+  c->gain_scale = 1.0;
+}
+
+static bool fr_config_valid(const tloam_frontier_config* c) {
+  const auto ok = [](double v) { return std::isfinite(v) && v >= 0.0; };
+  return c->free_max <= 252 && ok(c->min_frontier_size) && ok(c->potential_scale) && ok(c->gain_scale);
+}
+
+int tloam_b200_frontier_search(tloam_b200_handle* h, const tloam_frontier_config* cfg, tloam_frontier_info* info) {
+  if (!h || !cfg || !fr_config_valid(cfg)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->dist_built || !h->plan_built || h->plan_serial != h->dist_serial) return TLOAM_B200_ERR_NOT_READY;
+  FrontierLib lib;
+  int rc = fr_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  h->fr_kept = false;
+  const tloam_plan_info& f = h->plan_info;
+  const size_t n = f.width * f.height;     // >= 1: a plan has a goal cell
+  const size_t ntiles = ((f.width + TLOAM_FR_TILE - 1) / TLOAM_FR_TILE) * ((f.height + TLOAM_FR_TILE - 1) / TLOAM_FR_TILE);
+  if (n > h->cap_fr_labels) {
+    cudaFree(h->d_fr_labels); h->d_fr_labels = nullptr; h->cap_fr_labels = 0;
+    CU_TRY(cudaMalloc(&h->d_fr_labels, n * sizeof(unsigned)));
+    h->cap_fr_labels = n;
+  }
+  if (ntiles > h->cap_fr_tiles) {
+    cudaFree(h->d_fr_tiles); h->d_fr_tiles = nullptr; h->cap_fr_tiles = 0;
+    CU_TRY(cudaMalloc(&h->d_fr_tiles, ntiles));
+    h->cap_fr_tiles = ntiles;
+  }
+  const size_t small_state = TLOAM_FR_BLOCKS * sizeof(unsigned);
+  if (!h->d_fr_small) CU_TRY(cudaMalloc(&h->d_fr_small, small_state + sizeof(tloam_fr_state)));
+  tloam_fr_args a;
+  memset(&a, 0, sizeof(a));
+  a.costs = h->d_dist + 17 * h->cap_dist;
+  a.P = reinterpret_cast<const unsigned long long*>(h->d_plan);
+  a.width = (unsigned)f.width; a.height = (unsigned)f.height;
+  a.free_max = cfg->free_max;
+  a.labels = h->d_fr_labels;
+  a.tile_any = h->d_fr_tiles;
+  a.block_counts = reinterpret_cast<unsigned*>(h->d_fr_small);
+  a.state = reinterpret_cast<tloam_fr_state*>(h->d_fr_small + small_state);
+  a.device = h->device; a.stream = h->stream;
+  int e = 0, launches = 0;
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.label(&a, &launches)));
+  h->launches += launches > 0 ? launches - 1 : 0;
+  if ((rc = fr_status(h, e, "k_fr_tile / _border / _flatten")) != TLOAM_B200_OK) return rc;
+  tloam_fr_state st;
+  CU_TRY(cudaMemcpyAsync(&st, a.state, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  const size_t m = (size_t)st.cells;
+  size_t components = 0;
+  std::vector<tloam_fr_stat> stats;
+  if (m) {
+    if (m > h->cap_fr_sort) {
+      cudaFree(h->d_fr_sort); h->d_fr_sort = nullptr; h->cap_fr_sort = 0;
+      CU_TRY(cudaMalloc(&h->d_fr_sort, lib.sort_bytes(m)));
+      h->cap_fr_sort = m;
+    }
+    lib.sort_layout(h->d_fr_sort, h->cap_fr_sort, &a);
+    a.cells = m;
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.group(&a, &launches)));
+    h->launches += launches > 0 ? launches - 1 : 0;
+    if ((rc = fr_status(h, e, "k_fr_compact / radix sort / heads / k_fr_stats")) != TLOAM_B200_OK) return rc;
+    CU_TRY(cudaMemcpyAsync(&st, a.state, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    components = (size_t)st.gmm.n_vox;
+    stats.resize(components);
+    CU_TRY(cudaMemcpyAsync(stats.data(), a.stats, components * sizeof(tloam_fr_stat), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+  }
+  // the cost of each kept frontier in FP64, each operation rounded on its own; then the order
+  const double res = f.resolution;
+  const double per_m = 70.0 * (double)h->plan_cfg.neutral_cost;
+  std::vector<tloam_frontier> kept;
+  for (size_t j = 0; j < components; ++j) {
+    const tloam_fr_stat& s = stats[j];
+    const double size_m = (double)s.n * res;
+    if (!(size_m >= cfg->min_frontier_size)) continue;
+    tloam_frontier o;
+    memset(&o, 0, sizeof(o));
+    o.id = (unsigned)j;
+    o.size = s.n;
+    o.sum_i = s.sum_i; o.sum_j = s.sum_j;
+    o.min_i = s.min_i; o.min_j = s.min_j; o.max_i = s.max_i; o.max_j = s.max_j;
+    o.centroid_x = f.origin_x + ((double)s.sum_i / (double)s.n + 0.5) * res;
+    o.centroid_y = f.origin_y + ((double)s.sum_j / (double)s.n + 0.5) * res;
+    o.approach_i = s.approach % f.width; o.approach_j = s.approach / f.width;
+    o.approach_x = f.origin_x + ((double)o.approach_i + 0.5) * res;
+    o.approach_y = f.origin_y + ((double)o.approach_j + 0.5) * res;
+    o.approach_potential = s.approach_p;
+    o.status = s.approach_p == TLOAM_PLAN_INF ? 1 : 0;
+    if (o.status == 0) {
+      o.distance = ((double)s.approach_p / per_m) * res;
+      const double pot = cfg->potential_scale * o.distance;
+      const double gain = cfg->gain_scale * size_m;
+      o.cost = pot - gain;
+    } else {
+      o.distance = o.cost = HUGE_VAL;
+    }
+    kept.push_back(o);
+  }
+  // reachable by (cost, id), a NaN cost after every number; then unreachable by id
+  std::stable_sort(kept.begin(), kept.end(), [](const tloam_frontier& x, const tloam_frontier& y) {
+    if (x.status != y.status) return x.status < y.status;
+    if (x.status == 1) return false;
+    const bool xn = std::isnan(x.cost), yn = std::isnan(y.cost);
+    if (xn != yn) return yn;
+    return !xn && x.cost < y.cost;
+  });
+  tloam_frontier_info out;
+  memset(&out, 0, sizeof(out));
+  out.origin_x = f.origin_x; out.origin_y = f.origin_y; out.resolution = res;
+  out.width = f.width; out.height = f.height;
+  out.goal_i = f.goal_i; out.goal_j = f.goal_j;
+  out.cells = m; out.components = components; out.kept = kept.size();
+  for (const tloam_frontier& o : kept) out.reachable += o.status == 0 ? 1 : 0;
+  h->fr_ranked.swap(kept);
+  h->fr_info = out;
+  h->fr_sorted = (unsigned)(tloam_fr_passes(n) & 1);
+  h->fr_kept = true;
+  if (info) *info = out;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_frontier_download(tloam_b200_handle* h, tloam_frontier* out, size_t capacity) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->fr_kept) return TLOAM_B200_ERR_NOT_READY;
+  if (capacity < h->fr_ranked.size()) return TLOAM_B200_ERR_INVALID_ARG;
+  if (out) std::copy(h->fr_ranked.begin(), h->fr_ranked.end(), out);
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_frontier_cells(tloam_b200_handle* h, size_t* offsets, int* ij, double* xy, size_t capacity) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->fr_kept) return TLOAM_B200_ERR_NOT_READY;
+  const std::vector<tloam_frontier>& R = h->fr_ranked;
+  std::vector<size_t> off(R.size() + 1, 0);
+  for (size_t k = 0; k < R.size(); ++k) off[k + 1] = off[k] + R[k].size;
+  if (capacity < off.back()) return TLOAM_B200_ERR_INVALID_ARG;
+  if (offsets) std::copy(off.begin(), off.end(), offsets);
+  if (off.back() && (ij || xy)) {
+    // the sorted cells and the heads of the last search, each kept frontier's run copied in rank order
+    const tloam_frontier_info& f = h->fr_info;
+    tloam_fr_args a;
+    memset(&a, 0, sizeof(a));
+    FrontierLib lib;
+    int rc = fr_load(h, &lib);
+    if (rc != TLOAM_B200_OK) return rc;
+    lib.sort_layout(h->d_fr_sort, h->cap_fr_sort, &a);
+    CU_TRY(cudaSetDevice(h->device));
+    std::vector<unsigned> start(f.components + 1), rows(f.cells);
+    CU_TRY(cudaMemcpyAsync(start.data(), a.start, start.size() * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaMemcpyAsync(rows.data(), a.row[h->fr_sorted], rows.size() * sizeof(unsigned), cudaMemcpyDeviceToHost,
+                           h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    for (size_t k = 0; k < R.size(); ++k) {
+      const unsigned lo = start[R[k].id];
+      for (size_t q = 0; q < R[k].size; ++q) {
+        const unsigned c = rows[lo + q];
+        const size_t i = c % f.width, j = c / f.width, o = 2 * (off[k] + q);
+        if (ij) { ij[o] = (int)i; ij[o + 1] = (int)j; }
+        if (xy) {                        // the centre, each operation rounded on its own
+          xy[o] = f.origin_x + ((double)i + 0.5) * f.resolution;
+          xy[o + 1] = f.origin_y + ((double)j + 0.5) * f.resolution;
+        }
+      }
+    }
+  }
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_frontier_labels(tloam_b200_handle* h, unsigned* labels, size_t capacity) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->fr_kept) return TLOAM_B200_ERR_NOT_READY;
+  const size_t n = h->fr_info.width * h->fr_info.height;
+  if (capacity < n) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  if (labels) CU_TRY(cudaMemcpyAsync(labels, h->d_fr_labels, n * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
   return TLOAM_B200_OK;
 }
 

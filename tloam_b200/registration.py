@@ -258,6 +258,28 @@ class PlanPath:
 
 
 @dataclasses.dataclass(frozen=True)
+class Frontier:
+    """one kept frontier of a search (include/tloam_b200.h "Frontiers"), in rank order: id = its number before the filter
+    (ascending least cell index), size = cells, sums = (Si, Sj) of its cells' i and j, bbox = (min_i, min_j, max_i,
+    max_j), centroid = (x, y) m, approach = the approach cell (i, j), approach_xy its centre, approach_potential = the
+    plan's P there, status 0 reachable or 1 unreachable, distance = m of free-cell path and cost (+inf when unreachable),
+    cells (size, 2) int32 (i, j) ascending by linear index and xy (size, 2) their centres."""
+    id: int
+    size: int
+    sums: tuple
+    bbox: tuple
+    centroid: tuple
+    approach: tuple
+    approach_xy: tuple
+    approach_potential: int
+    status: int
+    distance: float
+    cost: float
+    cells: np.ndarray
+    xy: np.ndarray
+
+
+@dataclasses.dataclass(frozen=True)
 class OccupancyGrid:
     """a built occupancy grid (include/tloam_b200.h "Occupancy grid"): cells (height, width) int8 in nav_msgs/OccupancyGrid's
     values (-1 unknown, 0 .. 100), row j along y and column i along x, with the counts it came from (uint32 each); origin
@@ -1658,6 +1680,46 @@ class LocalRegistration:
                     "plan_path_cells")
         return [PlanPath(ij[offsets[s]:offsets[s + 1]], xy[offsets[s]:offsets[s + 1]], int(costs[s]), int(statuses[s]))
                 for s in range(n)]
+
+    # ---- frontiers (include/tloam_b200.h "Frontiers") ----
+    def frontier_search(self, **overrides):
+        """the frontiers of the last distance_build, ranked by the last plan_build (build it with its goal at the robot);
+        overrides: fields of tloam_frontier_config (free_max, min_frontier_size, potential_scale, gain_scale).  Returns
+        (info, frontiers): info a dict of tloam_frontier_info's fields, frontiers the kept ones in rank order."""
+        cfg = _lib.FrontierConfig()
+        self._L.tloam_b200_frontier_default_config(C.byref(cfg))
+        for k, v in overrides.items():
+            if not any(f[0] == k for f in cfg._fields_):
+                raise TypeError(f"unknown frontier field {k!r}")
+            setattr(cfg, k, v)
+        info = _lib.FrontierInfo()
+        self._check(self._L.tloam_b200_frontier_search(self._h, C.byref(cfg), C.byref(info)), "frontier_search")
+        recs = (_lib.FrontierRecord * max(info.kept, 1))()
+        self._check(self._L.tloam_b200_frontier_download(self._h, recs, info.kept), "frontier_download")
+        offsets = np.zeros(info.kept + 1, dtype=np.uintp)
+        m = sum(recs[k].size for k in range(info.kept))
+        ij = np.zeros((m, 2), dtype=np.int32)
+        xy = np.zeros((m, 2))
+        self._check(self._L.tloam_b200_frontier_cells(self._h, offsets.ctypes.data_as(C.POINTER(C.c_size_t)),
+                                                      ij.ctypes.data_as(C.POINTER(C.c_int)), _dp(xy), m), "frontier_cells")
+        out = []
+        for k in range(info.kept):
+            r = recs[k]
+            a, b = int(offsets[k]), int(offsets[k + 1])
+            out.append(Frontier(r.id, r.size, (r.sum_i, r.sum_j), (r.min_i, r.min_j, r.max_i, r.max_j),
+                                (r.centroid_x, r.centroid_y), (r.approach_i, r.approach_j), (r.approach_x, r.approach_y),
+                                r.approach_potential, r.status, r.distance, r.cost, ij[a:b], xy[a:b]))
+        self._frontier_shape = (info.height, info.width)
+        return {name: getattr(info, name) for name, _ in info._fields_}, out
+
+    def frontier_labels(self):
+        """the last frontier_search's label of every cell, (height, width) uint32: its frontier's id before the filter,
+        0xFFFFFFFF elsewhere"""
+        shape = getattr(self, "_frontier_shape", (0, 0))
+        lab = np.zeros(shape, dtype=np.uint32)
+        self._check(self._L.tloam_b200_frontier_labels(self._h, lab.ctypes.data_as(C.POINTER(C.c_uint)), lab.size),
+                    "frontier_labels")
+        return lab
 
     def localize_set_map_updated(self):
         """load the last map_update_build on the device as the prior map"""
