@@ -1722,6 +1722,116 @@ int tloam_b200_frontier_cells(tloam_b200_handle* h, size_t* offsets, int* ij, do
  * INVALID_ARG: capacity < width x height. */
 int tloam_b200_frontier_labels(tloam_b200_handle* h, unsigned* labels, size_t capacity);
 
+/* ---- Terrain: a 2.5D traversability map of a cloud (the elevation-map layers of grid_map / elevation_mapping): per cell
+ * the ground reference, the elevation, the step, the slope and the roughness, and a nav_msgs/OccupancyGrid value, so
+ * that the distance build, the planner and the frontier search see kerbs, drop-offs and steep ramps that the occupancy
+ * grid's obstacle band passes over.
+ *   - Source cloud C.  tloam_b200_terrain_build: the global map as it stands in stream order (after every enqueued append
+ *     and correction), all rows, or with static_only the rows tloam_b200_global_map_static_download keeps (the merge's
+ *     rule and counters); a correction moves the terrain with the map.  tloam_b200_terrain_build_cloud: a host cloud
+ *     (n x 3 FP64, such as a saved merged map or a prior map), with mapping on or off.  Rows with a non-finite
+ *     coordinate are skipped and counted.  The map's rows are per-frame voxel centroids: its voxel should be at most the
+ *     terrain's resolution (the reference's 1 m map gives a 1 m-scale terrain).
+ *   - Grid (the occupancy grid's conventions: nav_msgs/OccupancyGrid layout, row-major, i along x, the origin at the
+ *     corner of cell (0, 0)).  Over the finite rows of C: origin = resolution floor(min / resolution) per axis (on the
+ *     ordered encodings, -0.0 below +0.0), width = floor((max - origin) / resolution) + 1; a grid of more than 2^28 cells
+ *     is refused (VOXEL_RANGE) and an empty selection gives a 0 x 0 grid.  With combine_occupancy the geometry (origin,
+ *     resolution, width, height) is the last tloam_b200_occupancy_build's instead.  A row's cell is
+ *     (floor((x - ox) / res), floor((y - oy) / res)), the subtraction and the division each rounded on its own; a row whose
+ *     cell lies outside the grid is dropped and counted.
+ *   - Radii.  rg, rs, rp = (unsigned) ceil(radius / resolution) of ground_radius, step_radius, slope_radius, on the host.
+ *     W_r(c) is the (2r + 1)^2 window of c, clipped to the grid.
+ *   - Layers, per cell c.  Every FP64 operation is rounded on its own (no FMA), left to right as written; every extremum
+ *     is taken on the ordered 64-bit encoding of the doubles, so -0.0 orders below +0.0:
+ *       1. zlo(c), the least z of c's rows; n(c) their count.
+ *       2. G(c) = the least zlo over W_rg(c): the ground reference, +inf when the window has no row.
+ *       3. The ground-side rows of c are its rows with z <= G(c) + clearance; the others are overhangs (a bridge, a
+ *          canopy), left out and counted.  e(c), the elevation, is the largest z of the ground-side rows, m(c) their count.
+ *          c is known iff m(c) >= min_points.
+ *       4. step(c) (known c) = the largest e minus the least e over the known cells of W_rs(c).
+ *       5. The plane w = a u + b v + d fitted by least squares over the known cells k of W_rp(c): u, v the integer cell
+ *          offsets of k from c and w = e(k) - e(c).  The sums run over the window with dj outer and di inner, both
+ *          ascending: the integer moments N, Su, Sv, Suu, Suv, Svv exactly, and from +0.0 Sw = Sw + w, Suw = Suw + u w,
+ *          Svw = Svw + v w.  With the exact integer cofactors C11 = Svv N - Sv Sv, C12 = Sv Su - Suv N, C13 = Suv Sv - Svv Su,
+ *          C22 = Suu N - Su Su, C23 = Suv Su - Suu Sv, C33 = Suu Svv - Suv Suv and D = Suu C11 + Suv C12 + Su C13 (each
+ *          converted to FP64 exactly): a = ((C11 Suw + C12 Svw) + C13 Sw) / D, b = ((C12 Suw + C22 Svw) + C23 Sw) / D,
+ *          d = ((C13 Suw + C23 Svw) + C33 Sw) / D.  slope(c) = sqrt(a a + b b) / resolution (m per m), defined iff
+ *          N >= min_fit and D != 0, NaN otherwise.  roughness(c) = the largest |w - ((a u + b v) + d)| over the fit's
+ *          cells (from +0.0), NaN when the slope is.
+ *       6. A known cell is lethal iff step > max_step, or slope > tan(max_slope), or roughness > max_roughness (a NaN
+ *          comparison is false).  The host computes tan(max_slope) with std::tan; no transcendental runs on the device.
+ *       7. The value (int8): 100 lethal, 0 traversable, -1 not known.  With combine_occupancy it combines with the last
+ *          occupancy build's value o of the cell: 100 if the terrain value is 100 or o >= 65; else 0 if the terrain value
+ *          is 0 or 0 <= o <= 25; else -1.  The grid then knows the occupancy grid's ray-cast free space and the terrain's
+ *          ground geometry.  The values are map_server's classes: tloam_b200.save_occupancy_map saves them as they are.
+ *   - Costmap.  tloam_b200_distance_build_terrain runs the distance build ("Distance field and costmap") on the last
+ *     terrain build's values on the device; tloam_b200_plan_build and tloam_b200_frontier_search then work on it as on any
+ *     distance build.
+ *   - Limits (INVALID_ARG otherwise): resolution finite and > 0; clearance, the radii and the three thresholds finite and
+ *     >= 0; max_slope < pi / 2; rs, rp <= 16 and rg <= 1024 cells; min_points, min_fit >= 1; static_only only with the
+ *     map source.  NOT_READY: mapping off for the map source, static_only with removal off, or combine_occupancy with no
+ *     occupancy build.  VOXEL_RANGE: the grid limit.
+ *   - Lifetime.  A build is a snapshot: later appends, corrections, resets and occupancy builds leave it alone; the next
+ *     build replaces it (a build refused with INVALID_ARG, NOT_READY or VOXEL_RANGE keeps it) and tloam_b200_destroy
+ *     frees it.
+ *   - Unchanged.  Nothing is hooked into any other call: the map, its counters, the occupancy grid, the distance field
+ *     (until tloam_b200_distance_build_terrain), the plan, the frontiers and the launch counts of every other call keep
+ *     their bits, and nothing is allocated or loaded before the first terrain call.
+ *   - Device.  A build is k_ter_bounds and a read-back of the extent (not when combining), then k_ter_low (one thread per
+ *     row: atomicMax of the complemented encoding of z, and the count), k_ter_ground twice (the window max along x, then
+ *     along y), k_ter_high (one thread per row: atomicMax of the ground-side rows' encodings) and k_ter_layers (one block
+ *     per 32 x 32 tile with a halo of max(rs, rp) cells of the known elevations in shared memory: step, plane fit,
+ *     roughness, class, value), and a read-back of the counts; it synchronises.  The result does not depend on the
+ *     order of the atomics.  Memory: 65 B per cell (four 8 B encodings, two 4 B counts, three FP64 layers and the value)
+ *     and, for a host cloud, 24 B per row, on the device, allocated by the first build that needs them, grown only and
+ *     freed by tloam_b200_destroy.
+ *   - The kernels live in libtloam_b200_terrain.so, loaded from this library's directory by the first terrain call; if
+ *     it is missing the calls return ERR_CUDA (tloam_b200_last_error names the file). */
+typedef struct tloam_terrain_config {
+  double resolution;                   /* m per cell; with combine_occupancy the occupancy grid's is used */
+  double clearance;                    /* m above G: rows higher up are overhangs */
+  double ground_radius;                /* m: the window of the ground reference */
+  double step_radius;                  /* m: the window of the step */
+  double slope_radius;                 /* m: the window of the plane fit */
+  double max_step;                     /* m */
+  double max_slope;                    /* rad */
+  double max_roughness;                /* m */
+  unsigned min_points;                 /* ground-side rows of a known cell */
+  unsigned min_fit;                    /* known cells of a defined plane fit */
+  int static_only;                     /* the map source's static rows only (tloam_b200_terrain_build) */
+  int combine_occupancy;               /* on the last occupancy build's grid, its values combined */
+} tloam_terrain_config;
+typedef struct tloam_terrain_info {
+  double origin_x, origin_y;           /* the corner of cell (0, 0), m */
+  double resolution;
+  size_t width, height;                /* cells along x and y */
+  unsigned ground_cells, step_cells, slope_cells;   /* rg, rs, rp */
+  size_t rows;                         /* rows of C, selected ones for static_only */
+  size_t used;                         /* finite rows in the grid */
+  size_t skipped;                      /* rows with a non-finite coordinate */
+  size_t dropped;                      /* finite rows outside the grid */
+  size_t overhang;                     /* used rows above G + clearance */
+  size_t known, lethal;                /* known cells and the lethal ones among them (before any combination) */
+  int combined;                        /* the values are combined with the occupancy grid's */
+} tloam_terrain_info;
+/* resolution 0.2 m, clearance 2.0 m, ground_radius 1.6 m, step_radius 0.3 m, slope_radius 0.4 m, max_step 0.10 m,
+ * max_slope 15 deg, max_roughness 0.10 m, min_points 1, min_fit 6, static_only 0, combine_occupancy 0: a car with an
+ * HDL-64E (robot parameters, not calibrated values; DESIGN.md §4c has what was measured with them) */
+void tloam_b200_terrain_default_config(tloam_terrain_config* c);
+/* the terrain of the global map; synchronises.  info may be null. */
+int tloam_b200_terrain_build(tloam_b200_handle* h, const tloam_terrain_config* cfg, tloam_terrain_info* info);
+/* the terrain of a host cloud xyz (n x 3 FP64; null only when n == 0); synchronises.  info may be null. */
+int tloam_b200_terrain_build_cloud(tloam_b200_handle* h, const tloam_terrain_config* cfg, const double* xyz, size_t n,
+                                   tloam_terrain_info* info);
+/* the layers of the last terrain build, width x height each in the grid's layout, each may be null: values (int8), ground
+ * G (+inf: no row in the window), elevation e (NaN where m = 0), step, slope and roughness (NaN where not known or not
+ * defined) and points m; synchronises.  NOT_READY before any build.  INVALID_ARG: capacity < width x height. */
+int tloam_b200_terrain_download(tloam_b200_handle* h, signed char* values, double* ground, double* elevation, double* step,
+                                double* slope, double* roughness, unsigned* points, size_t capacity);
+/* the distance field and costmap of the last terrain build's values (see tloam_b200_distance_build); NOT_READY before
+ * any terrain build. */
+int tloam_b200_distance_build_terrain(tloam_b200_handle* h, const tloam_distance_config* cfg, tloam_distance_info* info);
+
 /* ---- Global registration (opt-in): two clouds aligned with no initial guess, by FPFH features (Rusu 2009, as PCL and
  * Open3D define them), mutual matches, a RANSAC search and a truncated-least-squares refinement.  The result is meant as
  * the guess of tloam_b200_loop_verify* and tloam_b200_localize*.  Every device operation is FP64 and separately rounded

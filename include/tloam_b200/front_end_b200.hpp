@@ -23,7 +23,8 @@
 // enableMapUpdate / addMapUpdateFrame / buildUpdatedMap keep that map up to date from the localized frames.
 // enableOccupancy / occupancyGrid give a 2D occupancy grid of the map; distanceField / queryDistance its distance field
 // and inflated costmap, or those of a saved grid; planPotential / planPaths plan paths on that costmap; frontiers finds
-// the exploration frontiers on it, ranked by the plan.
+// the exploration frontiers on it, ranked by the plan.  terrainMap builds a traversability map of the map (or of a saved
+// cloud) that sees kerbs and drop-offs, and distanceFieldTerrain the costmap of it.
 // enableGlobalRegistration / globalRegister / globalRegisterLoop align two clouds, or two loop keyframes, with no initial
 // guess: the guess for verifyLoop's ICP or for localizeFrame.
 // Without the reference headers (this repository's tests) define TLOAM_B200_MOCK_HOST_TYPES and provide the host types
@@ -336,6 +337,24 @@ class FrontEndB200 {
     if (!report(tloam_b200_distance_build_grid(h_, &cfg, reinterpret_cast<const signed char*>(cells.data()), width, height,
                                                origin_x, origin_y, resolution, &info), "distanceField"))
       return false;
+    return downloadDistance(sd, costs, values, info);
+  }
+  // Terrain (include/tloam_b200.h "Terrain"): the traversability map of the global map (cloud empty) or of a saved cloud
+  // (n x 3, m), values in nav_msgs/OccupancyGrid's classes and the elevation (NaN without a ground-side row) and slope
+  // layers in the grid's layout; distanceFieldTerrain gives the costmap of those values for planPotential.
+  bool terrainMap(const tloam_terrain_config& cfg, const std::vector<double>& cloud, std::vector<int8_t>& values,
+                  std::vector<double>& elevation, std::vector<double>& slope, tloam_terrain_info& info) {
+    const int rc = cloud.empty() ? tloam_b200_terrain_build(h_, &cfg, &info)
+                                 : tloam_b200_terrain_build_cloud(h_, &cfg, cloud.data(), cloud.size() / 3, &info);
+    if (!report(rc, "terrainMap")) return false;
+    const size_t n = info.width * info.height;
+    values.resize(n); elevation.resize(n); slope.resize(n);
+    return report(tloam_b200_terrain_download(h_, reinterpret_cast<signed char*>(values.data()), nullptr, elevation.data(),
+                                              nullptr, slope.data(), nullptr, nullptr, n), "terrainMap");
+  }
+  bool distanceFieldTerrain(const tloam_distance_config& cfg, std::vector<float>& sd, std::vector<uint8_t>& costs,
+                            std::vector<int8_t>& values, tloam_distance_info& info) {
+    if (!report(tloam_b200_distance_build_terrain(h_, &cfg, &info), "distanceFieldTerrain")) return false;
     return downloadDistance(sd, costs, values, info);
   }
   // the last field's distance at the points xy (n x 2, m) and its gradient (n x 2), bilinear between the cell centres;

@@ -8,4 +8,4 @@ from .occupancy import save_occupancy_map  # noqa: F401
 from .registration import (BatchRegistration, DistanceField, Frame, Frontier, GlobalRegistrationResult,  # noqa: F401
                            LocalRegistration, LoopResult, LoopVerifyResult,
                            OccupancyGrid, PlanField, PlanPath, PoseGraphResult, PoseGraphRobustResult, RegistrationError,
-                           default_config, packed_scan, packed_time)
+                           TerrainMap, default_config, packed_scan, packed_time)

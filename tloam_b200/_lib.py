@@ -224,6 +224,22 @@ class FrontierInfo(C.Structure):
                 ("components", C.c_size_t), ("kept", C.c_size_t), ("reachable", C.c_size_t)]
 
 
+class TerrainConfig(C.Structure):
+    """tloam_terrain_config (include/tloam_b200.h "Terrain"): the grid, the windows and the thresholds."""
+    _fields_ = [("resolution", C.c_double), ("clearance", C.c_double), ("ground_radius", C.c_double),
+                ("step_radius", C.c_double), ("slope_radius", C.c_double), ("max_step", C.c_double),
+                ("max_slope", C.c_double), ("max_roughness", C.c_double), ("min_points", C.c_uint), ("min_fit", C.c_uint),
+                ("static_only", C.c_int), ("combine_occupancy", C.c_int)]
+
+
+class TerrainInfo(C.Structure):
+    """tloam_terrain_info: the grid, the radii in cells, the rows' counts, the known and lethal cells"""
+    _fields_ = [("origin_x", C.c_double), ("origin_y", C.c_double), ("resolution", C.c_double), ("width", C.c_size_t),
+                ("height", C.c_size_t), ("ground_cells", C.c_uint), ("step_cells", C.c_uint), ("slope_cells", C.c_uint),
+                ("rows", C.c_size_t), ("used", C.c_size_t), ("skipped", C.c_size_t), ("dropped", C.c_size_t),
+                ("overhang", C.c_size_t), ("known", C.c_size_t), ("lethal", C.c_size_t), ("combined", C.c_int)]
+
+
 class PoseGraphConfig(C.Structure):
     """tloam_pose_graph_config (include/tloam_b200.h "Pose graph"): the edges' sigmas and the Gauss-Newton schedule."""
     _fields_ = [("sigma_odom_translation", C.c_double), ("sigma_odom_rotation", C.c_double),
@@ -378,6 +394,8 @@ EXPORTS = [
     "tloam_b200_plan_path_cells",
     "tloam_b200_frontier_default_config", "tloam_b200_frontier_search", "tloam_b200_frontier_download",
     "tloam_b200_frontier_cells", "tloam_b200_frontier_labels",
+    "tloam_b200_terrain_default_config", "tloam_b200_terrain_build", "tloam_b200_terrain_build_cloud",
+    "tloam_b200_terrain_download", "tloam_b200_distance_build_terrain",
     "tloam_b200_global_registration_default_config", "tloam_b200_global_registration_enable", "tloam_b200_global_register",
     "tloam_b200_global_register_loop", "tloam_b200_global_registration_side", "tloam_b200_global_registration_correspondences",
     "tloam_b200_global_registration_hypotheses",
@@ -641,6 +659,12 @@ def load():
     L.tloam_b200_frontier_download.argtypes = [vp, C.POINTER(FrontierRecord), C.c_size_t]
     L.tloam_b200_frontier_cells.argtypes = [vp, C.POINTER(C.c_size_t), C.POINTER(C.c_int), dp, C.c_size_t]
     L.tloam_b200_frontier_labels.argtypes = [vp, C.POINTER(C.c_uint), C.c_size_t]
+    L.tloam_b200_terrain_default_config.argtypes = [C.POINTER(TerrainConfig)]
+    L.tloam_b200_terrain_default_config.restype = None
+    L.tloam_b200_terrain_build.argtypes = [vp, C.POINTER(TerrainConfig), C.POINTER(TerrainInfo)]
+    L.tloam_b200_terrain_build_cloud.argtypes = [vp, C.POINTER(TerrainConfig), dp, C.c_size_t, C.POINTER(TerrainInfo)]
+    L.tloam_b200_terrain_download.argtypes = [vp, C.POINTER(C.c_byte), dp, dp, dp, dp, dp, C.POINTER(C.c_uint), C.c_size_t]
+    L.tloam_b200_distance_build_terrain.argtypes = [vp, C.POINTER(DistanceConfig), C.POINTER(DistanceInfo)]
     L.tloam_b200_global_registration_default_config.argtypes = [C.POINTER(GlobalRegistrationConfig)]
     L.tloam_b200_global_registration_default_config.restype = None
     L.tloam_b200_global_registration_enable.argtypes = [vp, C.POINTER(GlobalRegistrationConfig)]

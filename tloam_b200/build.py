@@ -1,8 +1,8 @@
 """In-tree build of libtloam_b200.so, libtloam_b200_gmi.so, libtloam_b200_unpack.so, libtloam_b200_deskew.so,
 libtloam_b200_loop.so, libtloam_b200_loopv.so, libtloam_b200_pg.so, libtloam_b200_gmc.so, libtloam_b200_pgr.so,
 libtloam_b200_loopvs.so, libtloam_b200_gmd.so, libtloam_b200_gmm.so, libtloam_b200_loc.so, libtloam_b200_reloc.so,
-libtloam_b200_mapu.so, libtloam_b200_occ.so, libtloam_b200_dist.so, libtloam_b200_plan.so, libtloam_b200_greg.so and
-libtloam_b200_frontier.so (hand-written CUDA for sm_90a; no torch, no CPU fallback).
+libtloam_b200_mapu.so, libtloam_b200_occ.so, libtloam_b200_dist.so, libtloam_b200_plan.so, libtloam_b200_greg.so,
+libtloam_b200_frontier.so and libtloam_b200_terrain.so (hand-written CUDA for sm_90a; no torch, no CPU fallback).
 
     python -m tloam_b200.build [--force]
 
@@ -19,7 +19,7 @@ prior map (csrc/relocalize.cu), libtloam_b200_mapu.so the update of a prior map 
 map (csrc/occupancy.cu), libtloam_b200_dist.so the distance field and costmap of an occupancy grid (csrc/distance.cu),
 libtloam_b200_plan.so the path planning on that costmap (csrc/plan.cu), libtloam_b200_greg.so the global registration
 of two clouds (csrc/global_registration.cu), libtloam_b200_frontier.so the exploration frontiers of the costmap
-(csrc/frontier.cu); libtloam_b200.so loads each from its own directory when first needed.
+(csrc/frontier.cu), libtloam_b200_terrain.so the terrain map of a cloud (csrc/terrain.cu); libtloam_b200.so loads each from its own directory when first needed.
 """
 import os
 import subprocess
@@ -67,6 +67,8 @@ GREG_LIB = os.path.join(HERE, "libtloam_b200_greg.so")
 GREG_SOURCES = [os.path.join(CSRC, "global_registration.cu")]
 FRONTIER_LIB = os.path.join(HERE, "libtloam_b200_frontier.so")
 FRONTIER_SOURCES = [os.path.join(CSRC, "frontier.cu")]
+TERRAIN_LIB = os.path.join(HERE, "libtloam_b200_terrain.so")
+TERRAIN_SOURCES = [os.path.join(CSRC, "terrain.cu")]
 import glob
 # every header the translation unit can include: editing any of them triggers a rebuild
 HEADERS = sorted(glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(CSRC, "*.h")) +
@@ -98,13 +100,14 @@ def _nvcc(lib, sources, verbose, extra):
 
 
 def build(force=False, verbose=False, extra=()):
-    """builds the twenty libraries (each only when out of date); returns the path of libtloam_b200.so"""
+    """builds the twenty-one libraries (each only when out of date); returns the path of libtloam_b200.so"""
     for lib, sources in ((LIB, SOURCES), (GMI_LIB, GMI_SOURCES), (UNPACK_LIB, UNPACK_SOURCES), (DESKEW_LIB, DESKEW_SOURCES),
                          (LOOP_LIB, LOOP_SOURCES), (LOOPV_LIB, LOOPV_SOURCES), (PG_LIB, PG_SOURCES), (GMC_LIB, GMC_SOURCES),
                          (PGR_LIB, PGR_SOURCES), (LOOPVS_LIB, LOOPVS_SOURCES), (GMD_LIB, GMD_SOURCES),
                          (GMM_LIB, GMM_SOURCES), (LOC_LIB, LOC_SOURCES), (RELOC_LIB, RELOC_SOURCES),
                          (MAPU_LIB, MAPU_SOURCES), (OCC_LIB, OCC_SOURCES), (DIST_LIB, DIST_SOURCES),
-                         (PLAN_LIB, PLAN_SOURCES), (GREG_LIB, GREG_SOURCES), (FRONTIER_LIB, FRONTIER_SOURCES)):
+                         (PLAN_LIB, PLAN_SOURCES), (GREG_LIB, GREG_SOURCES), (FRONTIER_LIB, FRONTIER_SOURCES),
+                         (TERRAIN_LIB, TERRAIN_SOURCES)):
         if force or needs_build(lib, sources):
             _nvcc(lib, sources, verbose, extra)
     return LIB

@@ -45,6 +45,7 @@
 #include "plan.h"
 #include "global_registration.h"
 #include "frontier.h"
+#include "terrain.h"
 
 
 
@@ -281,6 +282,13 @@ struct tloam_b200_handle {
   unsigned char* d_fr_sort = nullptr;      size_t cap_fr_sort = 0;                             // frontier cells of it
   bool fr_kept = false;                    tloam_frontier_info fr_info;
   std::vector<tloam_frontier> fr_ranked;   unsigned fr_sorted = 0;                             // row buffer of the cells
+  // ---- the terrain (tloam_b200_terrain*, libtloam_b200_terrain.so): the last build's cells (65 B each: four encodings,
+  //      three layers, two counts, the value), the host cloud's rows (24 B each) and the state; allocated by the first
+  //      build that needs them, grown only ----
+  unsigned char* d_ter = nullptr;          size_t cap_ter = 0;                                 // cells of the buffer
+  double* d_ter_cloud = nullptr;           size_t cap_ter_cloud = 0;                           // rows of the buffer
+  tloam_ter_state* d_ter_state = nullptr;
+  bool ter_built = false;                  tloam_terrain_info ter_info;
   // ---- the merged map (tloam_b200_global_map_merge*, libtloam_b200_gmm.so): the radix sort's scratch (24 B per map row)
   //      and the last merge's voxels (32 B each), allocated by the first merge and grown; the snapshot is dropped by
   //      enable / reset and by the next merge ----
@@ -609,6 +617,7 @@ int tloam_b200_destroy(tloam_b200_handle* h) {
   cudaFree(h->d_dist); cudaFree(h->d_dist_bands); cudaFree(h->d_dist_table); cudaFree(h->d_dist_small); cudaFree(h->d_dist_q);
   cudaFree(h->d_plan); cudaFree(h->d_plan_tiles); cudaFree(h->d_plan_state); cudaFree(h->d_plan_q); cudaFree(h->d_plan_cells);
   cudaFree(h->d_fr_labels); cudaFree(h->d_fr_tiles); cudaFree(h->d_fr_small); cudaFree(h->d_fr_sort);
+  cudaFree(h->d_ter); cudaFree(h->d_ter_cloud); cudaFree(h->d_ter_state);
   cudaFree(h->d_gmm_scratch); cudaFree(h->d_gmm_out);
   cudaFree(h->d_loc_map); cudaFree(h->d_loc_scratch); cudaFree(h->d_loc_qst); cudaFree(h->d_loc_reg); cudaFree(h->d_loc_fin);
   cudaFree(h->d_loc_q); cudaFree(h->d_loc_in); cudaFree(h->d_loc_run);
@@ -6218,6 +6227,221 @@ int tloam_b200_frontier_labels(tloam_b200_handle* h, unsigned* labels, size_t ca
   if (labels) CU_TRY(cudaMemcpyAsync(labels, h->d_fr_labels, n * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
   CU_TRY(cudaStreamSynchronize(h->stream));
   return TLOAM_B200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Terrain (the checks, the grid's geometry and the buffers here; the kernels in terrain.cu, loaded from
+// libtloam_b200_terrain.so by the first terrain call, so that the kernels of this library keep their SASS).
+// ---------------------------------------------------------------------------------------------
+struct TerrainLib { tloam_ter_fn bounds = nullptr; tloam_ter_fn build = nullptr; };
+static std::mutex g_ter_mu;
+static TerrainLib g_ter;
+
+static int ter_load(tloam_b200_handle* h, TerrainLib* out) {
+  std::lock_guard<std::mutex> lk(g_ter_mu);
+  if (!g_ter.bounds) {
+    const std::string path = sibling_path("libtloam_b200_terrain.so");
+    void* so = dlopen(path.c_str(), RTLD_NOW | RTLD_LOCAL);
+    TerrainLib l;
+    if (so) {
+      l.bounds = reinterpret_cast<tloam_ter_fn>(dlsym(so, "tloam_ter_bounds"));
+      l.build = reinterpret_cast<tloam_ter_fn>(dlsym(so, "tloam_ter_build"));
+    }
+    if (!l.bounds || !l.build) {
+      const char* why = dlerror();
+      snprintf(h->last_error, sizeof(h->last_error), "terrain: cannot load %s: %s", path.c_str(), why ? why : "missing symbol");
+      if (so) dlclose(so);
+      return TLOAM_B200_ERR_CUDA;
+    }
+    g_ter = l;
+  }
+  *out = g_ter;
+  return TLOAM_B200_OK;
+}
+
+static int ter_status(tloam_b200_handle* h, int e, const char* where) {
+  if (e == cudaSuccess) return TLOAM_B200_OK;
+  snprintf(h->last_error, sizeof(h->last_error), "terrain: %s: %s", where, cudaGetErrorString((cudaError_t)e));
+  return TLOAM_B200_ERR_CUDA;
+}
+
+void tloam_b200_terrain_default_config(tloam_terrain_config* c) {
+  c->resolution = 0.2;                     // a car with an HDL-64E; robot parameters, not calibrated
+  c->clearance = 2.0;
+  c->ground_radius = 1.6; c->step_radius = 0.3; c->slope_radius = 0.4;
+  c->max_step = 0.10; c->max_slope = 15.0 * M_PI / 180.0; c->max_roughness = 0.10;
+  c->min_points = 1; c->min_fit = 6;
+  c->static_only = 0; c->combine_occupancy = 0;
+}
+
+static bool ter_config_valid(const tloam_terrain_config* c) {
+  const auto ok = [](double v) { return std::isfinite(v) && v >= 0.0; };
+  return std::isfinite(c->resolution) && c->resolution > 0.0 && ok(c->clearance) && ok(c->ground_radius) &&
+         ok(c->step_radius) && ok(c->slope_radius) && ok(c->max_step) && ok(c->max_slope) && c->max_slope < M_PI / 2 &&
+         ok(c->max_roughness) && c->min_points >= 1 && c->min_fit >= 1;
+}
+
+// the radius in cells, false past `limit`
+static bool ter_cells(double radius, double resolution, unsigned limit, unsigned* r) {
+  const double v = std::ceil(radius / resolution);
+  if (!(v <= (double)limit)) return false;
+  *r = (unsigned)v;
+  return true;
+}
+
+// the build over `count` rows at `rows` (device), the selection's counters or null; cfg checked
+static int ter_run(tloam_b200_handle* h, const tloam_terrain_config* cfg, const double* rows, size_t count,
+                   const unsigned* through, const unsigned* hits, tloam_terrain_info* info) {
+  const bool combine = cfg->combine_occupancy != 0;
+  const double res = combine ? h->occ_info.resolution : cfg->resolution;
+  tloam_ter_args a;
+  memset(&a, 0, sizeof(a));
+  if (!ter_cells(cfg->ground_radius, res, 1024, &a.rg) || !ter_cells(cfg->step_radius, res, TLOAM_TER_HALO_MAX, &a.rs) ||
+      !ter_cells(cfg->slope_radius, res, TLOAM_TER_HALO_MAX, &a.rp))
+    return TLOAM_B200_ERR_INVALID_ARG;
+  TerrainLib lib;
+  int rc = ter_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaSetDevice(h->device));
+  if (!h->d_ter_state) CU_TRY(cudaMalloc(&h->d_ter_state, sizeof(tloam_ter_state)));
+  a.rows = rows; a.count = count;
+  if (through) { a.through = through; a.hits = hits; a.min_through = (unsigned)h->gmd_cfg.min_through; }
+  a.resolution = res;
+  a.state = h->d_ter_state;
+  a.device = h->device; a.stream = h->stream;
+  int e = 0, launches = 0;
+  tloam_ter_state st;
+  if (combine) {
+    a.origin_x = h->occ_info.origin_x; a.origin_y = h->occ_info.origin_y;
+    a.width = (unsigned)h->occ_info.width; a.height = (unsigned)h->occ_info.height;
+    a.occupancy = reinterpret_cast<const signed char*>(reinterpret_cast<const unsigned*>(h->d_occ_grid) + 2 * h->cap_occ_grid);
+  } else {
+    TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.bounds(&a, &launches)));
+    if ((rc = ter_status(h, e, "k_ter_bounds")) != TLOAM_B200_OK) return rc;
+    CU_TRY(cudaMemcpyAsync(&st, a.state, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    if (st.hi[0]) {                        // origin = res floor(min / res), width = floor((max - origin) / res) + 1
+      const double ox = res * std::floor(dec_ordered(~st.lo[0]) / res), oy = res * std::floor(dec_ordered(~st.lo[1]) / res);
+      const double fw = std::floor((dec_ordered(st.hi[0]) - ox) / res) + 1.0;
+      const double fh = std::floor((dec_ordered(st.hi[1]) - oy) / res) + 1.0;
+      if (!(fw <= (double)(1u << 28)) || !(fh <= (double)(1u << 28)) || !(fw * fh <= (double)(1u << 28)))
+        return TLOAM_B200_ERR_VOXEL_RANGE;
+      a.origin_x = ox; a.origin_y = oy;
+      a.width = (unsigned)fw; a.height = (unsigned)fh;
+    }
+  }
+  // from here on the last build is replaced
+  h->ter_built = false;
+  const size_t n = (size_t)a.width * a.height;
+  if (n > h->cap_ter) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_ter); h->d_ter = nullptr; h->cap_ter = 0;
+    CU_TRY(cudaMalloc(&h->d_ter, n * 65));
+    h->cap_ter = n;
+  }
+  const size_t cap = h->cap_ter;
+  unsigned char* b = h->d_ter;
+  a.lo = reinterpret_cast<unsigned long long*>(b);
+  a.gx = a.lo + cap; a.g = a.gx + cap; a.e = a.g + cap;
+  a.step = reinterpret_cast<double*>(a.e + cap); a.slope = a.step + cap; a.roughness = a.slope + cap;
+  a.n = reinterpret_cast<unsigned*>(a.roughness + cap); a.m = a.n + cap;
+  a.values = reinterpret_cast<signed char*>(a.m + cap);
+  a.clearance = cfg->clearance; a.max_step = cfg->max_step; a.max_roughness = cfg->max_roughness;
+  a.tan_max_slope = std::tan(cfg->max_slope);
+  a.min_points = cfg->min_points; a.min_fit = cfg->min_fit;
+  TL_LAUNCH(TLOAM_B200_K_SUBMAP, (e = lib.build(&a, &launches)));
+  h->launches += launches > 0 ? launches - 1 : 0;
+  if ((rc = ter_status(h, e, "k_ter_low / _ground / _high / _layers")) != TLOAM_B200_OK) return rc;
+  CU_TRY(cudaMemcpyAsync(&st, a.state, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  tloam_terrain_info out;
+  memset(&out, 0, sizeof(out));
+  out.origin_x = a.origin_x; out.origin_y = a.origin_y; out.resolution = res;
+  out.width = a.width; out.height = a.height;
+  out.ground_cells = a.rg; out.step_cells = a.rs; out.slope_cells = a.rp;
+  out.used = st.used; out.skipped = st.skipped; out.overhang = st.overhang;
+  out.dropped = st.dropped;
+  out.known = st.known; out.lethal = st.lethal;
+  out.combined = combine ? 1 : 0;
+  out.rows = out.used + out.skipped + out.dropped;
+  h->ter_info = out;
+  h->ter_built = true;
+  if (info) *info = out;
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_terrain_build(tloam_b200_handle* h, const tloam_terrain_config* cfg, tloam_terrain_info* info) {
+  if (!h || !cfg || !ter_config_valid(cfg)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->gmap_on || (cfg->static_only && !h->gmd_on)) return TLOAM_B200_ERR_NOT_READY;
+  if (cfg->combine_occupancy && (!h->occ_on || !h->occ_built)) return TLOAM_B200_ERR_NOT_READY;
+  GMapState st;
+  int rc = gmc_read(h, &st);               // the sticky flags stay for the next size / download call
+  if (rc != TLOAM_B200_OK) return rc;
+  return ter_run(h, cfg, h->d_gmap, st.count, cfg->static_only ? h->d_gmd_through : nullptr,
+                 cfg->static_only ? h->d_gmd_hits : nullptr, info);
+}
+
+int tloam_b200_terrain_build_cloud(tloam_b200_handle* h, const tloam_terrain_config* cfg, const double* xyz, size_t n,
+                                   tloam_terrain_info* info) {
+  if (!h || !cfg || !ter_config_valid(cfg) || cfg->static_only || (n && !xyz)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (cfg->combine_occupancy && (!h->gmap_on || !h->occ_on || !h->occ_built)) return TLOAM_B200_ERR_NOT_READY;
+  CU_TRY(cudaSetDevice(h->device));
+  if (n > h->cap_ter_cloud) {
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    cudaFree(h->d_ter_cloud); h->d_ter_cloud = nullptr; h->cap_ter_cloud = 0;
+    CU_TRY(cudaMalloc(&h->d_ter_cloud, n * 3 * sizeof(double)));
+    h->cap_ter_cloud = n;
+  }
+  if (n) CU_TRY(cudaMemcpyAsync(h->d_ter_cloud, xyz, n * 3 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  return ter_run(h, cfg, h->d_ter_cloud, n, nullptr, nullptr, info);
+}
+
+int tloam_b200_terrain_download(tloam_b200_handle* h, signed char* values, double* ground, double* elevation, double* step,
+                                double* slope, double* roughness, unsigned* points, size_t capacity) {
+  if (!h) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->ter_built) return TLOAM_B200_ERR_NOT_READY;
+  const size_t n = h->ter_info.width * h->ter_info.height;
+  if (capacity < n) return TLOAM_B200_ERR_INVALID_ARG;
+  CU_TRY(cudaSetDevice(h->device));
+  if (n) {
+    const size_t cap = h->cap_ter;
+    const unsigned long long* g = reinterpret_cast<const unsigned long long*>(h->d_ter) + 2 * cap;
+    const unsigned long long* e = g + cap;
+    const double* st = reinterpret_cast<const double*>(e + cap);
+    const unsigned* m = reinterpret_cast<const unsigned*>(st + 3 * cap) + cap;
+    const signed char* v = reinterpret_cast<const signed char*>(m + cap);
+    if (values) CU_TRY(cudaMemcpyAsync(values, v, n, cudaMemcpyDeviceToHost, h->stream));
+    if (step) CU_TRY(cudaMemcpyAsync(step, st, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    if (slope) CU_TRY(cudaMemcpyAsync(slope, st + cap, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    if (roughness) CU_TRY(cudaMemcpyAsync(roughness, st + 2 * cap, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    std::vector<unsigned> mm(n);
+    std::vector<unsigned long long> gk(ground ? n : 0), ek(elevation ? n : 0);
+    CU_TRY(cudaMemcpyAsync(mm.data(), m, n * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+    if (ground) CU_TRY(cudaMemcpyAsync(gk.data(), g, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+    if (elevation) CU_TRY(cudaMemcpyAsync(ek.data(), e, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(cudaStreamSynchronize(h->stream));
+    for (size_t c = 0; c < n; ++c) {      // the encodings decoded: G +inf without a row, e NaN without a ground-side row
+      if (ground) ground[c] = gk[c] ? dec_ordered(~gk[c]) : HUGE_VAL;
+      if (elevation) elevation[c] = mm[c] ? dec_ordered(ek[c]) : std::nan("");
+    }
+    if (points) std::copy(mm.begin(), mm.end(), points);
+  }
+  CU_TRY(cudaStreamSynchronize(h->stream));
+  return TLOAM_B200_OK;
+}
+
+int tloam_b200_distance_build_terrain(tloam_b200_handle* h, const tloam_distance_config* cfg, tloam_distance_info* info) {
+  if (!h || !cfg || !dist_config_valid(cfg)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!h->ter_built) return TLOAM_B200_ERR_NOT_READY;
+  const tloam_terrain_info& g = h->ter_info;
+  unsigned r2 = 0;
+  if (!dist_r2(cfg, g.resolution, &r2)) return TLOAM_B200_ERR_INVALID_ARG;
+  if (!dist_shape_ok(g.width, g.height)) return TLOAM_B200_ERR_VOXEL_RANGE;
+  DistLib lib;
+  int rc = dist_load(h, &lib);
+  if (rc != TLOAM_B200_OK) return rc;
+  const signed char* values = reinterpret_cast<const signed char*>(h->d_ter + 64 * h->cap_ter);
+  return dist_run(h, lib, cfg, values, false, g.width, g.height, g.origin_x, g.origin_y, g.resolution, r2, info);
 }
 
 // ---------------------------------------------------------------------------------------------

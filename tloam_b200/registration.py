@@ -280,6 +280,27 @@ class Frontier:
 
 
 @dataclasses.dataclass(frozen=True)
+class TerrainMap:
+    """a built terrain map (include/tloam_b200.h "Terrain"), each layer (height, width) in the grid's layout: values (int8:
+    100 lethal, 0 traversable, -1 not known; combined with the occupancy grid's when combined), ground G (+inf without a
+    row in its window), elevation e (NaN without a ground-side row), step, slope (m per m) and roughness (NaN where not
+    known or not defined), points m (ground-side rows); origin = (x, y) of the corner of cell (0, 0); radii = (rg, rs, rp)
+    in cells; info = tloam_terrain_info's counts."""
+    values: np.ndarray
+    ground: np.ndarray
+    elevation: np.ndarray
+    step: np.ndarray
+    slope: np.ndarray
+    roughness: np.ndarray
+    points: np.ndarray
+    origin: tuple
+    resolution: float
+    radii: tuple
+    combined: bool
+    info: dict
+
+
+@dataclasses.dataclass(frozen=True)
 class OccupancyGrid:
     """a built occupancy grid (include/tloam_b200.h "Occupancy grid"): cells (height, width) int8 in nav_msgs/OccupancyGrid's
     values (-1 unknown, 0 .. 100), row j along y and column i along x, with the counts it came from (uint32 each); origin
@@ -1611,6 +1632,20 @@ class LocalRegistration:
         """the distance field and costmap of the last occupancy_build (grid None), or of a host grid: (height, width) int8
         in nav_msgs/OccupancyGrid's values with its origin (x, y) and resolution; overrides: fields of
         tloam_distance_config (inscribed_radius, inflation_radius, cost_scaling_factor).  Returns a DistanceField."""
+        def build(cfg, info):
+            if grid is None:
+                self._check(self._L.tloam_b200_distance_build(self._h, C.byref(cfg), C.byref(info)), "distance_build")
+                return
+            g = np.ascontiguousarray(grid, dtype=np.int8)
+            if g.ndim != 2 or origin is None or resolution is None:
+                raise RegistrationError(_lib.ERR_INVALID_ARG, "distance_build_grid")
+            self._check(self._L.tloam_b200_distance_build_grid(
+                self._h, C.byref(cfg), g.ctypes.data_as(C.POINTER(C.c_byte)), g.shape[1], g.shape[0], float(origin[0]),
+                float(origin[1]), float(resolution), C.byref(info)), "distance_build_grid")
+        return self._distance_field(build, overrides)
+
+    def _distance_field(self, build, overrides):
+        """the distance config with the overrides, build(cfg, info) (a checked C call), then the field's download"""
         cfg = _lib.DistanceConfig()
         self._L.tloam_b200_distance_default_config(C.byref(cfg))
         for k, v in overrides.items():
@@ -1618,15 +1653,7 @@ class LocalRegistration:
                 raise TypeError(f"unknown distance field {k!r}")
             setattr(cfg, k, v)
         info = _lib.DistanceInfo()
-        if grid is None:
-            self._check(self._L.tloam_b200_distance_build(self._h, C.byref(cfg), C.byref(info)), "distance_build")
-        else:
-            g = np.ascontiguousarray(grid, dtype=np.int8)
-            if g.ndim != 2 or origin is None or resolution is None:
-                raise RegistrationError(_lib.ERR_INVALID_ARG, "distance_build_grid")
-            self._check(self._L.tloam_b200_distance_build_grid(
-                self._h, C.byref(cfg), g.ctypes.data_as(C.POINTER(C.c_byte)), g.shape[1], g.shape[0], float(origin[0]),
-                float(origin[1]), float(resolution), C.byref(info)), "distance_build_grid")
+        build(cfg, info)
         shape = (info.height, info.width)
         sd, sq = np.zeros(shape, dtype=np.float32), np.zeros(shape, dtype=np.uint32)
         costs, values = np.zeros(shape, dtype=np.uint8), np.zeros(shape, dtype=np.int8)
@@ -1635,6 +1662,40 @@ class LocalRegistration:
             costs.ctypes.data_as(C.POINTER(C.c_ubyte)), values.ctypes.data_as(C.POINTER(C.c_byte)), sd.size),
             "distance_download")
         return DistanceField(sd, sq, costs, values, (info.origin_x, info.origin_y), info.resolution, info.obstacles)
+
+    # ---- terrain (include/tloam_b200.h "Terrain") ----
+    def terrain_build(self, cloud=None, **overrides):
+        """the terrain map of the global map (cloud None) or of a host cloud (n, 3); overrides: fields of
+        tloam_terrain_config (resolution, clearance, ground_radius, step_radius, slope_radius, max_step, max_slope in
+        radians, max_roughness, min_points, min_fit, static_only, combine_occupancy).  Returns a TerrainMap."""
+        cfg = _lib.TerrainConfig()
+        self._L.tloam_b200_terrain_default_config(C.byref(cfg))
+        for k, v in overrides.items():
+            if not any(f[0] == k for f in cfg._fields_):
+                raise TypeError(f"unknown terrain field {k!r}")
+            setattr(cfg, k, v)
+        info = _lib.TerrainInfo()
+        if cloud is None:
+            self._check(self._L.tloam_b200_terrain_build(self._h, C.byref(cfg), C.byref(info)), "terrain_build")
+        else:
+            c = _f64(cloud).reshape(-1, 3)
+            self._check(self._L.tloam_b200_terrain_build_cloud(self._h, C.byref(cfg), _dp(c), c.shape[0], C.byref(info)),
+                        "terrain_build_cloud")
+        shape = (info.height, info.width)
+        values, points = np.zeros(shape, dtype=np.int8), np.zeros(shape, dtype=np.uint32)
+        layers = [np.zeros(shape) for _ in range(5)]
+        self._check(self._L.tloam_b200_terrain_download(self._h, values.ctypes.data_as(C.POINTER(C.c_byte)),
+                                                        *[_dp(a) for a in layers], points.ctypes.data_as(C.POINTER(C.c_uint)),
+                                                        values.size), "terrain_download")
+        return TerrainMap(values, *layers, points, (info.origin_x, info.origin_y), info.resolution,
+                          (info.ground_cells, info.step_cells, info.slope_cells), bool(info.combined),
+                          {name: getattr(info, name) for name, _ in info._fields_})
+
+    def distance_build_terrain(self, **overrides):
+        """the distance field and costmap of the last terrain_build's values; overrides: fields of tloam_distance_config.
+        Returns a DistanceField."""
+        return self._distance_field(lambda cfg, info: self._check(self._L.tloam_b200_distance_build_terrain(
+            self._h, C.byref(cfg), C.byref(info)), "distance_build_terrain"), overrides)
 
     def distance_query(self, xy):
         """(distance (n,), gradient (n, 2)) of the last distance_build at the points xy (n, 2): sd interpolated bilinearly
